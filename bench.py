@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- depth-maps/s of the PatchmatchNet cascade with the B200-native PatchMatch hot path.
+"""bench.py -- depth-maps/s of the PatchmatchNet cascade with the H100-native PatchMatch hot path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo (one JSON line on rank 0)
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]   # this repo (one JSON line on rank 0)
     python bench.py --impl reference [--steps K] [--warmup W]      # the reference algorithm on the host CPU
 
 Workload (BASELINE.json configs[1]): 1 reference + 4 source views, 640x512, full 3-stage cascade with
@@ -9,16 +9,20 @@ Workload (BASELINE.json configs[1]): 1 reference + 4 source views, 640x512, full
 no collective on the data path).  A "step" is one full forward over one batch of synthetic input.
 
 Numbers on the JSON line
-    value      depth-maps/s, inputs resident in HBM, forward replayed from a CUDA graph, L2 flushed
-               between timed steps, device time by CUDA events, max over ranks
+    value      depth-maps/s over exactly K timed steps, inputs resident in HBM, forward replayed from a CUDA graph,
+               L2 flushed between timed rounds, device time by CUDA events, max over ranks
     e2e        same metric through the public API (DepthEngine.infer_stream): pinned HOST inputs copied
                to the device and results copied back inside the timed region, every step
     roofline   the dominant hand-written kernel (fused warp+correlation, all source views per launch):
                algorithmic bytes per launch / CUDA-event duration of that launch, against the measured
-               HBM copy bandwidth in MEASURED_PEAKS.json
+               HBM copy bandwidth in MEASURED_PEAKS.json (else the H100 SXM data sheet's 3.35 TB/s)
     cpu_baseline  the oracle (CPU restatement of the reference, bit-identical to it) timed on the host
     gpu_eager_reference  the same oracle in eager PyTorch on the GPU, issuing the reference's own op sequence
-               (what the unmodified reference would do on this B200; SURVEY.md 8d "honest bar")
+               (what the unmodified reference would do on this GPU; SURVEY.md 8d "honest bar")
+
+--dump-outputs DIR writes what the timed path returned in its last timed step (depth [B,1,H,W] and confidence
+[B,H,W] of the flagship workload, float32) as DIR/depth.npy and DIR/confidence.npy.  Inputs are seeded and the
+weights are the committed fixture, so two builds given the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -674,13 +678,6 @@ def ka_roofline(net, wl, peak_gbs, peak_src, flush, steps):
     alg_mean = sum(r["algorithmic_bytes"] for r in detail) / n_l
     us_mean = sum(r["us"] for r in detail) / n_l
     traffic, traffic_src = None, None
-    tfile = os.path.join(REPO, "profiles", TRAFFIC_FILE)
-    if os.path.exists(tfile):
-        try:
-            t = json.load(open(tfile))
-            traffic, traffic_src = t.get("mean_dram_bytes_per_launch"), f"profiles/{TRAFFIC_FILE} ({t.get('capture', 'ncu --set full')})"
-        except Exception:  # noqa: BLE001
-            traffic = None
     achieved = alg_mean / (us_mean * 1e-6) / 1e9
     roofline = {"bound": "hbm", "kernel": f"fused warp + bilinear gather + group correlation + view aggregation + head (K-A), {n_l} launches per step",
                 "achieved": achieved, "peak": peak_gbs, "unit": "GB/s", "frac": achieved / peak_gbs, "traffic": traffic,
@@ -693,7 +690,18 @@ def ka_roofline(net, wl, peak_gbs, peak_src, flush, steps):
     return roofline, detail
 
 
-TRAFFIC_FILE = "r2_warp_corr_traffic.json"  # written from this round's ncu --set full capture (tools/summarize_ncu.py)
+def dump_outputs(eng, slot_idx: int, out_dir: str) -> None:
+    """The depth and confidence maps the timed path returned in its last step (slot `slot_idx` ran it), as float32 .npy."""
+    import numpy as np
+
+    torch.cuda.synchronize()
+    outs = eng._slots[slot_idx]["outs"]
+    if outs is None:  # --no-graph: the forward keeps no static outputs; the slot's inputs are unchanged, so run it again
+        outs = eng.run_slot(slot_idx)
+        torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in zip(("depth", "confidence"), outs):
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
 
 
 def main() -> None:
@@ -714,7 +722,9 @@ def main() -> None:
     ap.add_argument("--no-tf32", action="store_true", help="accepted for compatibility: fp32-accurate convolutions are the default")
     ap.add_argument("--slots", type=int, default=3, help="independent requests in flight per GPU (each its own stream + CUDA graph)")
     ap.add_argument("--cpu-samples", type=int, default=4)
-    ap.add_argument("--repeats", type=int, default=5, help="the K-step timed region is repeated this many times; the line reports the median")
+    ap.add_argument("--repeats", type=int, default=1, help="the K-step timed region is repeated this many times; the line reports the median")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the depth and confidence maps of the last timed step to DIR/<name>.npy (float32)")
     ap.add_argument("--no-sub", action="store_true", help="skip the fp32 / 1600x1184 / batch-8 sub-records (N=1 only)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
@@ -727,7 +737,7 @@ def main() -> None:
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 path has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py: no CUDA device; the H100 path has no CPU fallback (use --impl reference for the CPU arm)")
     numa = bind_to_gpu_numa_node(local)  # before any pinned allocation
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
@@ -756,7 +766,7 @@ def main() -> None:
     forwards_counted = eng.n_slots * (eng._warmup + (1 if eng.use_graph else 0))
     launches_per_step = lc.n // max(1, forwards_counted)
 
-    flush_buf = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush_buf = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2 of an H100
 
     def flush():
         flush_buf.zero_()
@@ -790,6 +800,8 @@ def main() -> None:
     dev_runs = [time_resident(wl, args.steps, flush, stream, barrier) for _ in range(max(1, args.repeats))]
     sampler.mark_end()
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(eng, (args.steps - 1) % S, args.dump_outputs)
     dev_runs = reduce_max(dev_runs)  # per repeat: the slowest rank
     dev_seconds = statistics.median(dev_runs)
 
@@ -812,8 +824,8 @@ def main() -> None:
         peaks = json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json")))
     except Exception:  # noqa: BLE001
         pass
-    peak_gbs = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "MEASURED_PEAKS.json hbm_gbs (measured copy bandwidth)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    peak_gbs = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "MEASURED_PEAKS.json hbm_gbs (measured copy bandwidth)" if "hbm_gbs" in peaks else "fallback 3350 GB/s (H100 SXM data sheet)"
     roofline, detail, detail_cold, cpu_baseline, gpu_eager, latency, sub = None, None, None, None, None, None, {}
     detail_kb_kc = None
     if rank == 0:
@@ -838,8 +850,7 @@ def main() -> None:
                 runs = [time_resident(wl_t, args.steps, flush, stream, barrier) for _ in range(3)]
                 sub["value_tf32"] = {"value": args.steps * B / statistics.median(runs), "unit": UNIT,
                                      "ms_per_step": 1e3 * statistics.median(runs) / args.steps,
-                                     "parity": "OUTSIDE the bound: depth rel-L1 vs the fp32 oracle 2.6e-3 (cfg 2) / 3.3e-3 (cfg 3) / 3.1e-3 (B=8), "
-                                               "north_star allows 1e-3 (tests/test_gpu_bench_mode.py, profiles/r2_run1_bench_mode_parity.json)",
+                                     "parity": "OUTSIDE the bound: north_star allows 1e-3 depth rel-L1 vs the fp32 oracle (tests/test_gpu_bench_mode.py)",
                                      "how": "same workload, torch default cudnn.allow_tf32=True: native convs with TF32 operands on the memory-bound "
                                             "layers, cuDNN TF32 on the FLOP-bound ones; median of 3"}
                 del wl_t, net_t

@@ -1,5 +1,5 @@
 /*
- * patchmatch_b200.h -- C ABI of the B200-native (sm_100a) learned-PatchMatch hot path.
+ * patchmatch_b200.h -- C ABI of the H100-native (sm_90a) learned-PatchMatch hot path.
  *
  * This is the drop-in boundary: plain device pointers, sizes and a CUDA stream;
  * no torch types.  The reference (FangjinhuaWang/PatchmatchNet) has no native
@@ -54,13 +54,13 @@ const char *pmb200_last_error(void);
 int pmb200_set_tuning(const char *key, int value);
 
 /* ------------------------------------------------------------------------------------
- * K-D5: channels-last convolution on the 5th-generation tensor cores (tcgen05 / TMEM / TMA), fp32-accurate (3xTF32 split).
+ * K-D5: channels-last convolution on Hopper's warpgroup tensor cores (wgmma / TMA), fp32-accurate (3xTF32 split).
  * Replaces, for the FLOP-bound layers in the fp32-accurate mode, the nn.Conv2d calls of reference models/net.py:9-70 (FeatureNet
  * conv2..10), models/patchmatch.py:288-311 (stage-2/3 offset convs), models/net.py:73-122 (Refinement).
  *   x_nhwc      [N,H,W,Cin] fp32, 16-byte aligned, Cin in {8,16,32,64}
  *   filter_tc5  pmb200_conv2d_tc5_filter_floats(Cin,Cout,KS) floats: [tap ky*KS+kx][Cin/32 blocks (1 if Cin <= 32)]
  *               [2 Npad rows: w_hi rows then w_lo rows, Npad = Cout rounded up to 16][min(Cin,32) channels]; every
- *               [2 Npad][row bytes] tile is ONE K-major tcgen05 operand (its first Npad rows double as the N = Npad operand)
+ *               [2 Npad][row bytes] tile is ONE K-major wgmma operand (its first Npad rows double as the N = Npad operand)
  *               stored in the tensor core's shared-memory swizzle for that row size (16-byte chunk j of row r sits at chunk
  *               j ^ (r % 8) for 128-byte rows, j ^ ((r / 2) % 4) for 64-byte rows, j ^ ((r / 4) % 2) for 32-byte rows);
  *               w_hi = weight rounded to TF32, w_lo = (weight - w_hi) rounded to TF32; rows >= Cout of each half are zero
@@ -74,7 +74,7 @@ int pmb200_conv2d_tc5(const float *x_nhwc, const float *filter_tc5, const float 
                       void *stream);
 /* Stride-1 form of the same convolution (K-D5h): the input halo of an 8 x 16 output tile is fetched ONCE (one dense TMA box),
  * split once into channel-chunk planes [Cin/4][rows][cols][4 floats]; every filter tap is a shifted view of them (no-swizzle
- * K-major tcgen05 operand: 8 consecutive pixels of a plane are one core matrix).  Same arguments minus the stride.
+ * K-major wgmma operand: 8 consecutive pixels of a plane are one core matrix).  Same arguments minus the stride.
  *   filter_tc5h  same float count as filter_tc5, layout [tap][Cin/4 chunks][w_hi rows Npad | w_lo rows Npad][4 floats] */
 int pmb200_conv2d_tc5h(const float *x_nhwc, const float *filter_tc5h, const float *bias, float *y_nhwc, int N, int H, int W, int Cin,
                        int Cout, int KS, int pad, int dil, int relu, int y_channel_stride, int y_channel_offset, void *stream);
@@ -167,7 +167,7 @@ int pmb200_upsample2x_add_nhwc(const float *x_nhwc, const float *y_nhwc, const f
  *                (models/net.py:60-66) fused into the lateral conv's epilogue (Ho, Wo, Cout even)
  *   y            [N,Ho,Wo,y_channel_stride], written at channels y_channel_offset .. +Cout (stride 0 = Cout: dense)
  *   precision    1: TF32 operands (the library's behaviour under torch.backends.cudnn.allow_tf32, torch's default:
- *                filter rounded by the host, activations truncated by the tensor core as for tcgen05 kind::tf32);
+ *                filter rounded by the host, activations truncated by the tensor core as for wgmma kind tf32);
  *                3: error-compensated 3xTF32, fp32-accurate
  *   rows_per_warp 0 = choose (tile = 16 columns x 4*rows_per_warp rows per 4-warp CTA); 1, 2 or 4 to force
  */

@@ -1,7 +1,7 @@
 """CPU restatement of the reference's geometric-consistency filtering (SURVEY.md 8f row f4).
 
 TEST INFRASTRUCTURE ONLY: nothing under patchmatchnet_b200/ imports this file; only tests/ and bench-side baselines
-may.  It follows, line by line, /root/reference/eval.py:
+may.  It follows, line by line, the reference's eval.py:
 
     reproject_with_depth          eval.py:86-146
     check_geometric_consistency   eval.py:149-190

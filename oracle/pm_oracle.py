@@ -16,11 +16,11 @@ bit-identical to the reference.
 
 Parity pin: the reference ships no tests or golden vectors ("parity unpinned"
 by the reference's own tests, SURVEY.md 8c).  The oracle is pinned instead
-against the UNMODIFIED reference imported from /root/reference in the build
-container (``tests/test_oracle_vs_reference.py``, max-abs diff == 0 on CPU) and
-against fixtures that script generated from the reference
-(``tests/golden/make_golden.py`` -> ``tests/golden/*.pt``), which travel to the
-GPU box where /root/reference does not exist.
+against what the UNMODIFIED reference computed on the same seeded inputs,
+recorded by ``tests/golden/make_golden.py`` and
+``tests/golden/make_reference_vectors.py`` into ``tests/golden/*.pt``
+(``tests/test_oracle_vs_reference.py``: max-abs diff == 0 on CPU;
+``tests/test_golden.py``).
 
 Every function cites the reference lines it restates.
 """

@@ -1,4 +1,4 @@
-"""patchmatchnet_b200 -- B200-native (sm_100a) learned-PatchMatch hot path of PatchmatchNet.
+"""patchmatchnet_b200 -- H100-native (sm_90a) learned-PatchMatch hot path of PatchmatchNet.
 
 Public surface (mirrors the reference's ``models`` package for this path):
 

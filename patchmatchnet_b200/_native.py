@@ -1,7 +1,7 @@
 """ctypes binding of the C ABI in ``include/patchmatch_b200.h`` (libpmb200.so).
 
 The library is built in-tree by ``build_library()`` (called from
-``__graft_entry__.build()``): a single ``nvcc -gencode arch=compute_100a,code=sm_100a``
+``__graft_entry__.build()``): a single ``nvcc -gencode arch=compute_90a,code=sm_90a``
 invocation, no torch headers.  There is NO fallback: if the shared object is
 missing or a call is made on a non-CUDA tensor the binding raises.
 """
@@ -25,7 +25,7 @@ HEADERS = [
     os.path.join(_REPO_DIR, "include", "patchmatch_b200.h"),
 ]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "--shared", "-Xcompiler", "-fPIC", "--threads", "0",
 ]
@@ -57,7 +57,7 @@ def needs_rebuild() -> bool:
 
 
 def build_library(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/*.cu for sm_100a into patchmatchnet_b200/libpmb200.so (in-tree)."""
+    """Compile csrc/*.cu for sm_90a into patchmatchnet_b200/libpmb200.so (in-tree)."""
     global _lib
     if not force and not needs_rebuild():
         return LIB_PATH
@@ -193,7 +193,7 @@ def lib() -> ctypes.CDLL:
         if not os.path.exists(LIB_PATH):
             raise NativeLibraryMissing(
                 f"{LIB_PATH} is missing -- run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(the B200 path has no CPU or PyTorch fallback)"
+                "(the H100 path has no CPU or PyTorch fallback)"
             )
         handle = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in _SIGNATURES.items():

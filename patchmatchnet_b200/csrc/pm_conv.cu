@@ -1,11 +1,11 @@
-// pm_conv.cu -- sm_100a channels-last 2-D convolution family for the small learned convs either side of the
+// pm_conv.cu -- sm_90a channels-last 2-D convolution family for the small learned convs either side of the
 // PatchMatch hot path: the offset convs ON the path (propa_conv / eval_conv, reference models/patchmatch.py:288-311),
 // the feature pyramid that produces the path's inputs (FeatureNet, reference models/net.py:9-70) and the refinement
 // head that consumes its output (Refinement, reference models/net.py:73-122).  SURVEY.md 8(f) rows f1 / f3.
 //
 // Why hand-written: these layers have 1..64 channels.  The library's implicit-GEMM kernels are tiled for hundreds of
-// channels (256x64x8 / 128x128x8 tiles) and ran the 23 convs of one 640x512 forward at ~28 TFLOP/s and far below HBM
-// speed (profiles/r1_run12_launches.md: 50 % of the device time of a forward).  At these widths a conv is a
+// channels (256x64x8 / 128x128x8 tiles) and run the 23 convs of one 640x512 forward far below HBM speed.  At these widths a
+// conv is a
 // memory-bound streaming op with a small dense contraction inside, so the design is:
 //
 //   * activations channels-last (NHWC) end to end -- the layout the fused PatchMatch kernels gather from;
@@ -19,18 +19,18 @@
 //     The filter is pre-arranged ON THE HOST in fragment order ([tap][k-slice][n-tile][lane]), so a warp fetches a B
 //     fragment with one coalesced read-only load that stays L1/L2-resident for every CTA of the layer: no shared
 //     memory for weights, no per-CTA weight staging; a 3x3 filter of <= 18 fragments lives in registers;
-//   * NO conversion instructions in the inner loop (profiles/r1_run17_conv_ncu.md: cvt.rna.tf32.f32 expands to an
-//     FSETP/IMAD sequence on sm_100 -- 38 issued instructions per MMA, XU pipe at 98-124 % -- in the first version).
+//   * NO conversion instructions in the inner loop (cvt.rna.tf32.f32 expands to a multi-instruction sequence that made
+//     the first version issue-bound).
 //     `precision == 1` (the library's behaviour under torch.backends.cudnn.allow_tf32 = True, torch's default): the
 //     host rounds the filter to TF32 (nearest, ties away) while packing, activations go to the tensor core as fp32
-//     bit patterns whose low 13 mantissa bits it ignores -- exactly what tcgen05 kind::tf32 does with the library's
+//     bit patterns whose low 13 mantissa bits it ignores -- exactly what wgmma kind tf32 does with the library's
 //     shared-memory operands.  `precision == 3` is the error-compensated 3xTF32 split (a_hi*b_hi + a_hi*b_lo +
 //     a_lo*b_hi; filter split on the host, activations split in registers), fp32-accurate, used by the parity tests;
 //   * bias + ReLU fused in the epilogue; the output may be written into a channel slice of a wider buffer
 //     (concat fusion) and a transposed stride-2 conv is the same kernel over a virtually zero-stuffed input.
 //
-// tcgen05/TMEM is deliberately not used here: with N <= 64 and K <= 64 per tap the operands are far below the
-// 128xNx8 UMMA tile economy, and the layers are bound by activation traffic, not by MMA issue.
+// wgmma is deliberately not used here: with N <= 64 and K <= 64 per tap the operands are far below a warpgroup MMA's
+// 64xNx8 tile economy, and the layers are bound by activation traffic, not by MMA issue.
 #include <atomic>
 
 #if !defined(PM_EMU)  // host emulation build (tests/warp_emu.h) brings its own CUDA vocabulary
@@ -159,7 +159,7 @@ __device__ __forceinline__ void stage_tile(const ConvParams &p, int tile, float 
 // of THREADS / row_chunks.  Everything that depends on the column -- the pixel, the channel vector, the x bounds test, the
 // zero-stuffing parity, the shared and global column offsets -- leaves the loop; per chunk there remain the row bounds test,
 // one multiply-add for the global row and the copy (~8 instructions instead of ~22: staging was ~45 % of the issued
-// instructions of the 8-channel full-resolution layers, tools/sass_lines.py on profiles/r1_run23_ncu.md's kernels).
+// instructions of the 8-channel full-resolution layers, tools/sass_lines.py).
 template <bool VEC, bool STUFF, int THREADS>
 __device__ __forceinline__ void stage_tile_cols(const ConvParams &p, int tile, float *buf, int rows_per_tile) {
     const int rows_per_iter = p.step_r[THREADS / 256];  // THREADS / row_chunks >= 1
@@ -326,7 +326,7 @@ __global__ void __launch_bounds__(128 * NSPLIT) conv_nhwc_mma_kernel(const __gri
                     // split without conversion instructions: a_hi = the TF32 the tensor core would read anyway (low 13 mantissa
                     // bits cleared), a_lo = a - a_hi, exact in fp32 (Sterbenz) and handed over as raw bits -- the hardware keeps
                     // its 11 leading bits, so a_hi + tf32(a_lo) carries >= 22 bits of a.  cvt.rna here was ~10 issue slots per
-                    // register on sm_100 (profiles/r1_run17_conv_ncu.md); this is one LOP3 and one FADD.
+                    // register; this is one LOP3 and one FADD.
                     ah[0] = split_hi(lo.x); ah[1] = split_hi(hi.x); ah[2] = split_hi(lo.y); ah[3] = split_hi(hi.y);
                     al[0] = __float_as_uint(lo.x - __uint_as_float(ah[0]));
                     al[1] = __float_as_uint(hi.x - __uint_as_float(ah[1]));
@@ -479,8 +479,8 @@ int sm_count(int dev) {
 #if !defined(PM_EMU)  // (the emulation build re-reads its pretend SM count every call)
     if (dev >= 0 && dev < 64 && info[dev].sms > 0) return info[dev].sms;
 #endif
-    int n = 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) n = 148;
+    int n = 132;  // H100 SXM
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) n = 132;
     if (dev >= 0 && dev < 64) info[dev].sms = n;
     return n;
 }

@@ -1,26 +1,27 @@
-// pm_conv5.cu -- K-D5: channels-last 2-D convolution as an implicit GEMM on the 5th-generation tensor cores
-// (tcgen05.mma kind::tf32, accumulators in TMEM, operands staged by TMA), fp32-accurate through the error-compensated
-// 3xTF32 split.  Serves the FLOP-bound layers of the cascade in the fp32-accurate (timed, parity) mode: FeatureNet conv2..10
-// (reference models/net.py:9-70), the stage-2/3 offset convs (models/patchmatch.py:288-311), Refinement's 16->8 conv
-// (models/net.py:73-122).  The memory-bound layers and everything with a fused epilogue stay on pm_conv.cu (mma.sync).
+// pm_conv5.cu -- K-D5: channels-last 2-D convolution as an implicit GEMM on Hopper's warpgroup tensor cores
+// (wgmma.mma_async kind tf32, fp32 accumulators in registers, operands staged by TMA behind mbarriers), fp32-accurate
+// through the error-compensated 3xTF32 split.  Serves the FLOP-bound layers of the cascade in the fp32-accurate (timed,
+// parity) mode: FeatureNet conv2..10 (reference models/net.py:9-70), the stage-2/3 offset convs (models/patchmatch.py:288-311),
+// Refinement's 16->8 conv (models/net.py:73-122).  The memory-bound layers and everything with a fused epilogue stay on
+// pm_conv.cu (mma.sync).
 //
 // GEMM view: D[128 output pixels, Cout] = sum over filter taps of A_tap[128, Cin] . W_tap[Cin, Cout].
 //   * A_tap is ONE TMA box per tap: tensor map over the channels-last input {Cin, W, H, N}, box {<=32 channels, 16*s, 8*s, 1}
 //     with element strides {1, s, s, 1} (s = conv stride), placed at (x0*s + kx*dil - pad, y0*s + ky*dil - pad): the
 //     padding border and the map edge come back as zeros from the copy engine, the 128 pixels of the 16 x 8 output tile
-//     land as 128 rows of a K-major operand in the shared-memory swizzle (32 / 64 / 128 B = row bytes) tcgen05 reads.
+//     land as 128 rows of a K-major operand in the shared-memory swizzle (32 / 64 / 128 B = row bytes) wgmma reads.
 //   * W_tap (hi and lo parts, Cout padded to a multiple of 16) is pre-packed by the host IN that shared-memory image
 //     (ops.pack_conv_filter_tc5) and fetched with one bulk copy per tap.
-//   * 3xTF32: four "worker" warps split every landed A tile in place into A_hi (13 low mantissa bits cleared -- what the
-//     tensor core would read anyway) and A_lo = A - A_hi (exact), then the MMA warp issues per 8-channel slice
-//     A_lo.W_hi, A_hi.W_lo, A_hi.W_hi into the same fp32 TMEM accumulator: >= 21 bits of every product.
-//   * Epilogue: tcgen05.ld (32 lanes x 32 bit, 16 columns at a time) -> bias, ReLU -> channels-last stores (channel slice
-//     of a wider tensor allowed).
-// Roles per CTA (320 threads): warp 0 = TMA producer, warp 1 = MMA issuer + TMEM owner, warps 2..5 = 3xTF32 split,
-// warps 6..9 = epilogue.  Two accumulators in TMEM: the epilogue of tile i drains one while the MMAs of tile i+1 fill the
-// other (run 3 measured the single-accumulator version, whose split warps also ran the epilogue, at 1.5 us per filter tap).
-// Persistent CTAs walk tiles blockIdx.x, +gridDim.x, ...; an S-deep ring of (A, A_lo, W_hi, W_lo) stages decouples the roles;
-// every mbarrier wait is bounded (a pipeline bug traps instead of hanging the GPU).
+//   * 3xTF32: every landed A tile is split in place into A_hi (13 low mantissa bits cleared -- what the tensor core would
+//     read anyway) and A_lo = A - A_hi (exact); per 8-channel slice two wgmmas accumulate a_hi x [w_hi | w_lo] (N = 2 Npad)
+//     and a_lo x w_hi (N = Npad) into the same fp32 registers: >= 21 bits of every product.  The accumulator fragment of
+//     N = Npad is the first half of the one of N = 2 Npad, so column c holds a_hi.w_hi + a_lo.w_hi and column Npad + c holds
+//     a_hi.w_lo; the epilogue adds the two.
+// Roles per CTA (288 threads): warps 0..3 and 4..7 are two consumer warpgroups, each owning 64 of the tile's 128 pixels
+// (split its rows, issue its wgmmas, run its epilogue); warp 8 is the TMA producer.  A consumer splits stage t+1 while
+// the wgmmas of stage t are still in flight (wgmma.wait_group 1).  Persistent CTAs walk tiles blockIdx.x, +gridDim.x, ...;
+// an S-deep ring of (A, A_lo, W) stages decouples producer and consumers; every mbarrier wait is bounded (a pipeline bug
+// traps instead of hanging the GPU).
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <cuda_runtime.h>
@@ -36,8 +37,9 @@ extern "C" int pmb200_internal_launch_status(const char *what);
 
 namespace {
 
-constexpr int kTW = 16, kTH = 8;  // output tile: 128 pixels = the M of one UMMA
-constexpr int kThreads = 320;
+constexpr int kTW = 16, kTH = 8;  // output tile: 128 pixels = two wgmma M = 64 halves
+constexpr int kThreads = 288;     // two consumer warpgroups + one producer warp
+constexpr int kProducerWarp = 8;
 
 struct Conv5Params {
     const float *wpack;  // [tap][kblock][w_hi rows Npad | w_lo rows Npad][RB bytes], swizzled image
@@ -51,9 +53,7 @@ struct Conv5Params {
     int a_bytes;   // 128 * RB * KB
     int w_bytes;   // Npad * RB * KB (one of hi / lo)
     int stage_bytes;
-    uint32_t idesc, idesc2;  // N = Npad / N = 2 Npad
-    uint32_t layout_type;  // UMMA smem-descriptor swizzle code: 2 = 128B, 4 = 64B, 6 = 32B
-    uint32_t tmem_cols;
+    uint32_t layout_type;  // wgmma smem-descriptor swizzle code (bits 62-63): 1 = 128B, 2 = 64B, 3 = 32B
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -91,78 +91,151 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t by
                  "l"(src), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void proxy_fence_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ bool elect_one() {  // one lane of the (converged) warp
-    uint32_t pred = 0;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void tc_commit(uint64_t *bar) {  // arrives on `bar` once every MMA issued so far has completed
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Shared-memory matrix descriptor of a K-major operand tile in the 32/64/128-byte swizzle (rows of RB bytes, 8-row groups
-// 8*RB apart): bits 0-13 start address >> 4, 16-29 leading byte offset (unused when swizzled: 1), 32-45 stride byte offset
-// (8*RB) >> 4, 46 version (Blackwell), 61-63 swizzle code (2 = 128B, 4 = 64B, 6 = 32B).  The kernels build it as two words.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// named barrier over `threads` threads (a multiple of 32); id 0 is __syncthreads
+__device__ __forceinline__ void bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+
+// wgmma bookkeeping: fence before the first wgmma that reads registers other code wrote, commit the issued wgmmas as one group,
+// wait until at most N groups of this warp are pending
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator registers across the asynchronous wgmma window
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// D[64, N] (+)= A[64, 8] . B[8, N]^T, tf32 operands from shared memory (both K-major), fp32 accumulators: thread (warp w, lane l)
+// holds for every 8-column chunk i the registers 4i..4i+3 = (row 16w + l/4, cols 8i + 2(l%4) + {0,1}), (row + 8, same cols).
+// scale_d == 0 overwrites the accumulators.
+template <int N>
+struct Wgmma;
+template <> struct Wgmma<16> {
+    static __device__ __forceinline__ void mma(float *d, uint64_t a, uint64_t b, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "l"(a), "l"(b), "r"(scale_d));
+    }
+};
+template <> struct Wgmma<32> {
+    static __device__ __forceinline__ void mma(float *d, uint64_t a, uint64_t b, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(a), "l"(b), "r"(scale_d));
+    }
+};
+template <> struct Wgmma<48> {
+    static __device__ __forceinline__ void mma(float *d, uint64_t a, uint64_t b, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+            : "l"(a), "l"(b), "r"(scale_d));
+    }
+};
+template <> struct Wgmma<64> {
+    static __device__ __forceinline__ void mma(float *d, uint64_t a, uint64_t b, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "l"(a), "l"(b), "r"(scale_d));
+    }
+};
+template <> struct Wgmma<96> {
+    static __device__ __forceinline__ void mma(float *d, uint64_t a, uint64_t b, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+            : "l"(a), "l"(b), "r"(scale_d));
+    }
+};
+template <> struct Wgmma<128> {
+    static __device__ __forceinline__ void mma(float *d, uint64_t a, uint64_t b, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "l"(a), "l"(b), "r"(scale_d));
+    }
+};
+// Shared-memory matrix descriptor: bits 0-13 start address >> 4, 16-29 leading byte offset >> 4 (distance of the K-adjacent
+// core matrix; unused by the swizzled K-major layouts), 32-45 stride byte offset >> 4 (distance of the next 8-row group),
+// 62-63 swizzle (0 none, 1 = 128B, 2 = 64B, 3 = 32B).  The kernels carry it as (lo, hi) words and only add 16-byte offsets
+// to lo (shared-memory addresses stay below 2^18, so the 14-bit field never carries).
+__device__ __forceinline__ uint64_t desc_of(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
+
+// the epilogue of one consumer warpgroup: its 64 accumulator rows -> bias, ReLU -> channels-last stores (channel slice of a
+// wider tensor allowed).  pix(m) maps the tile row m (0..127) to the output pixel; rows outside the map are dropped.
+template <int NPAD, typename PixOf>
+__device__ __forceinline__ void store_tile(const float (&acc)[NPAD], const float *bias, float *y, int n, int Ho, int Wo, int Cout,
+                                           int relu, int ycs, int yco, int row0, PixOf pix) {
+    const int lane = threadIdx.x & 31, w4 = (threadIdx.x >> 5) & 3;
+    const bool vec2 = ((ycs | yco) & 1) == 0;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int m = row0 + 16 * w4 + (lane >> 2) + 8 * h;
+        int oy, ox;
+        pix(m, oy, ox);
+        if (oy >= Ho || ox >= Wo) continue;
+        float *dst = y + (((size_t)n * Ho + oy) * Wo + ox) * ycs + yco;
+#pragma unroll
+        for (int i = 0; i < NPAD / 8; ++i) {
+            const int co = 8 * i + 2 * (lane & 3);
+            float v0 = acc[4 * i + 2 * h] + acc[4 * (i + NPAD / 8) + 2 * h];
+            float v1 = acc[4 * i + 2 * h + 1] + acc[4 * (i + NPAD / 8) + 2 * h + 1];
+            if (bias) {
+                v0 += co < Cout ? __ldg(bias + co) : 0.0f;
+                v1 += co + 1 < Cout ? __ldg(bias + co + 1) : 0.0f;
+            }
+            if (relu) { v0 = fmaxf(v0, 0.0f); v1 = fmaxf(v1, 0.0f); }
+            if (co + 1 < Cout && vec2) {
+                *reinterpret_cast<float2 *>(dst + co) = make_float2(v0, v1);
+            } else {
+                if (co < Cout) dst[co] = v0;
+                if (co + 1 < Cout) dst[co + 1] = v1;
+            }
+        }
+    }
+}
+
+__device__ __forceinline__ float4 tf32_hi(const float4 v) {
+    return make_float4(__uint_as_float(__float_as_uint(v.x) & 0xffffe000u), __uint_as_float(__float_as_uint(v.y) & 0xffffe000u),
+                       __uint_as_float(__float_as_uint(v.z) & 0xffffe000u), __uint_as_float(__float_as_uint(v.w) & 0xffffe000u));
+}
+
+template <int NPAD>
 __global__ void __launch_bounds__(kThreads) conv5_kernel(const Conv5Params p, const __grid_constant__ CUtensorMap xmap) {
     extern __shared__ unsigned char smem_raw[];
     // the swizzled operand tiles need 1024-byte alignment: align the dynamic segment by hand (the launch adds the slack)
     unsigned char *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    // [0, 256): barriers + TMEM address; stages start at 1024
+    // [0, 256): barriers; stages start at 1024
     uint64_t *full = reinterpret_cast<uint64_t *>(smem);  // [stages]  TMA landed
-    uint64_t *split = full + 8;                            // [stages]  A_hi / A_lo written
-    uint64_t *empty = split + 8;                           // [stages]  MMAs that read the stage have completed
-    uint64_t *acc_full = empty + 8;                        // [2] tile accumulated in TMEM buffer a
-    uint64_t *acc_empty = acc_full + 2;                    // [2] the epilogue has read buffer a
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_empty + 2);
+    uint64_t *empty = full + 8;                            // [stages]  the wgmmas that read the stage have completed (8 warps)
     unsigned char *stage0 = smem + 1024;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
         for (int s = 0; s < p.stages; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&split[s], 4);
-            mbar_init(&empty[s], 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&acc_full[a], 1);
-            mbar_init(&acc_empty[a], 4);
+            mbar_init(&empty[s], 8);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {  // TMEM: Npad fp32 columns x 128 lanes
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
     const int T = p.KS * p.KS;
     const int per_img = p.tiles_x * p.tiles_y;
 
-    if (warp == 0) {
+    if (warp == kProducerWarp) {
         // ------------------------------------------------ TMA producer ------------------------------------------------
         if (lane == 0) {
             int s = 0;
@@ -184,127 +257,63 @@ __global__ void __launch_bounds__(kThreads) conv5_kernel(const Conv5Params p, co
                 }
             }
         }
-    } else if (warp == 1) {
-        // ------------------------------------------------- MMA issuer -------------------------------------------------
-        // Whole warp on warp-uniform values, tcgen05 instructions from the elected lane (see conv5h_kernel); 2 MMAs per K
-        // slice: a_hi x [w_hi | w_lo] (N = 2 Npad, columns [0, 2 Npad)) and a_lo x w_hi (N = Npad, columns [0, Npad)).
-        const bool leader = elect_one();
-        int s = 0, it = 0;
-        uint32_t par = 0;
-        const int per_row = p.RB / 32;  // 8-channel slices per operand row
-        // descriptor words: lo = start address >> 4 | LBO field 1, hi = SBO (8 rows) >> 4 | version | swizzle code << 29
-        const uint32_t hiword = ((8u * (uint32_t)p.RB) >> 4) | (1u << 14) | (p.layout_type << 29);
-        const uint32_t stage_u32 = smem_u32(stage0);
-        const uint32_t a_kb16 = (128u * (uint32_t)p.RB) >> 4, w_kb16 = (2u * (uint32_t)p.Npad * (uint32_t)p.RB) >> 4;
-        for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-            const int ab = it & 1;                                  // accumulator buffer of this tile
-            const uint32_t tacc = tmem + (uint32_t)(ab * 2 * p.Npad);
-            mbar_wait(&acc_empty[ab], (((uint32_t)it >> 1) & 1u) ^ 1u);  // the epilogue of tile it-2 has drained this buffer
-            tc_fence_after();
-            uint32_t first = 0;
-            for (int t = 0; t < T; ++t) {
-                mbar_wait(&split[s], par);
-                tc_fence_after();
-                const uint32_t a_hi = ((stage_u32 + (uint32_t)(s * p.stage_bytes)) >> 4) | (1u << 16);
-                const uint32_t a_lo = a_hi + ((uint32_t)p.a_bytes >> 4), w0 = a_lo + ((uint32_t)p.a_bytes >> 4);
-                for (int kb = 0; kb < p.KB; ++kb) {
-                    for (int kin = 0; kin < per_row; ++kin) {
-                        const uint32_t ao = (uint32_t)kb * a_kb16 + 2u * kin, wo = (uint32_t)kb * w_kb16 + 2u * kin;  // 32 bytes per slice
-                        const uint64_t dw = ((uint64_t)hiword << 32) | (w0 + wo);
-                        if (leader) {
-                            tc_mma_tf32(tacc, ((uint64_t)hiword << 32) | (a_hi + ao), dw, p.idesc2, first);
-                            tc_mma_tf32(tacc, ((uint64_t)hiword << 32) | (a_lo + ao), dw, p.idesc, 1);
-                        }
-                        first = 1;
-                    }
-                }
-                if (leader) {
-                    tc_commit(&empty[s]);                        // stage free once these MMAs have read it
-                    if (t == T - 1) tc_commit(&acc_full[ab]);    // accumulator complete
-                }
-                if (++s == p.stages) { s = 0; par ^= 1u; }
-            }
-        }
-    } else if (warp < 6) {
-        // ------------------------------------------------ 3xTF32 split ------------------------------------------------
-        const int wt = threadIdx.x - 64;     // 0..127: operand row handled by this thread
-        int s = 0;
-        uint32_t par = 0;
-        const int chunks = p.RB / 16;        // 16-byte chunks per operand row of one K block
-        for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-            for (int t = 0; t < T; ++t) {
-                mbar_wait(&full[s], par);
-                unsigned char *a = stage0 + (size_t)s * p.stage_bytes;
-                for (int kb = 0; kb < p.KB; ++kb) {
-                    unsigned char *rowp = a + (size_t)kb * 128 * p.RB + (size_t)wt * p.RB;
-                    for (int j = 0; j < chunks; ++j) {
-                        const int c = (j + wt) & (chunks - 1);  // rotated: the 8 lanes of a quarter-warp hit different banks
-                        float4 *q = reinterpret_cast<float4 *>(rowp + c * 16);
-                        const float4 v = *q;
-                        float4 h, l;
-                        h.x = __uint_as_float(__float_as_uint(v.x) & 0xffffe000u); l.x = v.x - h.x;
-                        h.y = __uint_as_float(__float_as_uint(v.y) & 0xffffe000u); l.y = v.y - h.y;
-                        h.z = __uint_as_float(__float_as_uint(v.z) & 0xffffe000u); l.z = v.z - h.z;
-                        h.w = __uint_as_float(__float_as_uint(v.w) & 0xffffe000u); l.w = v.w - h.w;
-                        *q = h;
-                        *reinterpret_cast<float4 *>(reinterpret_cast<unsigned char *>(q) + p.a_bytes) = l;
-                    }
-                }
-                proxy_fence_async();  // generic-proxy writes above -> visible to the tensor core's async-proxy reads
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&split[s]);
-                if (++s == p.stages) { s = 0; par ^= 1u; }
-            }
-        }
-    } else {
-        // -------------------------------------------------- epilogue --------------------------------------------------
-        const int quad = warp & 3;           // TMEM lane quadrant this warp may read: lanes 32*quad .. 32*quad+31
-        const int row = quad * 32 + lane;    // accumulator row = pixel of the tile
-        const bool vec4 = ((p.ycs | p.yco) & 3) == 0;
-        int it = 0;
-        for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-            const int ab = it & 1;
-            mbar_wait(&acc_full[ab], ((uint32_t)it >> 1) & 1u);
-            tc_fence_after();
-            const int n = tile / per_img, tt = tile - n * per_img;
-            const int ty = tt / p.tiles_x, tx = tt - ty * p.tiles_x;
-            const int oy = ty * kTH + row / kTW, ox = tx * kTW + row % kTW;
-            const bool inside = oy < p.Ho && ox < p.Wo;
-            float *dst = p.y + (((size_t)n * p.Ho + (inside ? oy : 0)) * p.Wo + (inside ? ox : 0)) * p.ycs + p.yco;
-            for (int c0 = 0; c0 < p.Npad; c0 += 16) {
-                float v[16], u[16];
-                const uint32_t tcol = tmem + ((uint32_t)(quad * 32) << 16) + (uint32_t)(ab * 2 * p.Npad + c0);
-                tmem_ld16(tcol, v);                        // a_hi.w_hi + a_lo.w_hi
-                tmem_ld16(tcol + (uint32_t)p.Npad, u);     // a_hi.w_lo
-                if (c0 + 16 >= p.Npad) {  // last read of the accumulator: hand it back before the stores
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&acc_empty[ab]);
-                }
-                if (!inside) continue;
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const int co = c0 + i;
-                    float o = (v[i] + u[i]) + ((p.bias && co < p.Cout) ? __ldg(p.bias + co) : 0.0f);
-                    v[i] = p.relu ? fmaxf(o, 0.0f) : o;
-                }
-#pragma unroll
-                for (int i = 0; i < 16; i += 4) {
-                    const int co = c0 + i;
-                    if (co + 3 < p.Cout && vec4) {
-                        *reinterpret_cast<float4 *>(dst + co) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-                    } else {
-#pragma unroll
-                        for (int e = 0; e < 4; ++e)
-                            if (co + e < p.Cout) dst[co + e] = v[i + e];
-                    }
-                }
-            }
-        }
+        return;
     }
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(p.tmem_cols) : "memory");
+    // ------------------------------------------------- consumers -------------------------------------------------
+    const int wg = warp >> 2, wt = threadIdx.x & 127;
+    float acc[NPAD];
+    int s = 0, pend = -1;  // pend: stage whose wgmmas may still be in flight
+    uint32_t par = 0;
+    const int per_row = p.RB / 32;  // 8-channel slices per operand row
+    const uint32_t hiword = ((8u * (uint32_t)p.RB) >> 4) | (p.layout_type << 30);  // SBO = 8 rows
+    const uint32_t stage_u32 = smem_u32(stage0);
+    const uint32_t a_kb16 = (128u * (uint32_t)p.RB) >> 4, w_kb16 = (2u * (uint32_t)NPAD * (uint32_t)p.RB) >> 4;
+    const uint32_t half16 = (uint32_t)wg * ((64u * (uint32_t)p.RB) >> 4);  // this warpgroup's 64 rows
+    const int chunks = 4 * p.RB;                           // 16-byte chunks of 64 rows of one K block
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        for (int t = 0; t < T; ++t) {
+            mbar_wait(&full[s], par);
+            unsigned char *a = stage0 + (size_t)s * p.stage_bytes;
+            for (int kb = 0; kb < p.KB; ++kb) {
+                unsigned char *rows = a + (size_t)kb * 128 * p.RB + (size_t)wg * 64 * p.RB;
+                for (int c = wt; c < chunks; c += 128) {
+                    float4 *q = reinterpret_cast<float4 *>(rows + (size_t)c * 16);
+                    const float4 v = *q, h = tf32_hi(v);
+                    *q = h;
+                    *reinterpret_cast<float4 *>(reinterpret_cast<unsigned char *>(q) + p.a_bytes) =
+                        make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
+                }
+            }
+            proxy_fence_async();  // generic-proxy writes above -> visible to the tensor core's async-proxy reads
+            bar_sync(1 + wg, 128);
+            const uint32_t a_hi = ((stage_u32 + (uint32_t)(s * p.stage_bytes)) >> 4) + half16;
+            const uint32_t a_lo = a_hi + ((uint32_t)p.a_bytes >> 4), w0 = ((stage_u32 + (uint32_t)(s * p.stage_bytes)) >> 4) +
+                                                                           2u * ((uint32_t)p.a_bytes >> 4);
+            acc_fence(acc);
+            wg_fence();
+            for (int kb = 0; kb < p.KB; ++kb) {
+                for (int kin = 0; kin < per_row; ++kin) {
+                    const uint32_t ao = (uint32_t)kb * a_kb16 + 2u * kin, wo = (uint32_t)kb * w_kb16 + 2u * kin;  // 32 bytes per slice
+                    const uint64_t dw = desc_of((w0 + wo) | (1u << 16), hiword);
+                    Wgmma<2 * NPAD>::mma(acc, desc_of((a_hi + ao) | (1u << 16), hiword), dw, (t | kb | kin) ? 1u : 0u);
+                    Wgmma<NPAD>::mma(acc, desc_of((a_lo + ao) | (1u << 16), hiword), dw, 1u);
+                }
+            }
+            wg_commit();
+            acc_fence(acc);
+            wg_wait<1>();  // the wgmmas of the previous stage have completed: hand it back to the producer
+            if (pend >= 0 && lane == 0) mbar_arrive(&empty[pend]);
+            pend = s;
+            if (++s == p.stages) { s = 0; par ^= 1u; }
+        }
+        wg_wait<0>();
+        acc_fence(acc);
+        if (lane == 0) mbar_arrive(&empty[pend]);
+        pend = -1;
+        const int n = tile / per_img, tt = tile - n * per_img;
+        const int ty = tt / p.tiles_x, tx = tt - ty * p.tiles_x;
+        store_tile<NPAD>(acc, p.bias, p.y, n, p.Ho, p.Wo, p.Cout, p.relu, p.ycs, p.yco, 64 * wg,
+                         [&](int m, int &oy, int &ox) { oy = ty * kTH + m / kTW; ox = tx * kTW + m % kTW; });
     }
 }
 
@@ -316,21 +325,14 @@ __global__ void __launch_bounds__(kThreads) conv5_kernel(const Conv5Params p, co
 //   * 8 consecutive pixels of one plane ARE a core matrix (128 contiguous bytes),
 //   * the next 8-row group of the operand = the next output row = + (halo cols * 16) bytes      (descriptor SBO),
 //   * the second half of an 8-channel K slice = the next plane = + (halo rows * cols * 16) bytes (descriptor LBO),
-//   * filter tap (ky, kx) = start address + ((ky*dil) * cols + kx*dil) * 16 bytes -- always 16-byte aligned, no swizzle phase.
+//   * filter tap (ky, kx) = start address + ((ky*dil) * cols + kx*dil) * 16 bytes -- always 16-byte aligned, no swizzle phase,
+//   * the second consumer warpgroup's M = 64 half = output rows 8..15 = + 8 * cols * 16 bytes.
 // The halo tile arrives as ONE dense TMA box {Cin, cols, rows, 1} (rows of Cin*4 bytes, zero fill for the padding) in a staging
-// buffer; the four split warps, which touch every element anyway, write A_hi / A_lo TRANSPOSED into the planes (chunk order
-// rotated by pixel: conflict-free reads and writes).  (Run 6 measured the first version, whose 5-D tensor map {4, W, H, Cin/4, N}
-// made the TMA engine gather the planes itself in 16-byte pieces: correct, but 55 us on conv6/7 -- the engine is slow at that
-// granularity.)  Output tile: 8 wide x 16 tall.  Load and split happen ONCE per tile; the filter taps stream through a small
-// ring.  Roles and accumulator double buffering as conv5_kernel.
-//
-// MMA economy (tools/umma_rate.cu, profiles/r2_umma_rate.json): one tcgen05.mma with M = 128 costs max(49, N/2) cycles whatever
-// its kind -- below N = 128 the instruction, not the arithmetic, is the unit of cost, and the first version of this kernel
-// (3 MMAs of N = Npad per K slice, ~23 issue-thread instructions each) ran at 146 cycles per MMA, bound by the issuing thread.
-// So (a) the filter tap is stored as ONE operand [chunk][w_hi rows | w_lo rows][4 floats] (ops.pack_conv_filter_tc5h):
-// a_hi x [w_hi | w_lo] is one MMA of N = 2 Npad into columns [0, 2 Npad), a_lo x w_hi one of N = Npad into [0, Npad) -- 2 MMAs
-// per K slice instead of 3, the epilogue adds the two column halves; (b) the issue loop carries descriptors as (lo, hi) words
-// and only adds 16-byte offsets to the low word.
+// buffer; the two consumer warpgroups, which touch every element anyway, write A_hi / A_lo TRANSPOSED into the planes (chunk
+// order rotated by pixel: conflict-free reads and writes).  Output tile: 8 wide x 16 tall.  Load and split happen ONCE per
+// tile; the filter taps stay resident in shared memory when they fit, else stream through a small ring.
+// The filter tap is stored as ONE operand [chunk][w_hi rows | w_lo rows][4 floats] (ops.pack_conv_filter_tc5h): a_hi x
+// [w_hi | w_lo] is one wgmma of N = 2 Npad, a_lo x w_hi one of N = Npad -- 2 wgmmas per K slice instead of 3.
 // ----------------------------------------------------------------------------------------------------------------------
 constexpr int kHTW = 8, kHTH = 16;
 
@@ -344,12 +346,11 @@ struct Conv5hParams {
     int plane_bytes;      // hrows * hcols * 16
     int a_bytes;          // plane_bytes * Cin/4 (one of hi / lo) = what one TMA box delivers into a staging buffer
     int a_stride;         // a_bytes rounded up to 128: distance between staging buffers, hi -> lo, plane sets (2 * a_stride)
-    int hbufs;            // plane sets (hi, lo): 2 when they fit (split of tile i+1 under the MMAs of tile i), else 1
+    int hbufs;            // plane sets (hi, lo): 2 when they fit (split of tile i+1 while the other warpgroup finishes tile i), else 1
     int sbufs;            // staging buffers: 2 when they fit (TMA of tile i+1 under the split of tile i), else 1
     int w_bytes;          // Npad * Cin * 4 (one of hi / lo)
     int wstages;
     int w_resident;       // 1: wstages == KS*KS, every tap loaded once per CTA; 0: taps stream through the ring per tile
-    uint32_t idesc, idesc2, tmem_cols;  // idesc: N = Npad, idesc2: N = 2 Npad
     long long *trace;     // debugging aid (pmb200_debug_conv5h_trace): clock64 stamps of CTA 0's roles, [role][tile 0..15][event 0..3]
 };
 
@@ -357,33 +358,26 @@ __device__ __forceinline__ void stamp(const Conv5hParams &p, int role, int it, i
     if (p.trace && blockIdx.x == 0 && it < 16) p.trace[(role * 16 + it) * 4 + ev] = clock64();
 }
 
-// Operands of this kernel are no-swizzle K-major: core matrices of 8 rows x 16 bytes; descriptor LBO = distance of the
-// K-adjacent core matrix, SBO = distance of the next 8-row group, version bit 46, layout type 0.
-// the MMAs of one filter tap: per 8-channel slice a_hi x [w_hi | w_lo] (N = 2 Npad) and a_lo x w_hi (N = Npad)
-template <int KSL>
-__device__ __forceinline__ void issue_tap(bool leader, uint32_t tacc, uint32_t ah, uint32_t al, uint32_t w, uint32_t a_kstep, uint32_t w_kstep,
-                                          uint32_t a_hiword, uint32_t w_hiword, uint32_t idesc, uint32_t idesc2, uint32_t first) {
-    if (!leader) return;
+// the wgmmas of one filter tap: per 8-channel slice a_hi x [w_hi | w_lo] (N = 2 Npad) and a_lo x w_hi (N = Npad)
+template <int NPAD, int KSL>
+__device__ __forceinline__ void issue_tap(float (&acc)[NPAD], uint32_t ah, uint32_t al, uint32_t w, uint32_t a_kstep, uint32_t w_kstep,
+                                          uint32_t a_hiword, uint32_t w_hiword, uint32_t first) {
 #pragma unroll
     for (int k = 0; k < KSL; ++k) {
-        const uint64_t dw = ((uint64_t)w_hiword << 32) | (w + k * w_kstep);
-        tc_mma_tf32(tacc, ((uint64_t)a_hiword << 32) | (ah + k * a_kstep), dw, idesc2, k == 0 ? first : 1u);
-        tc_mma_tf32(tacc, ((uint64_t)a_hiword << 32) | (al + k * a_kstep), dw, idesc, 1);
+        const uint64_t dw = desc_of(w + k * w_kstep, w_hiword);
+        Wgmma<2 * NPAD>::mma(acc, desc_of(ah + k * a_kstep, a_hiword), dw, k == 0 ? first : 1u);
+        Wgmma<NPAD>::mma(acc, desc_of(al + k * a_kstep, a_hiword), dw, 1u);
     }
 }
 
+template <int NPAD>
 __global__ void __launch_bounds__(kThreads) conv5h_kernel(const Conv5hParams p, const __grid_constant__ CUtensorMap xmap) {
     extern __shared__ unsigned char smem_raw[];
     unsigned char *smem = smem_raw + ((128u - (smem_u32(smem_raw) & 127u)) & 127u);
     uint64_t *h_full = reinterpret_cast<uint64_t *>(smem);  // [2] halo tile landed in a staging buffer
     uint64_t *s_free = h_full + 2;                           // [2] the split has read the staging buffer
-    uint64_t *h_split = s_free + 2;                          // [2] A_hi / A_lo planes written
-    uint64_t *h_empty = h_split + 2;                         // [2] every MMA of the tile has read the plane set
-    uint64_t *w_full = h_empty + 2;                          // [25] filter tap landed
-    uint64_t *w_empty = w_full + 25;                         // [25] its MMAs have completed
-    uint64_t *acc_full = w_empty + 25;                       // [2]
-    uint64_t *acc_empty = acc_full + 2;                      // [2]
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_empty + 2);
+    uint64_t *w_full = s_free + 2;                           // [25] filter tap landed
+    uint64_t *w_empty = w_full + 25;                         // [25] its wgmmas have completed (8 consumer warps)
     unsigned char *stage0 = smem + 640;                                     // [sbufs][a_stride]  dense [rows][cols][Cin]
     unsigned char *halo0 = stage0 + (size_t)p.sbufs * p.a_stride;           // [hbufs][hi, lo][a_stride]  planes
     unsigned char *wring = halo0 + (size_t)p.hbufs * 2 * p.a_stride;        // [wstages][hi, lo][w_bytes]
@@ -392,32 +386,20 @@ __global__ void __launch_bounds__(kThreads) conv5h_kernel(const Conv5hParams p, 
     if (threadIdx.x == 0) {
         for (int a = 0; a < 2; ++a) {
             mbar_init(&h_full[a], 1);
-            mbar_init(&s_free[a], 4);
-            mbar_init(&h_split[a], 4);
-            mbar_init(&h_empty[a], 1);
-            mbar_init(&acc_full[a], 1);
-            mbar_init(&acc_empty[a], 4);
+            mbar_init(&s_free[a], 1);
         }
         for (int s = 0; s < p.wstages; ++s) {
             mbar_init(&w_full[s], 1);
-            mbar_init(&w_empty[s], 1);
+            mbar_init(&w_empty[s], 8);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
     const int T = p.KS * p.KS;
     const int per_img = p.tiles_x * p.tiles_y;
 
-    if (warp == 0) {
+    if (warp == kProducerWarp) {
         // ------------------------------------------------ TMA producer ------------------------------------------------
         if (lane == 0) {
             auto load_halo = [&](int tile, int use) {  // `use` = how many halo tiles this CTA has requested before
@@ -440,7 +422,7 @@ __global__ void __launch_bounds__(kThreads) conv5h_kernel(const Conv5hParams p, 
             int it = 0, s = 0;
             uint32_t wpar = 0;
             for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-                // the NEXT tile's halo first: its latency (and its split) hide under this tile's MMAs
+                // the NEXT tile's halo first: its latency (and its split) hide under this tile's wgmmas
                 if (tile + (int)gridDim.x < p.total_tiles) load_halo(tile + gridDim.x, it + 1);
                 if (p.w_resident) continue;
                 for (int t = 0; t < T; ++t) {
@@ -450,150 +432,88 @@ __global__ void __launch_bounds__(kThreads) conv5h_kernel(const Conv5hParams p, 
                 }
             }
         }
-    } else if (warp == 1) {
-        // ------------------------------------------------- MMA issuer -------------------------------------------------
-        // The WHOLE warp runs the loops, on warp-uniform values only (kernel parameters, blockIdx, loop counters): the
-        // compiler then keeps descriptors and addresses in uniform registers and the tcgen05 instructions issue back to back
-        // from the elected lane.  (Run under `if (lane == 0)` every MMA was wrapped in an R2UR / ELECT / BRA.U.ANY sequence:
-        // 108 cycles per MMA measured by the role trace, twice the tensor pipe's 49.)
-        const bool leader = elect_one();
-        int it = 0, s = 0;
-        uint32_t wpar = 0;
-        const int kslices = p.Cin / 8;
-        // descriptors as (lo, hi) words: lo = start address >> 4 | LBO >> 4 << 16, hi = SBO >> 4 | version; offsets are added
-        // to lo in 16-byte units (shared-memory addresses stay below 2^18, so the 14-bit field never carries)
-        const uint32_t a_hiword = ((uint32_t)p.hcols) | (1u << 14);           // SBO = hcols * 16 bytes
-        const uint32_t w_hiword = (128u >> 4) | (1u << 14);                   // SBO = 128 bytes
-        const uint32_t a_lbo16 = (uint32_t)p.plane_bytes >> 4, w_lbo16 = 2u * (uint32_t)p.Npad;  // next chunk: plane / 2 Npad rows
-        const uint32_t a_kstep = 2u * a_lbo16, w_kstep = 2u * w_lbo16;        // one K slice = two chunks
-        const uint32_t halo_u32 = smem_u32(halo0), ring_u32 = smem_u32(wring);
-        for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-            const int hb = it % p.hbufs, ab = it & 1;
-            const uint32_t tacc = tmem + (uint32_t)(ab * 2 * p.Npad);
-            mbar_wait(&acc_empty[ab], (((uint32_t)it >> 1) & 1u) ^ 1u);
-            if (lane == 0) stamp(p, 1, it, 0);
-            mbar_wait(&h_split[hb], (uint32_t)(it / p.hbufs) & 1u);
-            if (lane == 0) stamp(p, 1, it, 1);
-            tc_fence_after();
-            const uint32_t ahi_lo = ((halo_u32 + (uint32_t)(hb * 2 * p.a_stride)) >> 4) | (a_lbo16 << 16);
-            const uint32_t alo_lo = ahi_lo + ((uint32_t)p.a_stride >> 4);
-            uint32_t first = 0;  // 0 for the very first MMA of the tile (overwrites the accumulator)
-            for (int ky = 0; ky < p.KS; ++ky) {
-                for (int kx = 0; kx < p.KS; ++kx) {
-                    if (!p.w_resident || it == 0) {  // a resident filter is waited for once, during the first tile
-                        mbar_wait(&w_full[s], wpar);
-                        tc_fence_after();
-                    }
-                    const uint32_t shift = (uint32_t)((ky * p.dil) * p.hcols + kx * p.dil);
-                    const uint32_t ah = ahi_lo + shift, al = alo_lo + shift;
-                    const uint32_t w = ((ring_u32 + (uint32_t)(s * 2 * p.w_bytes)) >> 4) | (w_lbo16 << 16);
-                    switch (kslices) {  // unrolled: the per-slice descriptor steps become immediates of uniform adds
-                    case 1: issue_tap<1>(leader, tacc, ah, al, w, a_kstep, w_kstep, a_hiword, w_hiword, p.idesc, p.idesc2, first); break;
-                    case 2: issue_tap<2>(leader, tacc, ah, al, w, a_kstep, w_kstep, a_hiword, w_hiword, p.idesc, p.idesc2, first); break;
-                    case 4: issue_tap<4>(leader, tacc, ah, al, w, a_kstep, w_kstep, a_hiword, w_hiword, p.idesc, p.idesc2, first); break;
-                    default: issue_tap<8>(leader, tacc, ah, al, w, a_kstep, w_kstep, a_hiword, w_hiword, p.idesc, p.idesc2, first); break;
-                    }
-                    first = 1;
-                    if (p.w_resident) {
-                        if (++s == p.wstages) s = 0;  // phase 0 of every w_full completed once and stays complete
-                    } else {
-                        if (leader) tc_commit(&w_empty[s]);
-                        if (++s == p.wstages) { s = 0; wpar ^= 1u; }
-                    }
-                }
-            }
-            if (leader) {
-                tc_commit(&h_empty[hb]);   // plane set free once every MMA of the tile has read it
-                tc_commit(&acc_full[ab]);
-            }
-            if (lane == 0) stamp(p, 1, it, 2);
-        }
-    } else if (warp < 6) {
-        // ------------------------------------------------ 3xTF32 split ------------------------------------------------
-        const int wt = threadIdx.x - 64;  // 0..127
-        int it = 0;
-        const int P = p.hcols * p.hrows, NC = p.Cin / 4;  // pixels of the halo tile, 16-byte channel chunks per pixel
-        for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-            const int sb = it % p.sbufs, hb = it % p.hbufs;
-            mbar_wait(&h_full[sb], (uint32_t)(it / p.sbufs) & 1u);            // dense halo tile landed
-            if (wt == 0) stamp(p, 2, it, 0);
-            mbar_wait(&h_empty[hb], ((uint32_t)(it / p.hbufs) & 1u) ^ 1u);    // the MMAs that read this plane set are done
-            if (wt == 0) stamp(p, 2, it, 1);
+        return;
+    }
+    // ------------------------------------------------- consumers -------------------------------------------------
+    const int wg = warp >> 2, ct = threadIdx.x;  // ct: 0..255 over both consumer warpgroups
+    float acc[NPAD];
+    int it = 0, s = 0;
+    uint32_t wpar = 0;
+    const int kslices = p.Cin / 8;
+    const int P = p.hcols * p.hrows, NC = p.Cin / 4;  // pixels of the halo tile, 16-byte channel chunks per pixel
+    const uint32_t a_hiword = (uint32_t)p.hcols;          // SBO = hcols * 16 bytes, no swizzle
+    const uint32_t w_hiword = 128u >> 4;                  // SBO = 128 bytes
+    const uint32_t a_lbo16 = (uint32_t)p.plane_bytes >> 4, w_lbo16 = 2u * (uint32_t)NPAD;  // next chunk: plane / 2 Npad rows
+    const uint32_t a_kstep = 2u * a_lbo16, w_kstep = 2u * w_lbo16;                        // one K slice = two chunks
+    const uint32_t halo_u32 = smem_u32(halo0), ring_u32 = smem_u32(wring);
+    const uint32_t half16 = (uint32_t)wg * 8u * (uint32_t)p.hcols;  // output rows 8..15 for the second warpgroup
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
+        const int sb = it % p.sbufs, hb = it % p.hbufs;
+        // ---- split: dense staging tile -> A_hi / A_lo planes.  With two plane sets the set of tile it-2 is free: both
+        // warpgroups passed the barrier below for tile it-1 only after their wgmmas of tile it-2 completed.  With one set,
+        // wait here until the other warpgroup's wgmmas of tile it-1 have completed.
+        mbar_wait(&h_full[sb], (uint32_t)(it / p.sbufs) & 1u);
+        if (ct == 0) stamp(p, 2, it, 0);
+        if (p.hbufs == 1) bar_sync(1, 256);
+        {
             const float4 *src = reinterpret_cast<const float4 *>(stage0 + (size_t)sb * p.a_stride);
             float4 *ahi = reinterpret_cast<float4 *>(halo0 + (size_t)hb * 2 * p.a_stride);
             float4 *alo = reinterpret_cast<float4 *>(halo0 + (size_t)hb * 2 * p.a_stride + p.a_stride);
-            for (int px = wt; px < P; px += 128) {
+            for (int px = ct; px < P; px += 256) {
                 for (int j = 0; j < NC; ++j) {
                     const int c = (j + px) & (NC - 1);  // rotated by pixel: the 8 lanes of a quarter-warp read 8 bank groups
-                    const float4 v = src[px * NC + c];
-                    float4 h, l;
-                    h.x = __uint_as_float(__float_as_uint(v.x) & 0xffffe000u); l.x = v.x - h.x;
-                    h.y = __uint_as_float(__float_as_uint(v.y) & 0xffffe000u); l.y = v.y - h.y;
-                    h.z = __uint_as_float(__float_as_uint(v.z) & 0xffffe000u); l.z = v.z - h.z;
-                    h.w = __uint_as_float(__float_as_uint(v.w) & 0xffffe000u); l.w = v.w - h.w;
-                    ahi[c * P + px] = h;  // plane c: 16 bytes per pixel; consecutive lanes, consecutive pixels (P is even)
-                    alo[c * P + px] = l;
+                    const float4 v = src[px * NC + c], h = tf32_hi(v);
+                    ahi[c * P + px] = h;  // plane c: 16 bytes per pixel; consecutive lanes, consecutive pixels
+                    alo[c * P + px] = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
                 }
             }
-            proxy_fence_async();
-            __syncwarp();
-            if (lane == 0) {
-                mbar_arrive(&h_split[hb]);
-                mbar_arrive(&s_free[sb]);
-            }
-            if (wt == 0) stamp(p, 2, it, 2);
         }
-    } else {
-        // -------------------------------------------------- epilogue --------------------------------------------------
-        const int quad = warp & 3;
-        const int row = quad * 32 + lane;  // accumulator row m -> output pixel (y0 + m / 8, x0 + m % 8)
-        const bool vec4 = ((p.ycs | p.yco) & 3) == 0;
-        int it = 0;
-        for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-            const int ab = it & 1;
-            mbar_wait(&acc_full[ab], ((uint32_t)it >> 1) & 1u);
-            if (threadIdx.x == 192) stamp(p, 3, it, 0);
-            tc_fence_after();
-            const int n = tile / per_img, tt = tile - n * per_img;
-            const int ty = tt / p.tiles_x, tx = tt - ty * p.tiles_x;
-            const int oy = ty * kHTH + row / kHTW, ox = tx * kHTW + row % kHTW;
-            const bool inside = oy < p.Ho && ox < p.Wo;
-            float *dst = p.y + (((size_t)n * p.Ho + (inside ? oy : 0)) * p.Wo + (inside ? ox : 0)) * p.ycs + p.yco;
-            for (int c0 = 0; c0 < p.Npad; c0 += 16) {
-                float v[16], u[16];
-                const uint32_t tcol = tmem + ((uint32_t)(quad * 32) << 16) + (uint32_t)(ab * 2 * p.Npad + c0);
-                tmem_ld16(tcol, v);                        // a_hi.w_hi + a_lo.w_hi
-                tmem_ld16(tcol + (uint32_t)p.Npad, u);     // a_hi.w_lo
-                if (c0 + 16 >= p.Npad) {
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&acc_empty[ab]);
+        proxy_fence_async();
+        bar_sync(1, 256);
+        if (ct == 0) {
+            mbar_arrive(&s_free[sb]);
+            stamp(p, 2, it, 1);
+        }
+        // ---- wgmmas of this warpgroup's 64 rows
+        const uint32_t ahi_lo = (((halo_u32 + (uint32_t)(hb * 2 * p.a_stride)) >> 4) + half16) | (a_lbo16 << 16);
+        const uint32_t alo_lo = ahi_lo + ((uint32_t)p.a_stride >> 4);
+        int pend = -1;  // ring slot whose wgmmas may still be in flight
+        acc_fence(acc);
+        for (int ky = 0; ky < p.KS; ++ky) {
+            for (int kx = 0; kx < p.KS; ++kx) {
+                if (!p.w_resident || it == 0) mbar_wait(&w_full[s], wpar);  // a resident filter is waited for once
+                const uint32_t shift = (uint32_t)((ky * p.dil) * p.hcols + kx * p.dil);
+                const uint32_t ah = ahi_lo + shift, al = alo_lo + shift;
+                const uint32_t w = ((ring_u32 + (uint32_t)(s * 2 * p.w_bytes)) >> 4) | (w_lbo16 << 16);
+                const uint32_t first = (ky | kx) ? 1u : 0u;  // 0 for the very first wgmma of the tile (overwrites the accumulators)
+                wg_fence();
+                switch (kslices) {  // unrolled: the per-slice descriptor steps become immediates
+                case 1: issue_tap<NPAD, 1>(acc, ah, al, w, a_kstep, w_kstep, a_hiword, w_hiword, first); break;
+                case 2: issue_tap<NPAD, 2>(acc, ah, al, w, a_kstep, w_kstep, a_hiword, w_hiword, first); break;
+                case 4: issue_tap<NPAD, 4>(acc, ah, al, w, a_kstep, w_kstep, a_hiword, w_hiword, first); break;
+                default: issue_tap<NPAD, 8>(acc, ah, al, w, a_kstep, w_kstep, a_hiword, w_hiword, first); break;
                 }
-                if (!inside) continue;
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const int co = c0 + i;
-                    float o = (v[i] + u[i]) + ((p.bias && co < p.Cout) ? __ldg(p.bias + co) : 0.0f);
-                    v[i] = p.relu ? fmaxf(o, 0.0f) : o;
-                }
-#pragma unroll
-                for (int i = 0; i < 16; i += 4) {
-                    const int co = c0 + i;
-                    if (co + 3 < p.Cout && vec4) {
-                        *reinterpret_cast<float4 *>(dst + co) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-                    } else {
-#pragma unroll
-                        for (int e = 0; e < 4; ++e)
-                            if (co + e < p.Cout) dst[co + e] = v[i + e];
-                    }
+                wg_commit();
+                acc_fence(acc);
+                if (p.w_resident) {
+                    if (++s == p.wstages) s = 0;  // phase 0 of every w_full completed once and stays complete
+                } else {
+                    wg_wait<1>();  // the previous tap's wgmmas have completed: its ring slot goes back to the producer
+                    if (pend >= 0 && lane == 0) mbar_arrive(&w_empty[pend]);
+                    pend = s;
+                    if (++s == p.wstages) { s = 0; wpar ^= 1u; }
                 }
             }
-            if (threadIdx.x == 192) stamp(p, 3, it, 1);
         }
-    }
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(p.tmem_cols) : "memory");
+        wg_wait<0>();
+        acc_fence(acc);
+        if (pend >= 0 && lane == 0) mbar_arrive(&w_empty[pend]);
+        if (ct == 0) stamp(p, 1, it, 0);
+        const int n = tile / per_img, tt = tile - n * per_img;
+        const int ty = tt / p.tiles_x, tx = tt - ty * p.tiles_x;
+        store_tile<NPAD>(acc, p.bias, p.y, n, p.Ho, p.Wo, p.Cout, p.relu, p.ycs, p.yco, 64 * wg,
+                         [&](int m, int &oy, int &ox) { oy = ty * kHTH + m / kHTW; ox = tx * kHTW + m % kHTW; });
+        if (ct == 0) stamp(p, 3, it, 0);
     }
 }
 
@@ -625,7 +545,57 @@ bool optin_max_smem(Kern kern, std::atomic<unsigned long long> &done, int dev, i
     return true;
 }
 
+// CTAs per SM the kernel's registers allow at this shared-memory size (at least 1, at most `want`)
+template <typename Kern>
+int resident_ctas(Kern kern, int smem, int want) {
+    int n = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, kThreads, smem) != cudaSuccess) {
+        cudaGetLastError();
+        return 1;
+    }
+    return n < 1 ? 1 : (n > want ? want : n);
+}
+
 int npad_of(int cout) { return (cout + 15) / 16 * 16; }
+
+// one instantiation per padded Cout: the accumulator fragment is a register array of Npad floats per thread
+template <template <int> class Launch, typename... Args>
+int by_npad(int npad, Args &&...args) {
+    switch (npad) {
+    case 16: return Launch<16>::run(args...);
+    case 32: return Launch<32>::run(args...);
+    case 48: return Launch<48>::run(args...);
+    default: return Launch<64>::run(args...);
+    }
+}
+
+template <int NPAD>
+struct LaunchConv5 {
+    static int run(const Conv5Params &p, const CUtensorMap &xmap, int dev, int sms, int smem_optin, cudaStream_t st) {
+        static std::atomic<unsigned long long> optin_done{0};
+        if (!optin_max_smem(conv5_kernel<NPAD>, optin_done, dev, smem_optin))
+            return pmb200_internal_fail(PMB200_EUNSUPPORTED, "conv2d_tc5: shared-memory opt-in failed");
+        const int smem = 1024 + p.stages * p.stage_bytes + 1024;  // + slack for the 1024-byte alignment of the dynamic segment
+        const int two = (2 * smem <= smem_optin + 1024) ? 2 : 1;
+        long long grid = (long long)sms * resident_ctas(conv5_kernel<NPAD>, smem, two);
+        if (grid > p.total_tiles) grid = p.total_tiles;
+        conv5_kernel<NPAD><<<(unsigned)grid, kThreads, smem, st>>>(p, xmap);
+        return pmb200_internal_launch_status("conv2d_tc5");
+    }
+};
+
+template <int NPAD>
+struct LaunchConv5h {
+    static int run(const Conv5hParams &p, const CUtensorMap &xmap, int smem, int ctas, int dev, int sms, int smem_optin, cudaStream_t st) {
+        static std::atomic<unsigned long long> optin_done{0};
+        if (!optin_max_smem(conv5h_kernel<NPAD>, optin_done, dev, smem_optin))
+            return pmb200_internal_fail(PMB200_EUNSUPPORTED, "conv2d_tc5h: shared-memory opt-in failed");
+        long long grid = (long long)sms * resident_ctas(conv5h_kernel<NPAD>, smem, ctas);
+        if (grid > p.total_tiles) grid = p.total_tiles;
+        conv5h_kernel<NPAD><<<(unsigned)grid, kThreads, smem, st>>>(p, xmap);
+        return pmb200_internal_launch_status("conv2d_tc5h");
+    }
+};
 
 }  // namespace
 
@@ -674,29 +644,18 @@ int pmb200_conv2d_tc5(const float *x_nhwc, const float *filter_tc5, const float 
     p.w_bytes = p.Npad * p.RB * p.KB;
     p.stage_bytes = 2 * p.a_bytes + 2 * p.w_bytes;  // multiples of 1024 except tiny layers: keep every stage 1024-aligned
     p.stage_bytes = (p.stage_bytes + 1023) / 1024 * 1024;
-    p.layout_type = p.RB == 128 ? 2u : (p.RB == 64 ? 4u : 6u);
-    p.idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(p.Npad >> 3) << 17) | ((128u >> 4) << 24);  // F32 += TF32 . TF32, K-major both
-    p.idesc2 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(2 * p.Npad >> 3) << 17) | ((128u >> 4) << 24);
-    p.tmem_cols = 4 * p.Npad <= 64 ? 64u : (4 * p.Npad <= 128 ? 128u : 256u);  // two accumulators of 2 Npad fp32 columns
+    p.layout_type = p.RB == 128 ? 1u : (p.RB == 64 ? 2u : 3u);
 
     int dev = 0, sms = 0, smem_optin = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     // two CTAs per SM when the ring allows at least 3 stages each, else one CTA with as many stages as fit (<= 8)
-    int ctas = 2;
     int stages = ((smem_optin + 1024) / 2 - 1024 - 2048) / p.stage_bytes;
-    if (stages < 3) {
-        ctas = 1;
-        stages = (smem_optin - 2048) / p.stage_bytes;
-    }
+    if (stages < 3) stages = (smem_optin - 2048) / p.stage_bytes;
     if (stages > 8) stages = 8;
     if (stages < 2) return pmb200_internal_fail(PMB200_EUNSUPPORTED, "conv2d_tc5: a ring of two stages does not fit in shared memory");
     p.stages = stages;
-    const int smem = 1024 + stages * p.stage_bytes + 1024;  // + slack for the 1024-byte alignment of the dynamic segment
-    static std::atomic<unsigned long long> optin_done{0};
-    if (!optin_max_smem(conv5_kernel, optin_done, dev, smem_optin))
-        return pmb200_internal_fail(PMB200_EUNSUPPORTED, "conv2d_tc5: shared-memory opt-in failed");
     CUtensorMap xmap;
     const cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
     const cuuint64_t strides[3] = {(cuuint64_t)Cin * 4, (cuuint64_t)W * Cin * 4, (cuuint64_t)H * W * Cin * 4};
@@ -706,14 +665,11 @@ int pmb200_conv2d_tc5(const float *x_nhwc, const float *filter_tc5, const float 
     if (enc(&xmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float *>(x_nhwc), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
             CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
         return pmb200_internal_fail(PMB200_EINVAL, "conv2d_tc5: tensor map rejected (alignment / size)");
-    long long grid = (long long)sms * ctas;
-    if (grid > tiles) grid = tiles;
-    conv5_kernel<<<(unsigned)grid, kThreads, smem, reinterpret_cast<cudaStream_t>(stream)>>>(p, xmap);
-    return pmb200_internal_launch_status("conv2d_tc5");
+    return by_npad<LaunchConv5>(p.Npad, p, xmap, dev, sms, smem_optin, reinterpret_cast<cudaStream_t>(stream));
 }
 
 // Debugging aid: device buffer of 4 roles x 16 tiles x 4 events (256 int64) that the next K-D5h launches stamp with clock64
-// for CTA 0 (producer / MMA issuer / split / epilogue); nullptr switches it off.  Not part of the reference-facing surface.
+// for CTA 0 (producer / wgmmas done / split / epilogue done); nullptr switches it off.  Not part of the reference-facing surface.
 int pmb200_debug_conv5h_trace(long long *device_buffer_256) {
     g_conv5h_trace = device_buffer_256;
     return 0;
@@ -749,9 +705,6 @@ int pmb200_conv2d_tc5h(const float *x_nhwc, const float *filter_tc5h, const floa
     p.plane_bytes = p.hrows * p.hcols * 16;
     p.a_bytes = p.plane_bytes * (Cin / 4);
     p.w_bytes = p.Npad * Cin * 4;
-    p.idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(p.Npad >> 3) << 17) | ((128u >> 4) << 24);
-    p.idesc2 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(2 * p.Npad >> 3) << 17) | ((128u >> 4) << 24);
-    p.tmem_cols = 4 * p.Npad <= 64 ? 64u : (4 * p.Npad <= 128 ? 128u : 256u);  // two accumulators of 2 Npad fp32 columns
     if ((unsigned)p.plane_bytes >= (1u << 18) || p.hcols * 16 >= (1 << 18))
         return pmb200_internal_fail(PMB200_EUNSUPPORTED, "conv2d_tc5h: halo tile exceeds the descriptor's 14-bit offsets");
     int dev = 0, sms = 0, smem_optin = 0;
@@ -782,9 +735,6 @@ int pmb200_conv2d_tc5h(const float *x_nhwc, const float *filter_tc5h, const floa
     if (2 * (fixed + wst * 2 * p.w_bytes + 1024) <= smem_optin + 1024) ctas = 2;
     p.wstages = wst;
     const int smem = fixed + wst * 2 * p.w_bytes;
-    static std::atomic<unsigned long long> optin_done{0};
-    if (!optin_max_smem(conv5h_kernel, optin_done, dev, smem_optin))
-        return pmb200_internal_fail(PMB200_EUNSUPPORTED, "conv2d_tc5h: shared-memory opt-in failed");
     CUtensorMap xmap;
     const cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
     const cuuint64_t strides[3] = {(cuuint64_t)Cin * 4, (cuuint64_t)W * Cin * 4, (cuuint64_t)H * W * Cin * 4};
@@ -793,10 +743,7 @@ int pmb200_conv2d_tc5h(const float *x_nhwc, const float *filter_tc5h, const floa
     if (enc(&xmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float *>(x_nhwc), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
         return pmb200_internal_fail(PMB200_EINVAL, "conv2d_tc5h: tensor map rejected (alignment / size)");
-    long long grid = (long long)sms * ctas;
-    if (grid > tiles) grid = tiles;
-    conv5h_kernel<<<(unsigned)grid, kThreads, smem, reinterpret_cast<cudaStream_t>(stream)>>>(p, xmap);
-    return pmb200_internal_launch_status("conv2d_tc5h");
+    return by_npad<LaunchConv5h>(p.Npad, p, xmap, smem, ctas, dev, sms, smem_optin, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

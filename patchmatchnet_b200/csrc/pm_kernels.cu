@@ -1,4 +1,4 @@
-// pm_kernels.cu -- sm_100a forward kernels of the learned-PatchMatch hot path + their C ABI
+// pm_kernels.cu -- sm_90a forward kernels of the learned-PatchMatch hot path + their C ABI
 // (backward kernels: pm_backward.cu; per-element formulas shared with the CPU formula tests: pm_math.cuh).
 //
 // Kernel map (DESIGN.md has the byte/flop budgets and the measured numbers):
@@ -62,19 +62,14 @@ __device__ __forceinline__ float2 load_offset(const float *__restrict__ off, int
     return make_float2(__ldg(q), __ldg(q + HW));
 }
 
-// One 256-bit read-only global load (sm_100: SASS LDG.E.ENL2.256): a lane's 8 channels of a texel in ONE request.
-// The gather is bound by L1 data-pipe wavefronts; two LDG.128 at a 32-byte lane stride each touch every 128-byte
-// line of the texel, one LDG.256 touches it once.  The address must be 32-byte aligned (checked by the C entry points).
+// A lane's 8 channels of a texel: 32 contiguous bytes as two 128-bit read-only loads (LDG.E.128.CONSTANT; Hopper has
+// no 256-bit load).  The entry points keep the 32-byte alignment check so a lane's pair never straddles a sector.
 __device__ __forceinline__ void ldg256(const float4 *__restrict__ p, float4 &lo, float4 &hi) {
 #if defined(PM_EMU)
-    assert((reinterpret_cast<uintptr_t>(p) & 31u) == 0);  // what ld.global.nc.v8.f32 requires
-    lo = p[0];
-    hi = p[1];
-#else
-    asm("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-        : "=f"(lo.x), "=f"(lo.y), "=f"(lo.z), "=f"(lo.w), "=f"(hi.x), "=f"(hi.y), "=f"(hi.z), "=f"(hi.w)
-        : "l"(p));
+    assert((reinterpret_cast<uintptr_t>(p) & 31u) == 0);
 #endif
+    lo = __ldg(p);
+    hi = __ldg(p + 1);
 }
 
 inline bool misaligned32(const void *q) { return (reinterpret_cast<uintptr_t>(q) & 31u) != 0; }
@@ -138,20 +133,10 @@ __device__ __forceinline__ void load_reference(const float *__restrict__ ref_nhw
     r[4] = q1.x * s; r[5] = q1.y * s; r[6] = q1.z * s; r[7] = q1.w * s;
 }
 
-// Packed fp32x2 FMA (Blackwell: SASS FFMA2): two IEEE fp32 fused multiply-adds per issued instruction.  The K-A
-// kernels are bound by issue slots, not by the fp32 pipe, so halving the FFMA count of the head MLP, the blend and
-// the gather dot products buys back issue bandwidth at unchanged numerics.
+// Two IEEE fp32 fused multiply-adds on a pair of lanes of the head MLP, the blend and the gather dot products.  Hopper
+// has no packed fp32x2 FMA, so this is two FFMAs; the pairing keeps the input-major weight layout of MlpParams.
 __device__ __forceinline__ float2 ffma2(const float2 a, const float2 b, const float2 c) {
-#if defined(PM_EMU)
     return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
-#else
-    unsigned long long ra, rb, rc, rd;
-    ra = *reinterpret_cast<const unsigned long long *>(&a);
-    rb = *reinterpret_cast<const unsigned long long *>(&b);
-    rc = *reinterpret_cast<const unsigned long long *>(&c);
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-    return *reinterpret_cast<float2 *>(&rd);
-#endif
 }
 
 // Folded (conv3d 1x1x1 + eval-mode BatchNorm) weights of one G -> 16 -> 8 -> 1 head in the layout the device code
@@ -229,8 +214,7 @@ constexpr int kWarps2 = 4;  // warps per CTA of the third-generation kernel
 
 // ------------------------------------------------------------------------------------------
 // K-A, third generation.  Same three phases as the second, with the profile-driven changes
-// (profiles/r1_run3_ncu.md: phase 1 was 30 % of the issued instructions, the gather loop took 41 % of
-// the stall samples):
+// (phase 1 was a third of the issued instructions, the gather loop took most of the stall samples):
 //   * unique cells are numbered PER PIXEL in "layers" (slot = layer * PPW + pixel) straight from the
 //     ballot mask with one popc -- no shuffle prefix scan; every lane group then gathers the cells of
 //     its OWN pixel, so the reference vector stays in registers (no shared-memory copy of it);
@@ -1132,16 +1116,15 @@ __global__ void __launch_bounds__(256) adaptive_eval_kernel(const EvalParams p) 
 cudaStream_t as_stream(void *s) { return reinterpret_cast<cudaStream_t>(s); }
 
 // ------------------------------------------------------------------------------------------
-// Launch-configuration knobs.  Defaults are the values measured best on B200 (profiles/); a measurement tool
+// Launch-configuration knobs.  Defaults are the values measured best so far; a measurement tool
 // (tools/kbench.py) changes them through pmb200_set_tuning().  Nothing in the launch path reads the environment.
 // ------------------------------------------------------------------------------------------
 enum Tune { kTuneKaGen, kTuneKa3Dc, kTuneKa3DcVw, kTuneKa3Pipe, kTuneKa3MinB, kTuneKa4Nw, kTuneKa4Ctas, kTuneKa4Cap, kTuneKa4Grid,
             kTuneKa4Stages, kTuneKbTp, kTuneKbDy, kTuneStemPpt, kTuneCount };
 const char *const kTuneNames[kTuneCount] = {"ka_gen", "ka3_dc", "ka3_dc_vw", "ka3_pipe", "ka3_minb", "ka4_nw", "ka4_ctas", "ka4_cap",
                                             "ka4_grid", "ka4_stages", "kb_tp", "kb_dy", "stem_ppt"};
-// ka_gen: 3.  Generation 4 (TMA-staged windows) is parity-green on B200 but slower at every bench shape (cold us, gen 3 / gen 4:
-// 47.6 / 91.7, 20.5 / 33.0, 34.3 / 41.0, 37.0 / 49.1 -- profiles/r2_run3_kbench.json; DESIGN.md has the analysis)
-// stem_ppt: 2 (run 19, cold / warm us: 74.4 / 70.9 with 2 pixels per thread, 75.6 / 74.4 with 4: the LDCU : FFMA ratio is not the limiter)
+// ka_gen: 3.  Generation 4 (TMA-staged windows) is parity-green but was slower at every bench shape (DESIGN.md has the analysis)
+// stem_ppt: 2 (4 pixels per thread measured no faster: the LDCU : FFMA ratio is not the limiter)
 const int kTuneDefaults[kTuneCount] = {3, 0, 0, -1, 0, 0, 0, 0, 0, 0, 0, 0, 2};
 int g_tune[kTuneCount] = {3, 0, 0, -1, 0, 0, 0, 0, 0, 0, 0, 0, 2};
 inline int tune(Tune t) { return __atomic_load_n(&g_tune[t], __ATOMIC_RELAXED); }
@@ -1152,8 +1135,7 @@ void launch_wc3(const WarpCorrParams &p, const MlpParams &m, float *sims_out, cu
     const int HW = p.H * p.W;
     constexpr int pix_per_block = kWarps2 * LaneMap<C, G>::PPW;
     dim3 grid((HW + pix_per_block - 1) / pix_per_block, (p.D + DC - 1) / DC, p.B);
-    // measured on B200 with the round-2 kernels (profiles/r2_run3_kbench.json): the plain gather loop wins at every lane map
-    // (C = 32, 8 rows per pass: 34.3 us against 40.8 with the two-deep pipeline, whose 128 registers cost a resident CTA)
+    // the plain gather loop measured faster at every lane map than the two-deep pipeline, whose 128 registers cost a resident CTA
     constexpr int kPipeDefault = 0;
     const int pipe = tune(kTuneKa3Pipe) < 0 ? kPipeDefault : tune(kTuneKa3Pipe);
     if constexpr (EPI == kEpiScore && LaneMap<C, G>::PPW == 8) {
@@ -1555,7 +1537,8 @@ int pmb200_aggregate_views(const float *sims, const float *view_weights, float *
         return fail(PMB200_EINVAL, "aggregate_views: bad size");
     const size_t total = (size_t)B * G * D * H * W;
     size_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    const size_t max_blocks = (size_t)(device_facts().sms > 0 ? device_facts().sms : 1) * 16;
+    if (blocks > max_blocks) blocks = max_blocks;
     aggregate_views_kernel<<<(unsigned)blocks, 256, 0, as_stream(stream)>>>(sims, view_weights, out, V, B, G * D, H * W);
     return launch_status("aggregate_views");
 }
@@ -1644,11 +1627,10 @@ int pmb200_adaptive_eval(const float *score0, const float *depth_sample, const f
     p.B = B; p.D = D; p.H = H; p.W = W; p.K = K; p.dilation = dilation; p.is_inverse = is_inverse;
     p.interval_scale = interval_scale;
     const int HW = H * W;
-    // Block shape from the B200 sweep (profiles/r1_run20_kbench_eval.json): large maps want 32 pixels x few hypothesis
-    // lanes (each thread then walks D/DY hypotheses with the footprints it already decoded), small maps 16 pixels x 16
-    // lanes so that the grid still covers the SMs.
+    // Block shape: large maps want 32 pixels x few hypothesis lanes (each thread then walks D/DY hypotheses with the
+    // footprints it already decoded), small maps 16 pixels x 16 lanes so that the grid still covers every SM twice.
     int TP = 32, DY = D <= 16 ? (D < 4 ? D : 4) : 8;
-    if ((long long)((HW + 31) / 32) * B < 2 * 148) {
+    if ((long long)((HW + 31) / 32) * B < 2LL * device_facts().sms) {
         TP = 16;
         DY = D < 16 ? D : 16;
     }

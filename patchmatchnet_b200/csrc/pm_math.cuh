@@ -1,7 +1,7 @@
 // pm_math.cuh -- per-element arithmetic of the learned-PatchMatch path.
 //
 // Everything here is __host__ __device__ so the same source is (a) inlined into the
-// sm_100a kernels and (b) compiled with g++ into tests/_hostmath.so, where the
+// sm_90a kernels and (b) compiled with g++ into tests/_hostmath.so, where the
 // formulas (not the kernels) are checked against the oracle on the CPU build box.
 // The host build is test infrastructure only; it is never used by the product path.
 #pragma once

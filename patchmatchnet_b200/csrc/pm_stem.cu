@@ -15,8 +15,8 @@
 //     two float4 planes [ch 0-3 | ch 4-7][pixel] (consecutive lanes -> consecutive 16-byte slots: conflict-free LDS.128),
 //     conv1 reads 9 taps x 2 LDS.128 per pixel and writes channels-last [N,H,W,8];
 //   * the input is read as the caller's NCHW planes (coalesced along W): no NCHW -> NHWC conversion pass for the views.
-// Bound: fp32 FFMA issue -- (576 + 1.2 * 216) FFMA per pixel x 1.64 M pixels / (148 SMs x 128 lanes x 1.965 GHz) = 37 us at
-// 100 % issue; HBM traffic 20 MB in + 52 MB out = 11 us.
+// Bound: fp32 FFMA issue -- (576 + 1.2 * 216) FFMA per pixel x 1.64 M pixels / (132 SMs x 128 lanes x 1.98 GHz, H100 SXM)
+// = 41 us at 100 % issue; HBM traffic 20 MB in + 52 MB out = 21 us at the data sheet's 3.35 TB/s.
 #if !defined(PM_EMU)  // host emulation build (tests/warp_emu.h) brings its own CUDA vocabulary
 #include <cuda_runtime.h>
 #endif
@@ -39,7 +39,7 @@ constexpr int kSTW = 32, kSTH = 16;                    // output tile
 constexpr int kHW = kSTW + 2, kHH = kSTH + 2;          // conv0 outputs needed by the tile (conv1's halo)
 constexpr int kIW = kSTW + 4, kIH = kSTH + 4;          // image pixels needed by those
 // Output pixels per thread (PPT): 2 -> 256 threads per CTA, 4 -> 128.  Every weight reaches the FFMA through a uniform register
-// loaded by LDCU.128 (4 weights per load, no direct constant operand on sm_100); a thread's PPT pixels share the load, so PPT
+// loaded by LDCU.128 (4 weights per load); a thread's PPT pixels share the load, so PPT
 // sets the LDCU : FFMA ratio of the conv1 phase (1 : 4 PPT).  pmb200_set_tuning("stem_ppt", 2 | 4) for A/B runs.
 
 struct StemParams {

@@ -1,5 +1,5 @@
 // pm_warpcorr4.cuh -- K-A, fourth generation: the fused warp + correlation kernel as a persistent, warp-specialised
-// pipeline over shared-memory windows staged by the TMA engine (sm_100a).  Included by pm_kernels.cu inside its anonymous
+// pipeline over shared-memory windows staged by the TMA engine (sm_90a).  Included by pm_kernels.cu inside its anonymous
 // namespace, after MlpParams / WarpCorrParams / mlp_eval / ffma2.
 //
 // Reference: models/module.py:130-181 (differentiable_warping), models/patchmatch.py:192-217 (group-wise correlation and

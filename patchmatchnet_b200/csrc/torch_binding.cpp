@@ -32,7 +32,7 @@ void check(int rc, const char *what) {
 }
 
 Tensor dev_f32(const Tensor &t, const char *name, int64_t ndim) {
-    TORCH_CHECK(t.is_cuda(), name, ": the B200 path needs a CUDA tensor (got ", t.device(), "); there is no CPU fallback");
+    TORCH_CHECK(t.is_cuda(), name, ": the H100 path needs a CUDA tensor (got ", t.device(), "); there is no CPU fallback");
     TORCH_CHECK(t.scalar_type() == at::kFloat, name, ": expected float32, got ", t.scalar_type());
     TORCH_CHECK(t.dim() == ndim, name, ": expected ", ndim, " dims, got ", t.dim());
     return t.contiguous();

@@ -8,7 +8,7 @@ Same names, arguments, return values, exception texts and -- byte for byte -- th
     read_bin  data_io.py:165-191      save_bin  data_io.py:194-223
     read_pfm  data_io.py:226-288      save_pfm  data_io.py:291-322
 
-plus the two calls the B200 path itself uses so that a map never passes through a pageable temporary:
+plus the two calls the H100 path itself uses so that a map never passes through a pageable temporary:
 
     read_map_to_device(path, device)   file -> pinned host buffer -> one async copy to the GPU
     save_map_from_device(path, tensor) GPU -> pinned host buffer -> file (row flip / planar order folded into the write)
@@ -123,7 +123,7 @@ def save_pfm(filename: str, image: np.ndarray, scale: float = 1) -> None:
     if image.dtype.name != "float32":
         raise Exception("Image dtype must be float32.")
     if image.dtype.byteorder == ">":
-        raise Exception("big-endian arrays are not supported on the B200 host path")
+        raise Exception("big-endian arrays are not supported on the H100 host path")
     # the library prints "%f" of -scale; keep Python's own sign arithmetic for the written value (int 0 stays "0.000000")
     _write(filename, PFM, image, -float(-scale))
 

@@ -4,16 +4,18 @@
 ``PatchmatchNet.forward`` (cuDNN feature pyramid, the native PatchMatch kernels, refinement) into ONE
 CUDA graph per slot -- the cascade is ~120 short kernels, so at 640x512 launch latency, not bandwidth,
 is the enemy (SURVEY.md 7.3-1) -- runs independent requests concurrently on per-slot streams (most
-kernels of one request launch fewer CTAs than the 148 SMs hold) and moves data with pinned-memory
+kernels of one request launch fewer CTAs than the 132 SMs of an H100 hold) and moves data with pinned-memory
 async copies on a copy stream so uploads overlap compute.
 
     eng = DepthEngine(net, batch=1, n_views=5, height=512, width=640, device="cuda:0")
     depth, confidence = eng.infer(images, intrinsics, extrinsics, depth_min, depth_max)   # host in, host out
 
-There is no CPU path: construction fails without CUDA.
+The stage-3 random initialisation of each request slot draws from the slot's own generator, seeded with ``seed`` + slot
+index, so the same sequence of requests gives the same maps every run.  There is no CPU path: construction fails without CUDA.
 """
 from __future__ import annotations
 
+import contextlib
 from typing import Dict, Sequence, Tuple
 
 import torch
@@ -33,17 +35,22 @@ class DepthEngine:
         use_graph: bool = True,
         warmup: int = 3,
         n_slots: int = 3,
+        seed: int = 0,
     ) -> None:
         if not torch.cuda.is_available():
-            raise RuntimeError("DepthEngine needs a CUDA device (B200); there is no CPU fallback")
+            raise RuntimeError("DepthEngine needs a CUDA device (H100); there is no CPU fallback")
         self.device = torch.device(device)
         self.net = net.eval().to(self.device)
         self.shape = (batch, n_views, height, width)
         B, N, H, W = self.shape
         dev = self.device
-        # One slot = static device inputs + its own compute stream + its own captured graph + pinned host outputs.
+        # One slot = static device inputs + its own compute stream + its own captured graph + pinned host outputs + its own
+        # random generator (seed + slot index) for the stage-3 random initialisation.  A generator's graph-replay state
+        # (seed / offset tensors) is rewritten on the replaying stream at every replay, so slots replaying concurrently from
+        # ONE generator race on it and draw from each other's offsets; with one generator per slot every replay draws
+        # exactly what its slot's sequence of forwards dictates, run after run.
         # Several slots let independent requests overlap on the GPU: most kernels of a 640x512 forward launch far
-        # fewer CTAs than 148 SMs hold, so one request alone cannot fill the machine.
+        # fewer CTAs than 132 SMs hold, so one request alone cannot fill the machine.
         self.n_slots = max(1, int(n_slots))
         self._slots = []
         for _ in range(self.n_slots):
@@ -52,6 +59,7 @@ class DepthEngine:
                 stream=torch.cuda.Stream(device=dev),
                 host_depth=torch.empty(B, 1, H, W).pin_memory(),
                 host_conf=torch.empty(B, H, W).pin_memory(),
+                gen=torch.Generator(device=dev).manual_seed(seed + len(self._slots)),
                 graph=None,
                 outs=None,
             )
@@ -94,9 +102,22 @@ class DepthEngine:
         return 4 * host_pack.numel()
 
     # ------------------------------------------------------------------
+    @contextlib.contextmanager
+    def _draws_from(self, gen: torch.Generator):
+        """PatchMatch stages whose random draw the caller has not pinned (``rand_source``) draw from `gen` meanwhile."""
+        mods = [m for m in self.net.modules() if hasattr(m, "rand_source") and m.rand_source is None]
+        for m in mods:
+            m.rand_source = lambda size, device: torch.rand(size, device=device, generator=gen)
+        try:
+            yield
+        finally:
+            for m in mods:
+                m.rand_source = None
+
     def _forward(self, slot: Dict[str, Tensor]) -> Tuple[Tensor, Tensor]:
         imgs = [slot["images"][i] for i in range(self.shape[1])]
-        depth, conf, _ = self.net(imgs, slot["intrinsics"].clone(), slot["extrinsics"], slot["depth_min"], slot["depth_max"])
+        with self._draws_from(slot["gen"]):
+            depth, conf, _ = self.net(imgs, slot["intrinsics"].clone(), slot["extrinsics"], slot["depth_min"], slot["depth_max"])
         return depth, conf
 
     def set_device_inputs(self, slot_idx: int, images, intrinsics, extrinsics, depth_min, depth_max) -> None:
@@ -121,6 +142,7 @@ class DepthEngine:
             if self.use_graph:
                 for slot in self._slots:
                     g = torch.cuda.CUDAGraph()
+                    g.register_generator_state(slot["gen"])
                     with torch.cuda.graph(g, stream=slot["stream"]):
                         slot["outs"] = self._forward(slot)
                     slot["graph"] = g

@@ -1,7 +1,7 @@
 """Caller-side shell: ``PatchmatchNet`` with the reference constructor / forward
 signatures and parameter names (reference ``models/net.py:125-301``).
 
-Only ``PatchMatch`` (the hot path) is native B200 code.  The dense 2-D convs of
+Only ``PatchMatch`` (the hot path) is native H100 code.  The dense 2-D convs of
 the feature pyramid and the refinement head stay library ops (cuDNN), as the
 scope table (SURVEY.md 8a/8f) says; they are here because the reference's
 ``models/net.py`` does not exist on the GPU box and the end-to-end metric
@@ -113,7 +113,7 @@ class _ConvBnReLU2d(nn.Module):
 
     Training, or CPU: the three ops as written in the reference.  Eval on CUDA: BatchNorm is folded into
     the conv weights (cached) and conv + bias + ReLU run as ONE cuDNN call on channels-last data -- the
-    separate cudnn bn_fw_inf kernel alone was 55 % of the forward's GPU time (profiles/r1_launches_v0.md)."""
+    separate cudnn bn_fw_inf kernel would otherwise be a launch (and a full activation pass) per layer."""
 
     def __init__(self, cin: int, cout: int, k: int = 3, stride: int = 1, pad: int = 1) -> None:
         super().__init__()
@@ -139,7 +139,7 @@ class _ConvBnReLU2d(nn.Module):
         return self._frag_cache.get(srcs, make, key=prec)
 
     def folded_tc5(self, mode: str):
-        """(filter image for the tcgen05 conv in the given form, folded bias)."""
+        """(filter image for the wgmma conv in the given form, folded bias)."""
         from . import ops
 
         bn = self.bn
@@ -459,7 +459,7 @@ class PatchmatchNet(nn.Module):
     ) -> None:
         super().__init__()
         if patchmatch_cls is None:
-            from .patchmatch import PatchMatch as patchmatch_cls  # the B200-native stage
+            from .patchmatch import PatchMatch as patchmatch_cls  # the H100-native stage
         self.stages = 4
         self.feature = FeatureNet()
         self.patchmatch_num_sample = patchmatch_num_sample

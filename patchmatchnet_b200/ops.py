@@ -31,7 +31,7 @@ def _device_guard(t: Tensor):
 
 def _require(t: Tensor, name: str, ndim: Optional[int] = None) -> Tensor:
     if not _on_device(t):
-        raise RuntimeError(f"{name}: the B200 path needs a CUDA tensor (got {t.device}); there is no CPU fallback")
+        raise RuntimeError(f"{name}: the H100 path needs a CUDA tensor (got {t.device}); there is no CPU fallback")
     if t.dtype != torch.float32:
         raise RuntimeError(f"{name}: expected float32, got {t.dtype}")
     if ndim is not None and t.dim() != ndim:
@@ -170,18 +170,15 @@ NATIVE_CONVS_ALL = os.environ.get("PMB200_NATIVE_CONVS", "1") == "all"  # A/B ai
 
 
 def conv_prefers_native(cin: int, cout: int, ks: int) -> bool:
-    """Which implementation runs a small conv in eval mode.  Measured per layer on B200 (profiles/r1_run17_convbench.json,
-    tools/convbench.py): the native channels-last kernel wins on the memory-bound layers -- every 1x1 conv and every
-    layer with at most 3200 multiply-adds per output pixel (full-resolution 3->8 / 8->8 / 8->16 convs, the refinement
-    head, the stage-1 offset conv: 1.2-3.7x faster than the library) -- while the FLOP-heavy 16..64-channel 3x3 / 5x5
-    layers stay with cuDNN, whose tcgen05 implicit-GEMM kernels reach 100-150 TFLOP/s there against ~50 for the
-    legacy mma.sync path this kernel issues (measured peak of that path: ~245 TFLOP/s TF32)."""
+    """Which implementation runs a small conv in eval mode (per-layer timings: tools/convbench.py).  The native
+    channels-last kernel takes the memory-bound layers -- every 1x1 conv and every layer with at most 3200 multiply-adds
+    per output pixel (full-resolution 3->8 / 8->8 / 8->16 convs, the refinement head, the stage-1 offset conv) -- while in
+    the TF32 mode the FLOP-heavy 16..64-channel 3x3 / 5x5 layers stay with cuDNN's implicit-GEMM kernels."""
     if not NATIVE_CONVS:
         return False
     # fp32-accurate mode (cudnn.allow_tf32 off): the library's fp32 kernels for the FLOP-bound layers do not use the tensor
-    # cores at all (value_fp32 of profiles/r2_run1_bench.json: 2.62 ms per forward against 0.755), the native 3xTF32 kernel
-    # does -> every conv native.  The parity configuration and the bench default are this mode (the depth maps of the TF32
-    # mode are 2.6e-3 .. 3.3e-3 off the fp32 reference, outside north_star's 1e-3: tests/test_gpu_bench_mode.py).
+    # cores at all, the native 3xTF32 kernels do -> every conv native.  The parity configuration and the bench default are
+    # this mode (the depth maps of the TF32 mode are outside north_star's 1e-3: tests/test_gpu_bench_mode.py).
     return NATIVE_CONVS_ALL or conv_precision() == 3 or ks == 1 or cin * cout * ks * ks <= 3200
 
 
@@ -231,21 +228,20 @@ def pack_conv_filter(weight: Tensor, precision: int, transposed: bool = False) -
     return torch.cat((hi, lo), dim=-1).contiguous().view(-1)
 
 
-# K-D5 (csrc/pm_conv5.cu): tcgen05 / TMEM / TMA implicit-GEMM convolution, fp32-accurate (3xTF32).  Used in the
+# K-D5 (csrc/pm_conv5.cu): wgmma / TMA implicit-GEMM convolution, fp32-accurate (3xTF32).  Used in the
 # fp32-accurate mode for the layers it serves when TC5_CONVS is on (PMB200_TC5=0 hands them back to the mma.sync kernel).
 TC5_CONVS = os.environ.get("PMB200_TC5", "1") != "0"
 
 
-# (Cin, Cout, KS, stride) of the layers a tcgen05 form beats the mma.sync kernel's 3xTF32 mode on (cold us per launch at the
-# 640x512 sizes, tools/convbench.py, profiles/r2_run16_convbench.json).  Per-tap form K-D5 (the only one for stride 2):
-# conv5 70 vs 93, conv8 50 vs 63; it loses on conv2 (137 vs 91: Cin = 8, one K slice per tap).  PMB200_TC5=all takes every
-# supported layer (A/B measurements), PMB200_TC5=0 none.
+# (Cin, Cout, KS, stride) of the layers a wgmma form serves instead of the mma.sync kernel's 3xTF32 mode (cold time per launch
+# at the 640x512 sizes: tools/convbench.py).  Per-tap form K-D5 (the only one for stride 2): the 16->32 and 32->64 5x5 stride-2
+# layers; not conv2 (Cin = 8: one K slice per tap, the instruction count is the cost).  PMB200_TC5=all takes every supported
+# layer (A/B measurements), PMB200_TC5=0 none.
 TC5_LAYERS = {(16, 32, 5, 2), (32, 64, 5, 2)}
 TC5_ALL = os.environ.get("PMB200_TC5", "1") == "all"
 # Stride-1 layers served by the halo-tile form K-D5h (one TMA box + one split per output tile, taps as shifted descriptors,
-# [w_hi | w_lo] as one operand): mma.sync 3xTF32 -> K-D5h, cold us: conv3/4 58 -> 36, conv6/7 67 -> 29, conv9/10 47 -> 29,
-# output2 27 -> 25, output3 77 -> 44, stage-3 offset convs 39 / 40 -> 17 / 18, stage-2 25 / 27 -> 18 / 21, stage-1 32 -> 30.
-# It loses where Cin = 8 (conv1 93 vs 70: one K slice per tap, the instruction count is the cost) and ties on Refinement.
+# [w_hi | w_lo] as one operand): FeatureNet conv3/4, conv6/7, conv9/10, output2/3 and the offset convs of every stage.  Not
+# where Cin = 8 (conv1: one K slice per tap, the instruction count is the cost) nor Refinement.
 # PMB200_TC5H=all: every stride-1 layer the kernel takes (A/B measurements); =0: none.
 TC5H_LAYERS = {(16, 16, 3, 1), (32, 32, 3, 1), (64, 64, 3, 1), (64, 32, 1, 1), (64, 16, 1, 1),
                (64, 32, 3, 1), (64, 18, 3, 1), (32, 16, 3, 1), (32, 18, 3, 1), (16, 18, 3, 1)}
@@ -254,7 +250,7 @@ TC5H_OFF = os.environ.get("PMB200_TC5H", "1") == "0"
 
 
 def conv_tc5_mode(cin: int, cout: int, ks: int, stride: int = 1, transposed: bool = False, fused_add: bool = False) -> str:
-    """"" (mma.sync kernel), "halo" (K-D5h) or "tap" (K-D5): which tcgen05 form, if any, runs this conv.  Only in the
+    """"" (mma.sync kernel), "halo" (K-D5h) or "tap" (K-D5): which wgmma form, if any, runs this conv.  Only in the
     fp32-accurate mode (the arithmetic of both IS the 3xTF32 split), never with a fused transposed / upsample-add epilogue, and
     only for layers on the measured lists above."""
     if not (NATIVE_CONVS and TC5_CONVS) or transposed or fused_add or conv_precision() != 3:
@@ -280,7 +276,7 @@ def pack_conv_filter_tc5_for(weight: Tensor, mode: str) -> Tensor:
 def pack_conv_filter_tc5(weight: Tensor) -> Tensor:
     """Conv filter [Cout,Cin,KS,KS] -> the shared-memory image `pmb200_conv2d_tc5` copies per tap (include/patchmatch_b200.h):
     [tap][Cin/32 blocks][2 Npad rows][min(Cin,32) channels], rows 0..Npad-1 = w_hi (TF32-rounded weight), Npad..2Npad-1 = w_lo
-    (TF32-rounded remainder) -- ONE K-major tcgen05 operand of N = 2 Npad whose first Npad rows double as the N = Npad operand --
+    (TF32-rounded remainder) -- ONE K-major wgmma operand of N = 2 Npad whose first Npad rows double as the N = Npad operand --
     in the swizzle of the tensor core for its row size.  Pure layout / rounding work on the weight's device (CPU-testable)."""
     if weight.dim() != 4 or weight.shape[2] != weight.shape[3]:
         raise RuntimeError(f"pack_conv_filter_tc5: expected [Cout,Cin,KS,KS], got {tuple(weight.shape)}")
@@ -309,7 +305,7 @@ def pack_conv_filter_tc5(weight: Tensor) -> Tensor:
 
 def pack_conv_filter_tc5h(weight: Tensor) -> Tensor:
     """Conv filter [Cout,Cin,KS,KS] -> the image `pmb200_conv2d_tc5h` streams per tap: [tap][Cin/4 chunks][2 Npad rows][4 floats],
-    rows 0..Npad-1 = w_hi, Npad..2Npad-1 = w_lo: ONE tcgen05 operand of N = 2 Npad (a_hi x [w_hi | w_lo] is a single MMA), whose
+    rows 0..Npad-1 = w_hi, Npad..2Npad-1 = w_lo: ONE wgmma operand of N = 2 Npad (a_hi x [w_hi | w_lo] is a single MMA), whose
     first Npad rows double as the N = Npad operand of a_lo x w_hi.  No swizzle: 8 rows of one chunk are one core matrix."""
     if weight.dim() != 4 or weight.shape[2] != weight.shape[3]:
         raise RuntimeError(f"pack_conv_filter_tc5h: expected [Cout,Cin,KS,KS], got {tuple(weight.shape)}")
@@ -826,7 +822,7 @@ def fuse_points(final_mask: Tensor, depth_averaged: Tensor, ref_img: Tensor, cam
     final_mask bool / uint8 [H,W], depth_averaged float64 [H,W] (as geometric_filter returns them), ref_img float32
     [H,W,3] in [0,1].  One host synchronisation at the end (the vertex count sizes the result)."""
     if not _on_device(final_mask) or not _on_device(depth_averaged) or not _on_device(ref_img):
-        raise RuntimeError("fuse_points: the B200 path needs CUDA tensors; there is no CPU fallback")
+        raise RuntimeError("fuse_points: the H100 path needs CUDA tensors; there is no CPU fallback")
     H, W = depth_averaged.shape
     if depth_averaged.dtype != torch.float64 or tuple(final_mask.shape) != (H, W) or tuple(ref_img.shape) != (H, W, 3) or ref_img.dtype != torch.float32:
         raise RuntimeError("fuse_points: final_mask [H,W], depth_averaged float64 [H,W], ref_img float32 [H,W,3]")

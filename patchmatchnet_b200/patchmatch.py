@@ -1,4 +1,4 @@
-"""B200-native ``PatchMatch``: drop-in for reference ``models/patchmatch.py:242-529``.
+"""H100-native ``PatchMatch``: drop-in for reference ``models/patchmatch.py:242-529``.
 
 Same constructor, same ``forward`` signature and return triple, same parameter /
 buffer names and shapes (the reference checkpoints load with every key matched),
@@ -8,7 +8,7 @@ same error behaviour (``assert`` on view/matrix count mismatch,
 What runs where (per PatchMatch iteration; DESIGN.md has the byte budgets):
 
     propa_conv / eval_conv, the three 1x1x1 MLP heads ... cuDNN (library ops, as the scope says)
-    everything else ..................................... five hand-written sm_100a kernels
+    everything else ..................................... five hand-written sm_90a kernels
         K-C  init_propagate   hypothesis init + neighbour gather + sort          (a8, a9, a7)
         K-A  warp_corr        warp + bilinear gather + group correlation
                               + view-weighted aggregation, all views, one launch (a1, a2, a3)
@@ -61,7 +61,7 @@ def _offset_conv(conv: nn.Conv2d, x: Tensor, native: bool) -> Tensor:
             cached = (stamp, (pack, conv.bias.detach().clone()))
         _FOLD_CACHE[conv] = cached
     frag, bias = cached[1]
-    if tc5:  # tcgen05 implicit GEMM (csrc/pm_conv5.cu); its channels-last output is consumed in place like the other's
+    if tc5:  # wgmma implicit GEMM (csrc/pm_conv5.cu); its channels-last output is consumed in place like the other's
         return ops.conv2d_tc5(x, frag, bias, conv.out_channels, conv.kernel_size[0], 1, conv.padding[0], conv.dilation[0], halo=tc5 == "halo")
     return ops.conv2d_nhwc(x, frag, bias, conv.out_channels, conv.kernel_size[0], 1, conv.padding[0], conv.dilation[0])
 
@@ -417,7 +417,7 @@ class PatchMatch(nn.Module):
             ), "Patchmatch Evaluation: Different number of images and view weights"
         if not ops._on_device(ref_feature):
             raise RuntimeError(
-                "patchmatchnet_b200.PatchMatch runs on CUDA (sm_100a) only; there is no CPU fallback "
+                "patchmatchnet_b200.PatchMatch runs on CUDA (sm_90a) only; there is no CPU fallback "
                 f"(got a tensor on {ref_feature.device})"
             )
         # autograd is needed when anything upstream or any parameter can receive a gradient

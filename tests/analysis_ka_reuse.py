@@ -1,6 +1,6 @@
 """K-A gather statistics on the REAL hypotheses of a 640x512 cascade (analysis script, CPU only, not a test):
 
-    python tests/analysis_ka_reuse.py > profiles/r1_ka_gather_stats.json
+    python tests/analysis_ka_reuse.py > ka_gather_stats.json
 
 For every K-A launch of one forward (hypotheses, projections captured from the oracle port of the reference running the
 synthetic 1+4-view input with the shipped checkpoint) it reports, for the kernel's (pixels per warp, rows per pass):

@@ -1,6 +1,6 @@
 """K-A gen-4 design aid (analysis script, CPU only, not a test): source-window statistics of reference-pixel tiles.
 
-    python tests/analysis_ka_window.py > profiles/r2_ka_window_stats.json
+    python tests/analysis_ka_window.py > ka_window_stats.json
 
 For every K-A launch of one 640x512 forward (hypotheses / projections captured from the oracle port running the synthetic
 1+4-view input with the shipped checkpoint) and for several (tile, hypothesis rows per item) decompositions it reports,

@@ -11,7 +11,7 @@ Every conv of the network (oracle port of the reference behind the repo's shell,
     3x          a_hi.w_hi + a_hi.w_lo + a_lo.w_hi            (pm_conv.cu precision 3)
 "native" layers = ops.conv_prefers_native's rule (memory-bound), "library" layers = the FLOP-bound ones.
 
-    python tests/analysis_tf32_modes.py > profiles/r2_tf32_modes.json
+    python tests/analysis_tf32_modes.py > tf32_modes.json
 """
 import json
 import os

@@ -11,14 +11,13 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if REPO not in sys.path:
     sys.path.insert(0, REPO)
 GOLDEN = os.path.join(REPO, "tests", "golden")
-REFERENCE = "/root/reference"
 
 warnings.filterwarnings("ignore", message="torch.meshgrid")
 warnings.filterwarnings("ignore", message=".*torch.jit.*is deprecated.*")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -48,18 +47,6 @@ def golden_net_case():
 @pytest.fixture(scope="session")
 def golden_config1():
     return torch.load(os.path.join(GOLDEN, "config1_case.pt"), map_location="cpu")
-
-
-@pytest.fixture(scope="session")
-def reference_models():
-    """The unmodified reference, importable only in the build container."""
-    if not os.path.isdir(os.path.join(REFERENCE, "models")):
-        pytest.skip("/root/reference not present (GPU box): oracle is pinned by the golden fixtures instead")
-    sys.path.insert(0, REFERENCE)
-    import models.net as ref_net
-    import models.patchmatch as ref_pm
-    import models.module as ref_mod
-    return ref_net, ref_pm, ref_mod
 
 
 @pytest.fixture(scope="session")

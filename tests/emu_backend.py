@@ -104,7 +104,7 @@ class EmulatedLibrary:
                                                    d_fw, B, D, H, W, K, dilation, scale, inverse)
 
     def pmb200_conv2d_tc5_supported(self, cin, cout, ks, stride):
-        return 0  # tcgen05 / TMEM has no emulation: the convs take the mma.sync kernel here, K-D5 is checked on the GPU only
+        return 0  # wgmma has no emulation: the convs take the mma.sync kernel here, K-D5 is checked on the GPU only
 
     def pmb200_conv2d_filter_floats(self, cin, cout, ks, prec):
         return self.conv.emu_conv2d_filter_floats(cin, cout, ks, prec)

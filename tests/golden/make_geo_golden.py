@@ -1,8 +1,8 @@
 """Generate tests/golden/geo_case.npz from the UNMODIFIED reference's geometric-consistency code.
 
-Run in the build container only (needs /root/reference and cv2):
+Needs a checkout of the reference (FangjinhuaWang/PatchmatchNet) and cv2:
 
-    python tests/golden/make_geo_golden.py
+    python tests/golden/make_geo_golden.py <path to the reference checkout>
 
 `eval.py` itself cannot be imported here (it imports `plyfile`, which is absent), so the two functions are executed from
 its own source text -- `reproject_with_depth` and `check_geometric_consistency`, eval.py:86-190, byte for byte -- and
@@ -21,7 +21,9 @@ REPO = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, REPO)
 from tests import geo_cases  # noqa: E402
 
-src = open("/root/reference/eval.py").read()
+if len(sys.argv) != 2:
+    raise SystemExit(__doc__)
+src = open(os.path.join(sys.argv[1], "eval.py")).read()
 ns = {"np": np, "cv2": cv2, "Tuple": Tuple}
 exec(src[src.index("def reproject_with_depth("):src.index("def filter_depth(")], ns)
 

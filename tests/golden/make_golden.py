@@ -1,8 +1,8 @@
 """Generate the golden fixtures in this directory from the UNMODIFIED reference.
 
-Run in the build container only (needs /root/reference, which does not exist on the GPU box):
+Needs a checkout of the reference (FangjinhuaWang/PatchmatchNet), checkpoints included:
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py <path to the reference checkout>
 
 Writes
     weights_000007.pt   the reference's shipped weights (checkpoints/params_000007.ckpt["model"],
@@ -24,7 +24,10 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, REPO)
-sys.path.insert(0, "/root/reference")
+if len(sys.argv) != 2:
+    raise SystemExit(__doc__)
+REFERENCE = os.path.abspath(sys.argv[1])
+sys.path.insert(0, REFERENCE)
 warnings.filterwarnings("ignore")
 
 from models.net import PatchmatchNet as RefNet  # noqa: E402
@@ -35,7 +38,7 @@ from tests import pm_cases  # noqa: E402
 
 def main() -> None:
     torch.set_num_threads(8)
-    ck = torch.load("/root/reference/checkpoints/params_000007.ckpt", map_location="cpu", weights_only=False)["model"]
+    ck = torch.load(os.path.join(REFERENCE, "checkpoints", "params_000007.ckpt"), map_location="cpu", weights_only=False)["model"]
     weights = {k[len("module."):]: v.clone() for k, v in ck.items()}
     torch.save(weights, os.path.join(HERE, "weights_000007.pt"))
 

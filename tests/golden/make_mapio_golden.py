@@ -1,8 +1,8 @@
 """Generate tests/golden/maps/* with the UNMODIFIED reference's map writers (datasets/data_io.py save_pfm / save_bin) and
 record what its readers return (read_pfm / read_bin) in tests/golden/maps/expected.npz.
 
-Run in the build container only (imports /root/reference):  python tests/golden/make_mapio_golden.py
-The files travel to the GPU box, where /root/reference does not exist."""
+Needs a checkout of the reference (FangjinhuaWang/PatchmatchNet):
+    python tests/golden/make_mapio_golden.py <path to the reference checkout>"""
 import os
 import sys
 
@@ -10,7 +10,9 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(HERE, "maps")
-sys.path.insert(0, "/root/reference")
+if len(sys.argv) != 2:
+    raise SystemExit(__doc__)
+sys.path.insert(0, os.path.abspath(sys.argv[1]))
 from datasets import data_io as ref  # noqa: E402
 
 os.makedirs(OUT, exist_ok=True)

@@ -105,3 +105,13 @@ def rel_l1(a: torch.Tensor, b: torch.Tensor) -> float:
     """north_star's metric: sum|a-b| / sum|b|."""
     a, b = a.detach().double().cpu(), b.detach().double().cpu()
     return float((a - b).abs().sum() / b.abs().sum().clamp_min(1e-30))
+
+
+def warp_case_inputs(B, H, W):
+    """Seeded depth planes (the first one behind the camera) and learned-offset maps for the warping / sampling-grid
+    comparison with the reference (tests/test_oracle_vs_reference.py, tests/golden/make_reference_vectors.py)."""
+    g = torch.Generator().manual_seed(7)
+    depth = 400.0 + 600.0 * torch.rand(B, 5, H, W, generator=g)
+    depth[:, 0] = -50.0  # behind the camera -> exactly zero
+    offsets = {kind: torch.randn(B, 2 * count, H * W, generator=g) for kind, count in (("propagation", 16), ("evaluation", 9))}
+    return depth, offsets

@@ -72,21 +72,6 @@ def test_error_conventions_cpu():
             PatchMatch(evaluate_neighbors=10)(**kw)
 
 
-def test_drops_into_unmodified_reference_net(reference_models, golden_weights, monkeypatch):
-    """models/net.py binds PatchMatch by name at import (net.py:6); rebinding that one name swaps the hot path."""
-    ref_net, _, _ = reference_models
-    monkeypatch.setattr(ref_net, "PatchMatch", PatchMatch)
-    net = ref_net.PatchmatchNet(**pm_cases.NET_KWARGS)
-    assert all(type(getattr(net, f"patchmatch_{i}")) is PatchMatch for i in (1, 2, 3))
-    missing, unexpected = net.load_state_dict(golden_weights, strict=True)
-    assert not missing and not unexpected
-    net.eval()
-    inp = pm_cases.make_net_inputs(pm_cases.NET_CASE)
-    with torch.no_grad(), pytest.raises(RuntimeError, match="no CPU fallback"):
-        # FeatureNet (reference code) runs; the first PatchMatch call refuses the CPU tensors
-        net(inp["images"], inp["intrinsics"], inp["extrinsics"], inp["depth_min"], inp["depth_max"])
-
-
 def test_zero_copy_view_detection_needs_one_storage():
     """Back-to-back addresses are not enough (the caching allocator can place separate tensors adjacently):
     the zero-copy re-view is only taken for views of ONE storage."""

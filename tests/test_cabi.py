@@ -52,12 +52,12 @@ def test_ctypes_signatures_have_the_headers_parameter_counts():
         assert len(args) == counts[name], f"{name}: ctypes binding has {len(args)} parameters, the header declares {counts[name]}"
 
 
-def test_library_is_sm100a_only():
+def test_library_is_sm90a_only():
     import subprocess
 
     out = subprocess.run(["cuobjdump", "--list-elf", _native.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
-    assert not re.search(r"sm_(?!100a)\d+", out), out
+    assert "sm_90a" in out
+    assert not re.search(r"sm_(?!90a)\d+", out), out
 
 
 def test_abi_version_and_errors_without_gpu(lib):

@@ -200,7 +200,7 @@ TC5_LAYERS = sorted(n for n, (cin, cout, ks, S, pad, dil, relu) in LAYERS.items(
 def test_tc5_filter_image_matches_the_address_swizzle():
     """ops.pack_conv_filter_tc5 against the element-by-element definition in include/patchmatch_b200.h: byte offset `off` of
     the dense [Npad][row bytes] tile moves to off ^ ((off >> 3) & mask), mask 0x70 / 0x30 / 0x10 for 128 / 64 / 32-byte rows
-    (what TMA writes and tcgen05 reads for a K-major operand); hi + lo restores the weight to 2^-22."""
+    (what TMA writes and wgmma reads for a K-major operand); hi + lo restores the weight to 2^-22."""
     torch.manual_seed(0)
     for (cout, cin, ks) in [(16, 8, 5), (18, 32, 3), (64, 64, 3), (8, 16, 3), (32, 16, 5), (64, 64, 1)]:
         w = torch.randn(cout, cin, ks, ks)
@@ -230,7 +230,7 @@ def test_tc5_filter_image_matches_the_address_swizzle():
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", TC5_LAYERS)
 def test_gpu_tc5_conv_matches_cudnn_fp32(name, fp32_library):
-    """K-D5 (tcgen05 / TMEM / TMA implicit GEMM, 3xTF32) against cuDNN in full fp32: every layer shape it can take, ragged
+    """K-D5 (wgmma / TMA implicit GEMM, 3xTF32) against cuDNN in full fp32: every layer shape it can take, ragged
     map sizes (partial tiles on both axes, zero padding from the TMA's out-of-bounds fill), two images, strides 1 and 2,
     dilation up to 6, output channels that are not a multiple of 16."""
     cin, cout, ks, S, pad, dil, relu = LAYERS[name]

@@ -94,7 +94,7 @@ def test_emulated_source_matches_conv2d(emu_conv, name):
 @pytest.mark.parametrize("name", ["feature.conv0", "feature.conv1", "feature.conv2", "feature.conv3", "feature.conv9", "stage1.eval_conv"])
 def test_emulated_persistent_double_buffered_path(emu_conv, name, monkeypatch):
     """On a pretend 1-SM device the planner gives the same small map several tiles per CTA and two halo buffers: the
-    persistent loop with the next tile's prefetch in flight (what every full-size layer runs on the B200)."""
+    persistent loop with the next tile's prefetch in flight (what every full-size layer runs on the GPU)."""
     monkeypatch.setenv("PM_EMU_SMS", "1")
     cin, cout, ks, S, pad, dil, relu = LAYERS[name]
     g = torch.Generator().manual_seed(sum(map(ord, name)) + 1)

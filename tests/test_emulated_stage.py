@@ -105,37 +105,6 @@ def test_native_network_on_emulated_kernels_matches_oracle(backend, golden_weigh
     assert n.get("pmb200_conv_stem") == 1 and n.get("pmb200_refine_low") == 1 and n.get("pmb200_refine_full") == 1, n
 
 
-def test_drop_in_executes_inside_the_unmodified_reference_net(backend, golden_weights, golden_net_case, reference_models, monkeypatch):
-    """The drop-in, EXECUTED: the reference's own `models/net.py` (unmodified, from /root/reference) builds its
-    PatchmatchNet with `PatchMatch` rebound to this package's class, loads the shipped checkpoint with every key matched,
-    and runs a full forward -- the reference's FeatureNet, stage glue and Refinement around three native PatchMatch stages
-    (real host code, every hand-written kernel under the emulator) -- and the result is compared with what the unmodified
-    reference produced for the same input (tests/golden/net_case.pt).  (VERDICT r1, missing #6.)"""
-    ref_net, ref_pm, _ = reference_models
-    monkeypatch.setattr(torch.backends.cudnn, "allow_tf32", False)  # native offset convs in the fp32-accurate mode
-    monkeypatch.setattr(ref_net, "PatchMatch", PatchMatch)  # net.py binds the name at import (net.py:6): rebind it there
-    net = ref_net.PatchmatchNet(**pm_cases.NET_KWARGS)
-    assert all(type(getattr(net, f"patchmatch_{i}")) is PatchMatch for i in (1, 2, 3))
-    missing, unexpected = net.load_state_dict(golden_weights, strict=True)
-    assert not missing and not unexpected
-    net.eval()
-    inp = pm_cases.make_net_inputs(pm_cases.NET_CASE)
-    assert pm_cases.checksum(inp) == golden_net_case["checksum"]
-    net.patchmatch_3.rand_source = lambda size, device: inp["rand48"]  # the draw the reference made for the fixture
-    with torch.no_grad():
-        depth, conf, per_stage = net(inp["images"], inp["intrinsics"], inp["extrinsics"], inp["depth_min"], inp["depth_max"])
-    assert depth.shape == golden_net_case["depth"].shape
-    assert pm_cases.rel_l1(depth, golden_net_case["depth"]) <= 2e-4
-    for s, ds in golden_net_case["per_stage"].items():
-        assert len(per_stage[s]) == len(ds)
-        for x, y in zip(per_stage[s], ds):
-            assert pm_cases.rel_l1(x, y) <= 2e-4
-    assert float((conf - golden_net_case["confidence"]).abs().mean()) <= 1e-3
-    n = backend.calls  # the native path ran (not a torch re-implementation): 5 fused warp+correlation launches, 5 K-B, 5 K-C
-    assert n.get("pmb200_warp_corr_score") == 4 and n.get("pmb200_warp_corr_view_weights") == 1
-    assert n.get("pmb200_adaptive_eval") == 5 and n.get("pmb200_init_propagate") == 5 and n.get("pmb200_conv2d_nhwc", 0) >= 5
-
-
 # ------------------------------------------------------------------------------------------------
 # training configuration: native forward + native backward kernels behind patchmatchnet_b200.autograd, on the CPU box
 # ------------------------------------------------------------------------------------------------

@@ -1,5 +1,5 @@
 """The oracle against the committed golden fixtures (generated from the unmodified reference by
-tests/golden/make_golden.py).  Runs everywhere, including the GPU box where /root/reference is absent.
+tests/golden/make_golden.py).  Needs nothing outside this repository.
 Same torch build + CPU => the comparison is tight (1e-6 relative; it is bit-exact in the build box)."""
 import pytest
 import torch

@@ -88,25 +88,6 @@ def test_scripted_module_is_inference_only(golden_weights):
         sm(*kw)
 
 
-def test_unmodified_reference_net_scripts_with_the_rebind(reference_models, golden_weights, monkeypatch, tmp_path):
-    """Exactly what train.py:50-55 does, with models.net.PatchMatch rebound: eval(), torch.jit.script, save; then
-    eval.py:38's torch.jit.load."""
-    ref_net, _, _ = reference_models
-    monkeypatch.setattr(ref_net, "PatchMatch", PatchMatch)
-    net = ref_net.PatchmatchNet(**pm_cases.NET_KWARGS)
-    net.load_state_dict(golden_weights, strict=True)
-    net.eval()
-    sm = torch.jit.script(net)
-    path = str(tmp_path / "module_000007.pt")
-    sm.save(path)
-    back = torch.jit.load(path)
-    assert "pmb200::warp_corr_score_" in str(back.patchmatch_3._forward_script.graph)
-    assert set(back.state_dict()) == set(golden_weights)
-    inp = pm_cases.make_net_inputs(pm_cases.NET_CASE)
-    with torch.no_grad(), pytest.raises(Exception):  # FeatureNet runs; the first pmb200 op has no CPU backend
-        back(inp["images"], inp["intrinsics"], inp["extrinsics"], inp["depth_min"], inp["depth_max"])
-
-
 # ----------------------------------------------------------------------------------------------------------------
 def _stage_kwargs(case):
     return [

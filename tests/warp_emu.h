@@ -324,11 +324,11 @@ using std::min;
 inline cudaError_t cudaGetLastError() { return cudaSuccess; }
 inline const char *cudaGetErrorString(cudaError_t) { return "emulated"; }
 inline cudaError_t cudaGetDevice(int *dev) { *dev = 0; return cudaSuccess; }
-// the launch planner sizes persistent grids from the SM count: 148 (B200) unless PM_EMU_SMS says otherwise -- a tiny "GPU"
+// the launch planner sizes persistent grids from the SM count: 132 (H100) unless PM_EMU_SMS says otherwise -- a tiny "GPU"
 // makes small test maps run the multi-tile, double-buffered paths
 inline cudaError_t cudaDeviceGetAttribute(int *v, cudaDeviceAttr, int) {
     const char *e = getenv("PM_EMU_SMS");
-    *v = (e && atoi(e) > 0) ? atoi(e) : 148;
+    *v = (e && atoi(e) > 0) ? atoi(e) : 132;
     return cudaSuccess;
 }
 template <typename F>

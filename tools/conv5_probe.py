@@ -1,4 +1,4 @@
-"""One layer through the tcgen05 convs (both forms) and the mma.sync 3xTF32 conv, a few launches each: the target of an
+"""One layer through the wgmma convs (both forms) and the mma.sync 3xTF32 conv, a few launches each: the target of an
 `ncu -k regex:conv5 --set full --import-source on` capture.
 
     python tools/conv5_probe.py N cin cout ks stride pad dil h w

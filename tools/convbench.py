@@ -1,7 +1,7 @@
 """Per-layer micro-benchmark of the native channels-last tensor-core conv (csrc/pm_conv.cu) against the cuDNN call it
 replaces, at the sizes of one 640x512 1+4-view forward (5 stacked views through FeatureNet, 1 view through the rest).
 
-    python tools/convbench.py > gpurun_out/convbench.json
+    python tools/convbench.py > convbench.json
 
 cold = L2 flushed before each launch (CUDA events on the launching stream), warm = 10 back-to-back launches.
 GB/s = (input + output activation bytes) / cold time: the traffic a perfectly fused layer must move.
@@ -105,7 +105,7 @@ for (name, N, cin, cout, ks, S, pad, dil, relu, h, w) in LAYERS:
                 row["native_tf32_gbs"] = round(act_bytes / (c * 1e-6) / 1e9, 1)
                 row["native_tf32_tflops"] = round(flops / (c * 1e-6) / 1e12, 2)
                 row["speedup_vs_cudnn_cold"] = round(row["cudnn_tf32_us"]["cold"] / c, 2)
-    if cin in (8, 16, 32, 64):  # K-D5: tcgen05 implicit GEMM, 3xTF32 (fp32-accurate) -- compare with native_p3
+    if cin in (8, 16, 32, 64):  # K-D5: wgmma implicit GEMM, 3xTF32 (fp32-accurate) -- compare with native_p3
         try:
             f5 = ops.pack_conv_filter_tc5(wt)
             c, cmin, wm = timeit(lambda: ops.conv2d_tc5(x, f5, b, cout, ks, S, pad, dil, relu=relu))

@@ -1,6 +1,6 @@
 """Geometric-consistency filtering (SURVEY.md 8f row f4): the one-launch kernel vs the reference algorithm on the host CPU.
 
-    python tools/geobench.py > gpurun_out/geobench.json
+    python tools/geobench.py > geobench.json
 
 GPU: CUDA events on the launching stream, L2 flushed before each launch, depth maps resident; `e2e` additionally uploads
 the (1 + V) depth maps + confidence from pinned host memory and downloads the three masks + averaged depth every call.

@@ -2,7 +2,7 @@
 hypotheses have the cascade's real clustering) and time each one in isolation -- L2 flushed, CUDA events --
 for a sweep of kernel variants selected through environment variables (read per call by libpmb200.so).
 
-    python tools/kbench.py > gpurun_out/kbench.json
+    python tools/kbench.py > kbench.json
 """
 import itertools
 import json

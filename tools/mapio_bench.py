@@ -1,8 +1,8 @@
 """Host-side timing of the depth-map file I/O (SURVEY.md 8f row f5): native (libpmb200.so via patchmatchnet_b200.data_io)
-against the unmodified reference functions (datasets/data_io.py, when /root/reference is present) on the same arrays, in
+against the unmodified reference functions (datasets/data_io.py of a reference checkout given with --reference) on the same arrays, in
 the same tmpfs directory.  Host code only -- no GPU involved; prints one JSON object.
 
-    python tools/mapio_bench.py [--height 1184 --width 1600 --repeat 5]"""
+    python tools/mapio_bench.py [--height 1184 --width 1600 --repeat 5] [--reference <checkout>]"""
 import argparse
 import json
 import os
@@ -31,10 +31,11 @@ def main():
     ap.add_argument("--height", type=int, default=1184)
     ap.add_argument("--width", type=int, default=1600)
     ap.add_argument("--repeat", type=int, default=5)
+    ap.add_argument("--reference", default=None, help="checkout of the reference project to time against")
     args = ap.parse_args()
     ref = None
-    if os.path.isdir("/root/reference/datasets"):
-        sys.path.insert(0, "/root/reference")
+    if args.reference:
+        sys.path.insert(0, os.path.abspath(args.reference))
         from datasets import data_io as ref  # noqa: E402
     rng = np.random.default_rng(0)
     arr = rng.uniform(425, 935, size=(args.height, args.width)).astype(np.float32)

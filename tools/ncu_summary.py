@@ -1,6 +1,6 @@
 """Summarise an `ncu --set full` report into a markdown table incl. the top warp-stall reasons.
 
-    python tools/ncu_summary.py gpurun_out/x.ncu-rep "title" profiles/out.md
+    python tools/ncu_summary.py x.ncu-rep "title" out.md
 """
 import csv
 import io

@@ -1,7 +1,7 @@
 """Static instruction budget of one kernel: SASS instructions attributed to source lines (needs -lineinfo).
 
     cuobjdump -xelf all patchmatchnet_b200/libpmb200.so        (in a scratch directory)
-    nvdisasm -g pm_kernels.sm_100a.cubin > pmk.sass
+    nvdisasm -g pm_kernels.sm_90a.cubin > pmk.sass
     python tools/sass_lines.py pmk.sass 'warp_corr3_kernelILi32ELi8ELi2ELi8ELi1ELi4E' [--ranges 700-733:phase1,...]
 
 Counts are STATIC (one per SASS instruction, loops not weighted); inlined callee lines are reported with the innermost

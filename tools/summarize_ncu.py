@@ -1,6 +1,6 @@
 """Summarise an `ncu --set full` report (.ncu-rep) into a markdown table + a traffic JSON for bench.py.
 
-    python tools/summarize_ncu.py gpurun_out/native_full.ncu-rep "title" profiles/rX_ncu.md [profiles/r2_warp_corr_traffic.json]
+    python tools/summarize_ncu.py native_full.ncu-rep "title" ncu.md [warp_corr_traffic.json]
 
 The traffic JSON carries `mean_dram_bytes_per_launch` over the K-A (warp_corr*) launches of the capture: bench.py's `roofline.traffic`.
 """
