@@ -210,6 +210,32 @@ int pmb200_fuse_points(const unsigned char *final_mask, const double *depth_avg,
                        int H, int W, unsigned char *ply_body_out, int *count_out, int *block_scratch, void *stream);
 
 /* ------------------------------------------------------------------------------------
+ * DTU point-cloud evaluation (reference evaluations/dtu/*.m; INTEGRATION.md "DTU evaluation"), float64 throughout.
+ * Both calls sort the cloud into a fine / coarse cell hash held in a caller-owned device workspace of
+ * *_workspace_bytes(n) bytes (O(n), whatever the extent of the cloud; the size query returns bytes or a negative PMB200_E*).
+ *
+ * pmb200_thin_points (reducePts_haa.m): the points that survive thinning to a minimum distance `dst` when they are visited
+ * in the order of `rank` (a permutation of 0 .. n-1, earlier = smaller).  A point survives iff no surviving point of
+ * smaller rank lies within distance <= dst of it: the lexicographically-first maximal independent set, computed in parallel
+ * rounds with a bound of 256 rounds.
+ *   points [n,3] float64, rank [n] int32, keep_out [n] uint8 (1 = kept)
+ *   undecided_out  ONE int (device): 0, or the number of points left undecided when the round bound was reached (their
+ *                  keep_out is 0 and the result must not be used)
+ * pmb200_nearest_distance (MaxDistCP.m): for each "from" point, min(exact distance to the nearest "to" point, max_dist) if it
+ * lies in one of MaxDistCP's blocks of the box bb_host (BB_lo + k * max_dist <= x < BB_lo + k * max_dist + max_dist,
+ * k = 0 .. floor((BB_hi - BB_lo) / max_dist) per axis), else max_dist.
+ *   to_points [n_to,3], from_points [n_from,3], dist_out [n_from]: float64 device;  bb_host: HOST, 6 doubles (lo xyz, hi xyz)
+ *   cell: edge of the fine search cells, max_dist / 256 <= cell (speed only: the result does not depend on it); the search
+ *         visits at most 5^3 fine cells, then rings of 16^3-cell coarse cells out to max_dist (at most 35^3 coarse cells)
+ * Sort + table launches, then the search; no host synchronisation.  Point and output pointers may be NULL for empty clouds. */
+int64_t pmb200_thin_points_workspace_bytes(int64_t n);
+int pmb200_thin_points(const double *points, const int *rank, int64_t n, double dst, unsigned char *keep_out, int *undecided_out,
+                       void *workspace, int64_t workspace_bytes, void *stream);
+int64_t pmb200_nearest_distance_workspace_bytes(int64_t n_to);
+int pmb200_nearest_distance(const double *to_points, int64_t n_to, const double *from_points, int64_t n_from, const double *bb_host,
+                            double max_dist, double cell, double *dist_out, void *workspace, int64_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------
  * Depth / confidence map files either side of the path (SURVEY 8f row f5): PFM and COLMAP .bin, read straight into /
  * written straight from caller-owned host buffers (pinned, so the next step is one cudaMemcpyAsync).  Host code, no
  * stream.  Replaces reference datasets/data_io.py read_pfm :257-288, save_pfm :291-322, read_bin :165-191,

@@ -186,3 +186,71 @@ def save_ply(path: str, body) -> None:
         f.write(header.encode("ascii"))
         for b in parts:
             f.write(b.numpy().tobytes())
+
+
+_PLY_TYPES = {
+    "char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2", "ushort": "u2", "uint16": "u2",
+    "int": "i4", "int32": "i4", "uint": "u4", "uint32": "u4", "float": "f4", "float32": "f4", "double": "f8", "float64": "f8",
+}
+
+
+def read_ply_points(path: str) -> np.ndarray:
+    """Vertex positions of a PLY file -> float64 [n,3] (float32 coordinates widen exactly).
+
+    Reads `binary_little_endian` and `ascii` files whose `vertex` element has scalar properties x, y, z among any others
+    (colours, normals, ...) in any order, e.g. this project's save_ply output and the DTU `stl%03d_total.ply` files.  The
+    header becomes a numpy structured dtype, so the body is read in one call.  Other formats raise ValueError."""
+    with open(path, "rb") as f:
+        if f.readline().strip() != b"ply":
+            raise ValueError(f"{path}: not a PLY file")
+        fmt, elements, current = None, [], None
+        while True:
+            line = f.readline()
+            if not line:
+                raise ValueError(f"{path}: PLY header has no end_header")
+            words = line.decode("ascii", "replace").split()
+            if not words or words[0] in ("comment", "obj_info"):
+                continue
+            if words[0] == "end_header":
+                break
+            if words[0] == "format":
+                fmt = words[1]
+            elif words[0] == "element":
+                current = (words[1], int(words[2]), [])
+                elements.append(current)
+            elif words[0] == "property":
+                if current is None:
+                    raise ValueError(f"{path}: PLY property outside an element")
+                if words[1] == "list":
+                    current[2].append((words[-1], None))
+                else:
+                    if words[1] not in _PLY_TYPES:
+                        raise ValueError(f"{path}: unknown PLY property type {words[1]!r}")
+                    current[2].append((words[2], _PLY_TYPES[words[1]]))
+        if fmt not in ("binary_little_endian", "ascii"):
+            raise ValueError(f"{path}: PLY format {fmt!r} is not supported (binary_little_endian or ascii)")
+        for name, count, props in elements:
+            if name == "vertex":
+                break
+            if count:  # an element before the vertices would have to be skipped row by row
+                raise ValueError(f"{path}: PLY element {name!r} precedes the vertex element")
+        else:
+            raise ValueError(f"{path}: PLY file has no vertex element")
+        if any(t is None for _, t in props):
+            raise ValueError(f"{path}: list properties in the vertex element are not supported")
+        names = [p for p, _ in props]
+        if not all(a in names for a in ("x", "y", "z")):
+            raise ValueError(f"{path}: PLY vertex element lacks x, y or z")
+        if fmt == "ascii":
+            data = np.loadtxt(f, dtype=np.float64, max_rows=count, ndmin=2) if count else np.zeros((0, len(names)))
+            if data.shape != (count, len(names)):
+                raise ValueError(f"{path}: PLY body has {data.shape[0]} rows of {data.shape[1]} values, header says {count} of {len(names)}")
+            return np.ascontiguousarray(data[:, [names.index(a) for a in ("x", "y", "z")]])
+        dtype = np.dtype([(p, "<" + t) for p, t in props])
+        data = np.fromfile(f, dtype=dtype, count=count)
+        if data.shape[0] != count:
+            raise ValueError(f"{path}: PLY body holds {data.shape[0]} vertices, header says {count}")
+        out = np.empty((count, 3), dtype=np.float64)
+        for a, axis in enumerate(("x", "y", "z")):
+            out[:, a] = data[axis]
+        return out

@@ -846,3 +846,78 @@ def split_ply_body(body: Tensor):
     """uint8 [n,15] vertex records -> (vertices float32 [n,3], colours uint8 [n,3]) on the CPU."""
     b = body.detach().cpu().contiguous()
     return b[:, :12].contiguous().view(torch.float32).view(-1, 3), b[:, 12:].contiguous()
+
+
+def _points_arg(p: Tensor, name: str) -> Tensor:
+    if not _on_device(p):
+        raise RuntimeError(f"{name}: the H100 path needs a CUDA tensor (got {p.device}); there is no CPU fallback")
+    if p.dtype != torch.float64 or p.dim() != 2 or p.shape[1] != 3:
+        raise RuntimeError(f"{name}: expected a float64 [n,3] tensor, got {p.dtype} {tuple(p.shape)}")
+    return p.contiguous()
+
+
+def thin_points(points: Tensor, rank: Tensor, dst: float) -> Tensor:
+    """Thinning of a point cloud to a minimum distance (reference evaluations/dtu/reducePts_haa.m): the points visited in the
+    order of `rank` (int32 [n], a permutation of 0..n-1) that survive, i.e. that no surviving earlier point lies within
+    distance <= dst of.  points float64 [n,3] CUDA -> keep bool [n].  One host synchronisation at the end (the round-bound
+    check)."""
+    pts = _points_arg(points, "thin_points")
+    n = pts.shape[0]
+    if rank.shape != (n,) or rank.dtype != torch.int32 or rank.device != pts.device:
+        raise RuntimeError("thin_points: rank must be an int32 [n] tensor on the points' device")
+    rk = rank.contiguous()
+    keep = torch.empty(n, dtype=torch.uint8, device=pts.device)
+    undecided = torch.empty(1, dtype=torch.int32, device=pts.device)
+    lib = _native.lib()
+    ws_bytes = lib.pmb200_thin_points_workspace_bytes(n)
+    if ws_bytes < 0:
+        _native.check(int(ws_bytes), "thin_points_workspace_bytes")
+    ws = torch.empty(max(int(ws_bytes), 1), dtype=torch.uint8, device=pts.device)
+    with _device_guard(pts):
+        rc = lib.pmb200_thin_points(pts.data_ptr(), rk.data_ptr(), n, float(dst), keep.data_ptr(), undecided.data_ptr(),
+                                    ws.data_ptr(), int(ws_bytes), _stream(pts))
+    _native.check(rc, "thin_points")
+    left = int(undecided.item())
+    if left:
+        raise RuntimeError(f"thin_points: {left} points still undecided after the round bound of the native thinning")
+    return keep.bool()
+
+
+def default_search_cell(n_to: int, bb, max_dist: float) -> float:
+    """Fine cell edge for nearest_distance: about twice the spacing of n_to points spread over a surface the size of the box.
+    It only sets the speed of the search, never its result."""
+    import math
+
+    ext = [max(float(bb[1][a]) - float(bb[0][a]), 1e-9) for a in range(3)]
+    side = (ext[0] * ext[1] * ext[2]) ** (1.0 / 3.0)
+    cell = 2.0 * side / math.sqrt(max(n_to, 1))
+    return min(max(cell, max_dist / 256.0), max_dist / 8.0)  # the library requires cell >= max_dist / 256
+
+
+def nearest_distance(to_points: Tensor, from_points: Tensor, bb, max_dist: float = 60.0, cell: Optional[float] = None) -> Tensor:
+    """Distance from every `from` point to the nearest `to` point, capped at max_dist, with the block membership of the
+    reference's evaluations/dtu/MaxDistCP.m: a point outside its max_dist blocks over the box `bb` ([[x,y,z] lo, [x,y,z] hi])
+    gets max_dist.  Exact float64 distances.  to_points [m,3], from_points [n,3] float64 CUDA -> float64 [n]."""
+    import ctypes
+
+    to = _points_arg(to_points, "nearest_distance (to)")
+    frm = _points_arg(from_points, "nearest_distance (from)")
+    if to.device != frm.device:
+        raise RuntimeError("nearest_distance: both clouds must be on the same device")
+    box = [float(v) for row in bb for v in row]
+    if len(box) != 6:
+        raise RuntimeError("nearest_distance: bb must be 2 x 3 (lo, hi)")
+    if cell is None:
+        cell = default_search_cell(to.shape[0], [box[:3], box[3:]], max_dist)
+    out = torch.empty(frm.shape[0], dtype=torch.float64, device=frm.device)
+    lib = _native.lib()
+    ws_bytes = lib.pmb200_nearest_distance_workspace_bytes(to.shape[0])
+    if ws_bytes < 0:
+        _native.check(int(ws_bytes), "nearest_distance_workspace_bytes")
+    ws = torch.empty(max(int(ws_bytes), 1), dtype=torch.uint8, device=frm.device)
+    bb_host = (ctypes.c_double * 6)(*box)
+    with _device_guard(frm):
+        rc = lib.pmb200_nearest_distance(to.data_ptr(), to.shape[0], frm.data_ptr(), frm.shape[0], bb_host, float(max_dist), float(cell),
+                                         out.data_ptr(), ws.data_ptr(), int(ws_bytes), _stream(frm))
+    _native.check(rc, "nearest_distance")
+    return out
