@@ -18,6 +18,7 @@ There is no Python fallback: without libpmb200.so every call raises ``NativeLibr
 from __future__ import annotations
 
 import os
+from typing import List
 from typing import Tuple
 
 import numpy as np
@@ -88,6 +89,66 @@ def scale_to_max_dim(image: np.ndarray, max_dim: int) -> Tuple[np.ndarray, int, 
 
         image = cv2.resize(image, (int(scale * original_width), int(scale * original_height)), interpolation=cv2.INTER_LINEAR)
     return image, original_height, original_width
+
+
+def read_image(filename: str, max_dim: int = -1) -> Tuple[np.ndarray, int, int]:
+    """data_io.py:34-47 -> (image float32 [H,W,C] in [0,1], scaled to `max_dim` when that shrinks it; original_h; original_w)."""
+    from PIL import Image
+
+    np_image = np.array(Image.open(filename), dtype=np.float32) / 255.0
+    return scale_to_max_dim(np_image, max_dim)
+
+
+def save_image(filename: str, image: np.ndarray) -> None:
+    """data_io.py:50-64: bool -> uint8 0 / 255, float32 / float64 -> uint8(value * 255), anything else -> uint8; PIL picks
+    the file format from the extension (the mask PNGs of the fusion)."""
+    from PIL import Image
+
+    if image.dtype == bool:
+        image = image.astype(np.uint8) * 255
+    elif image.dtype == np.float32 or image.dtype == np.float64:
+        image = (image * 255).astype(np.uint8)
+    else:
+        image = image.astype(np.uint8)
+    Image.fromarray(image).save(filename)
+
+
+def read_cam_file(filename: str) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """data_io.py:85-106 -> (intrinsics float32 [3,3] from lines 8-10, extrinsics float32 [4,4] from lines 2-5, depth params
+    float32 from line 12 -- (depth_min, depth_max) in the DTU files -- or an empty float64 array when the file has no line 12).
+    The numbers go through np.fromstring(..., float32, sep=' ') as in the reference, so every value has the same bits."""
+    with open(filename) as f:
+        lines = [line.rstrip() for line in f.readlines()]
+    extrinsics = np.fromstring(" ".join(lines[1:5]), dtype=np.float32, sep=" ").reshape((4, 4))
+    intrinsics = np.fromstring(" ".join(lines[7:10]), dtype=np.float32, sep=" ").reshape((3, 3))
+    if len(lines) >= 12:
+        depth_params = np.fromstring(lines[11], dtype=np.float32, sep=" ")
+    else:
+        depth_params = np.empty(0)
+    return intrinsics, extrinsics, depth_params
+
+
+def read_pair_file(filename: str) -> List[Tuple[int, List[int]]]:
+    """data_io.py:109-127 -> [(reference view, [source views in file order])]; entries without source views are dropped."""
+    data = []
+    with open(filename) as f:
+        num_viewpoint = int(f.readline())
+        for _ in range(num_viewpoint):
+            ref_view = int(f.readline().rstrip())
+            src_views = [int(x) for x in f.readline().rstrip().split()[1::2]]
+            if len(src_views) != 0:
+                data.append((ref_view, src_views))
+    return data
+
+
+def scale_intrinsics(intrinsics: np.ndarray, image_hw: Tuple[int, int], original_h: int, original_w: int) -> np.ndarray:
+    """The intrinsics of a view whose image read_image scaled from original_h x original_w to image_hw: row 0 times
+    width / original width, row 1 times height / original height, in float32 (datasets/mvs.py:83-84, eval.py:210-211).
+    Returns a scaled copy."""
+    k = np.array(intrinsics, dtype=np.float32, copy=True)
+    k[0] *= image_hw[1] / original_w
+    k[1] *= image_hw[0] / original_h
+    return k
 
 
 def read_map(path: str, max_dim: int = -1) -> np.ndarray:
