@@ -236,6 +236,36 @@ int pmb200_nearest_distance(const double *to_points, int64_t n_to, const double 
                             double max_dist, double cell, double *dist_out, void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------
+ * COLMAP sparse model -> scene folder (reference colmap_input.py:318-373; INTEGRATION.md "COLMAP interop"), float64 throughout.
+ * The model: points xyz [n_points,3]; observations in CSR form, obs_offsets [n_images+1] (int32, obs_offsets[0] = 0) and
+ * obs_points [n_obs] (int32 dense point indices in each image's own 2D-point order, -1 entries removed); camera centres
+ * [n_images,3] and extrinsics [n_images,4,4] row-major, composed on the host.  1 <= n_images < 65536, n_obs < 2^31.
+ *
+ * View scores: for i < j, score[i,j] = score[j,i] = sum over the entries x of obs_i, in obs_i's order, whose point is in obs_j of
+ *     exp(-(theta - theta0)^2 / (2 sigma^2)),  theta = (180 / pi) acos(clamp(dot(c_i - x, c_j - x) / |c_i - x| / |c_j - x|)),
+ *     sigma = sigma1 if theta <= theta0 else sigma2;  a point on c_i or c_j adds 0; the diagonal is 0.
+ * Two calls over ONE caller-owned workspace:
+ *   pmb200_view_scores_count   sorts the observations by point and counts the contributions T (pairs of an entry of obs_i and
+ *                              a distinct image j > i that also observes its point); writes T to total_out (ONE int64, device).
+ *                              Workspace: pmb200_view_scores_workspace_bytes(n_images, n_obs, 0).
+ *   pmb200_view_scores         emits, sorts and sums the contributions into score_out [n_images,n_images] (zeroed by the
+ *                              call); n_contrib = the T of the count call, whose results the workspace (now of at least
+ *                              pmb200_view_scores_workspace_bytes(n_images, n_obs, T) bytes, the same first part) still holds.
+ * T >= 2^31 is rejected.  Each pair is summed by one thread in obs_i order: deterministic, no floating-point atomics.
+ * Depth ranges: per image, the z (row 2 of extrinsic . [x,y,z,1]) of every entry of obs_i, sorted; ranges_out [n_images,2] =
+ *   (zs[int(n * 0.01)], zs[int(n * 0.99)]), NaN for an image without entries.
+ * The size queries return bytes or a negative PMB200_E* (they need a CUDA device to size the CUB sorts).  Enqueues only. */
+int64_t pmb200_view_scores_workspace_bytes(int n_images, int64_t n_obs, int64_t n_contrib);
+int pmb200_view_scores_count(const int *obs_offsets, const int *obs_points, int n_images, int64_t n_obs, int64_t *total_out,
+                             void *workspace, int64_t workspace_bytes, void *stream);
+int pmb200_view_scores(const double *xyz, int64_t n_points, const int *obs_offsets, const int *obs_points, const double *centers,
+                       int n_images, int64_t n_obs, int64_t n_contrib, double theta0, double sigma1, double sigma2, double *score_out,
+                       void *workspace, int64_t workspace_bytes, void *stream);
+int64_t pmb200_depth_ranges_workspace_bytes(int n_images, int64_t n_obs);
+int pmb200_depth_ranges(const double *xyz, int64_t n_points, const int *obs_offsets, const int *obs_points, const double *extrinsics,
+                        int n_images, int64_t n_obs, double *ranges_out, void *workspace, int64_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------
  * Depth / confidence map files either side of the path (SURVEY 8f row f5): PFM and COLMAP .bin, read straight into /
  * written straight from caller-owned host buffers (pinned, so the next step is one cudaMemcpyAsync).  Host code, no
  * stream.  Replaces reference datasets/data_io.py read_pfm :257-288, save_pfm :291-322, read_bin :165-191,

@@ -17,7 +17,7 @@ from typing import Optional
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 _REPO_DIR = os.path.dirname(_PKG_DIR)
 LIB_PATH = os.path.join(_PKG_DIR, "libpmb200.so")
-SOURCES = [os.path.join(_PKG_DIR, "csrc", f) for f in ("pm_kernels.cu", "pm_backward.cu", "pm_conv.cu", "pm_conv5.cu", "pm_stem.cu", "pm_refine.cu", "pm_geo.cu", "pm_cloud.cu", "pm_mapio.cpp")]
+SOURCES = [os.path.join(_PKG_DIR, "csrc", f) for f in ("pm_kernels.cu", "pm_backward.cu", "pm_conv.cu", "pm_conv5.cu", "pm_stem.cu", "pm_refine.cu", "pm_geo.cu", "pm_cloud.cu", "pm_colmap.cu", "pm_mapio.cpp")]
 HEADERS = [
     os.path.join(_PKG_DIR, "csrc", "pm_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_warpcorr4.cuh"),
@@ -126,6 +126,12 @@ _SIGNATURES = {
     "pmb200_thin_points": (c_int, [c_void_p, c_void_p, c_int64, c_double, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
     "pmb200_nearest_distance_workspace_bytes": (c_int64, [c_int64]),
     "pmb200_nearest_distance": (c_int, [c_void_p, c_int64, c_void_p, c_int64, POINTER(c_double), c_double, c_double, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pmb200_view_scores_workspace_bytes": (c_int64, [c_int, c_int64, c_int64]),
+    "pmb200_view_scores_count": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pmb200_view_scores": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_int64, c_double, c_double, c_double,
+                                   c_void_p, c_void_p, c_int64, c_void_p]),
+    "pmb200_depth_ranges_workspace_bytes": (c_int64, [c_int, c_int64]),
+    "pmb200_depth_ranges": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_int64, c_void_p]),
     "pmb200_map_probe": (c_int, [c_char_p, c_int, _PMAP]),
     "pmb200_map_read": (c_int, [c_char_p, c_int, c_void_p, c_int64, _PMAP]),
     "pmb200_map_write": (c_int, [c_char_p, c_int, c_void_p, c_int, c_int, c_int, c_double]),

@@ -921,3 +921,73 @@ def nearest_distance(to_points: Tensor, from_points: Tensor, bb, max_dist: float
                                          out.data_ptr(), ws.data_ptr(), int(ws_bytes), _stream(frm))
     _native.check(rc, "nearest_distance")
     return out
+
+
+def _model_args(xyz: Tensor, obs_offsets: Tensor, obs_points: Tensor, per_image: Tensor, per_image_shape, name: str):
+    """Checks of a sparse model held on the device (ops.view_scores / ops.depth_ranges) -> contiguous tensors and N, M."""
+    for t, what in ((xyz, "xyz"), (obs_offsets, "obs_offsets"), (obs_points, "obs_points"), (per_image, "per-image cameras")):
+        if not _on_device(t):
+            raise RuntimeError(f"{name}: {what} must be a CUDA tensor (got {t.device}); there is no CPU fallback")
+        if t.device != xyz.device:
+            raise RuntimeError(f"{name}: every tensor must be on xyz's device")
+    if xyz.dtype != torch.float64 or xyz.dim() != 2 or xyz.shape[1] != 3:
+        raise RuntimeError(f"{name}: xyz must be float64 [P,3], got {xyz.dtype} {tuple(xyz.shape)}")
+    if obs_offsets.dtype != torch.int32 or obs_offsets.dim() != 1 or obs_offsets.shape[0] < 2:
+        raise RuntimeError(f"{name}: obs_offsets must be int32 [N+1] with N >= 1")
+    if obs_points.dtype != torch.int32 or obs_points.dim() != 1:
+        raise RuntimeError(f"{name}: obs_points must be int32 [M]")
+    n = obs_offsets.shape[0] - 1
+    if per_image.dtype != torch.float64 or tuple(per_image.shape) != (n,) + tuple(per_image_shape):
+        raise RuntimeError(f"{name}: expected float64 {(n,) + tuple(per_image_shape)} per-image cameras, got {per_image.dtype} "
+                           f"{tuple(per_image.shape)}")
+    return xyz.contiguous(), obs_offsets.contiguous(), obs_points.contiguous(), per_image.contiguous(), n, obs_points.shape[0]
+
+
+def _workspace(nbytes: int, what: str, device) -> Tensor:
+    if nbytes < 0:
+        _native.check(int(nbytes), what)
+    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device)
+
+
+def view_scores(xyz: Tensor, obs_offsets: Tensor, obs_points: Tensor, centers: Tensor, theta0: float = 5.0, sigma1: float = 1.0,
+                sigma2: float = 10.0) -> Tensor:
+    """View selection scores of a sparse model (reference colmap_input.py:336-373): float64 [N,N], symmetric, zero diagonal.
+    xyz float64 [P,3], obs_offsets int32 [N+1], obs_points int32 [M] (dense point indices, -1 entries removed), centers
+    float64 [N,3]; all CUDA.  One host read: the number of contributions, which sizes the second phase."""
+    xyz, offs, pts, ctr, n, m = _model_args(xyz, obs_offsets, obs_points, centers, (3,), "view_scores")
+    lib = _native.lib()
+    total = torch.empty(1, dtype=torch.int64, device=xyz.device)
+    with _device_guard(xyz):
+        ws_bytes = int(lib.pmb200_view_scores_workspace_bytes(n, m, 0))
+        ws = _workspace(ws_bytes, "view_scores_workspace_bytes", xyz.device)
+        rc = lib.pmb200_view_scores_count(offs.data_ptr(), pts.data_ptr(), n, m, total.data_ptr(), ws.data_ptr(), ws_bytes, _stream(xyz))
+        _native.check(rc, "view_scores_count")
+        t = int(total.item())
+        need = int(lib.pmb200_view_scores_workspace_bytes(n, m, t))
+        if need < 0:
+            _native.check(need, "view_scores_workspace_bytes")
+        if need > ws_bytes:  # grow, keeping the first part the count call filled
+            grown = torch.empty(need, dtype=torch.uint8, device=xyz.device)
+            grown[:ws_bytes].copy_(ws[:ws_bytes])
+            ws, ws_bytes = grown, need
+        score = torch.empty((n, n), dtype=torch.float64, device=xyz.device)
+        rc = lib.pmb200_view_scores(xyz.data_ptr(), xyz.shape[0], offs.data_ptr(), pts.data_ptr(), ctr.data_ptr(), n, m, t, float(theta0),
+                                    float(sigma1), float(sigma2), score.data_ptr(), ws.data_ptr(), ws_bytes, _stream(xyz))
+    _native.check(rc, "view_scores")
+    return score
+
+
+def depth_ranges(xyz: Tensor, obs_offsets: Tensor, obs_points: Tensor, extrinsics: Tensor) -> Tensor:
+    """Relaxed depth range per image (reference colmap_input.py:318-333): float64 [N,2] = the 1 % and 99 % order statistics of
+    the z of the image's observations (duplicates included), NaN for an image without observations.  Arguments as
+    view_scores, with extrinsics float64 [N,4,4] (world -> camera) instead of the centres."""
+    xyz, offs, pts, ext, n, m = _model_args(xyz, obs_offsets, obs_points, extrinsics, (4, 4), "depth_ranges")
+    lib = _native.lib()
+    out = torch.empty((n, 2), dtype=torch.float64, device=xyz.device)
+    with _device_guard(xyz):
+        ws_bytes = int(lib.pmb200_depth_ranges_workspace_bytes(n, m))
+        ws = _workspace(ws_bytes, "depth_ranges_workspace_bytes", xyz.device)
+        rc = lib.pmb200_depth_ranges(xyz.data_ptr(), xyz.shape[0], offs.data_ptr(), pts.data_ptr(), ext.data_ptr(), n, m, out.data_ptr(),
+                                     ws.data_ptr(), ws_bytes, _stream(xyz))
+    _native.check(rc, "depth_ranges")
+    return out
