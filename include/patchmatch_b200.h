@@ -266,6 +266,36 @@ int pmb200_depth_ranges(const double *xyz, int64_t n_points, const int *obs_offs
                         int n_images, int64_t n_obs, double *ranges_out, void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------
+ * Training loss and metrics (reference models/net.py:321-342 patchmatchnet_loss, train.py:174-180 create_stage_images,
+ * utils.py:187-221 absolute_depth_error_metrics / threshold_metrics; DESIGN.md K-L).
+ *   depth_gt [B,H,W] float32 and mask [B,H,W] uint8 (0 / non-0) at full resolution.  The level-l ground truth and mask at
+ *   (y, x) are the full-resolution values at (y << l, x << l) (F.interpolate(scale_factor=0.5**l, mode="nearest")).
+ *   maps_host: HOST array of device pointers; map m is float32 [B, H >> l_m, W >> l_m] at level levels_host[m] in 0..3.
+ *
+ * pmb200_depth_loss: terms_out float64 [n_maps + 4]: for each map the sum over the level's masked pixels of smooth-L1(d - gt)
+ *   (beta 1; each term formed in float32 as torch forms it, accumulated in float64), then the mask count of levels 0..3.
+ *   Per-block partials go to the caller-owned workspace of pmb200_depth_loss_workspace_bytes(...) bytes (or a negative
+ *   PMB200_E*), and one final launch sums them in index order: reruns are bit-identical.  1 <= n_maps <= 16.
+ * pmb200_depth_loss_backward: grads_host[m] (device, the shape of map m) = mask ? clamp(d - gt, -1, 1) * g * scale / count_l : 0,
+ *   with g = *grad_loss (device float32 scalar) and count_l from terms.  One launch over all maps.
+ * pmb200_depth_metrics: maps_host[l] is the map of level l (4 pointers); out float64 [B, 8 + n_thr], per image:
+ *   the sum of |d - gt| (difference in float32) over the masked pixels of levels 0..3, the mask counts of levels 0..3, then
+ *   per threshold the number of masked level-0 pixels with float32 |d - gt| > thresholds_host[k].  n_thr <= 8.  One launch,
+ *   one block per (image, level).
+ * No atomics; enqueue only. */
+#define PMB200_DEPTH_LOSS_MAX_MAPS 16
+#define PMB200_DEPTH_METRICS_MAX_THRESHOLDS 8
+int64_t pmb200_depth_loss_workspace_bytes(const int *levels_host, int n_maps, int B, int H, int W);
+int pmb200_depth_loss(const float *const *maps_host, const int *levels_host, int n_maps, const float *depth_gt,
+                      const unsigned char *mask, int B, int H, int W, double *terms_out, void *workspace,
+                      int64_t workspace_bytes, void *stream);
+int pmb200_depth_loss_backward(const float *const *maps_host, const int *levels_host, int n_maps, const float *depth_gt,
+                               const unsigned char *mask, int B, int H, int W, const double *terms, const float *grad_loss,
+                               float scale, float *const *grads_host, void *stream);
+int pmb200_depth_metrics(const float *const *maps_host, const float *depth_gt, const unsigned char *mask, int B, int H, int W,
+                         const float *thresholds_host, int n_thr, double *out, void *stream);
+
+/* ------------------------------------------------------------------------------------
  * Depth / confidence map files either side of the path (SURVEY 8f row f5): PFM and COLMAP .bin, read straight into /
  * written straight from caller-owned host buffers (pinned, so the next step is one cudaMemcpyAsync).  Host code, no
  * stream.  Replaces reference datasets/data_io.py read_pfm :257-288, save_pfm :291-322, read_bin :165-191,

@@ -178,3 +178,39 @@ class AdaptiveEval(torch.autograd.Function):
             )
         _native.check(rc, "adaptive_eval_backward")
         return d_score0, d_hyp, None, d_off, d_fw, None, None, None, None, None
+
+
+def loss_from_terms(terms: Tensor, levels) -> Tensor:
+    """sum_m terms[m] / terms[n_maps + levels[m]] in float64 on the device, cast to float32 (nan for a level without masked
+    pixels, as the reference's mean of an empty selection)."""
+    n = len(levels)
+    counts = terms[n + torch.tensor(list(levels), dtype=torch.int64).to(terms.device, non_blocking=True)]
+    return (terms[:n] / counts).sum().float()
+
+
+class DepthLoss(torch.autograd.Function):
+    """patchmatchnet_loss (reference models/net.py:321-342) on the K-L kernels: loss = sum_m terms[m] / terms[n_maps + l_m],
+    formed on the device in float64 and cast to float32 (no host synchronisation; a level without masked pixels gives nan,
+    as the reference's mean of an empty selection does).  Gradients: the depth maps, in one launch.
+
+        loss = DepthLoss.apply(levels, depth_gt, mask, all_reduce, scale, *maps)
+
+    levels: the pyramid level of each map; depth_gt float32 [B,H,W], mask [B,H,W] at full resolution.  all_reduce: None, or a
+    callable that sums the float64 terms across ranks in place before the loss is formed, so every rank holds the loss of the
+    global batch; scale: the factor the backward applies (the world size when the parameter gradients are then averaged)."""
+
+    @staticmethod
+    def forward(ctx, levels, depth_gt: Tensor, mask: Tensor, all_reduce, scale: float, *maps: Tensor) -> Tensor:
+        maps = [m.detach() for m in maps]
+        terms = ops.depth_loss_terms(maps, levels, depth_gt, mask)
+        if all_reduce is not None:
+            all_reduce(terms)
+        ctx.levels, ctx.scale = list(levels), float(scale)
+        ctx.save_for_backward(depth_gt, mask, terms, *maps)
+        return loss_from_terms(terms, levels)
+
+    @staticmethod
+    def backward(ctx, g: Tensor):
+        gt, mask, terms, *maps = ctx.saved_tensors
+        grads = ops.depth_loss_backward(maps, ctx.levels, gt, mask, terms, g.contiguous(), ctx.scale)
+        return (None, None, None, None, None, *grads)

@@ -991,3 +991,112 @@ def depth_ranges(xyz: Tensor, obs_offsets: Tensor, obs_points: Tensor, extrinsic
                                      ws.data_ptr(), ws_bytes, _stream(xyz))
     _native.check(rc, "depth_ranges")
     return out
+
+
+DEPTH_LOSS_MAX_MAPS = 16
+DEPTH_METRICS_MAX_THRESHOLDS = 8
+
+
+def _ground_truth_args(depth_gt: Tensor, mask: Tensor, name: str):
+    """float32 [B,H,W] ground truth and uint8 / bool [B,H,W] mask on one device -> contiguous (gt, uint8 mask)."""
+    gt = _require(depth_gt, f"{name} (depth_gt)", 3)
+    if not _on_device(mask) or mask.device != gt.device or tuple(mask.shape) != tuple(gt.shape):
+        raise RuntimeError(f"{name}: mask must be a CUDA tensor of depth_gt's shape {tuple(gt.shape)} on its device, got "
+                           f"{tuple(mask.shape)} on {mask.device}")
+    if mask.dtype == torch.bool:
+        mask = mask.view(torch.uint8)
+    if mask.dtype != torch.uint8:
+        raise RuntimeError(f"{name}: mask must be uint8 or bool, got {mask.dtype}")
+    return gt, mask.contiguous()
+
+
+def _level_maps(maps: Sequence[Tensor], levels: Sequence[int], shape, device, name: str):
+    """Maps at pyramid levels: each float32 [B, H >> l, W >> l] (a [B,1,h,w] map is taken as [B,h,w]) -> contiguous [B,h,w]."""
+    B, H, W = shape
+    out = []
+    for m, l in zip(maps, levels):
+        if not 0 <= int(l) <= 3:
+            raise RuntimeError(f"{name}: level {l} outside 0..3")
+        want = (B, H >> int(l), W >> int(l))
+        t = _require(m, name)
+        if t.device != device or t.numel() != want[0] * want[1] * want[2] or tuple(t.shape[-2:]) != want[1:] or t.shape[0] != B:
+            raise RuntimeError(f"{name}: a level-{l} map must be {want} (or [B,1,h,w]) on {device}, got {tuple(m.shape)} on {m.device}")
+        out.append(t)
+    return out
+
+
+def depth_loss_terms(maps: Sequence[Tensor], levels: Sequence[int], depth_gt: Tensor, mask: Tensor) -> Tensor:
+    """The sums behind patchmatchnet_loss (reference models/net.py:321-342) without a host synchronisation: float64
+    [n_maps + 4] = for each map, the sum of smooth-L1(d - gt) (beta 1) over the masked pixels of its level, then the mask
+    counts of levels 0..3.  Map m is at pyramid level levels[m]; depth_gt float32 [B,H,W] and mask (uint8 or bool) [B,H,W] are
+    full resolution, and level l reads them at (y << l, x << l) as F.interpolate(scale_factor=0.5**l, mode="nearest") does.
+    Deterministic: reruns are bit-identical."""
+    import ctypes
+
+    gt, mk = _ground_truth_args(depth_gt, mask, "depth_loss_terms")
+    n = len(maps)
+    if len(levels) != n or not 1 <= n <= DEPTH_LOSS_MAX_MAPS:
+        raise RuntimeError(f"depth_loss_terms: 1..{DEPTH_LOSS_MAX_MAPS} maps, one level each (got {n} maps, {len(levels)} levels)")
+    ms = _level_maps(maps, levels, tuple(gt.shape), gt.device, "depth_loss_terms")
+    B, H, W = gt.shape
+    lv = (ctypes.c_int * n)(*[int(l) for l in levels])
+    lib = _native.lib()
+    terms = torch.empty(n + 4, dtype=torch.float64, device=gt.device)
+    with _device_guard(gt):
+        ws_bytes = int(lib.pmb200_depth_loss_workspace_bytes(lv, n, B, H, W))
+        ws = _workspace(ws_bytes, "depth_loss_workspace_bytes", gt.device)
+        ptrs, keep = _native.pointer_array([m.data_ptr() for m in ms])
+        rc = lib.pmb200_depth_loss(ptrs, lv, n, gt.data_ptr(), mk.data_ptr(), B, H, W, terms.data_ptr(), ws.data_ptr(), ws_bytes,
+                                   _stream(gt))
+    _native.check(rc, "depth_loss")
+    return terms
+
+
+def depth_loss_backward(maps: Sequence[Tensor], levels: Sequence[int], depth_gt: Tensor, mask: Tensor, terms: Tensor,
+                        grad_loss: Tensor, scale: float = 1.0) -> list:
+    """Gradient of  loss = sum_m terms[m] / terms[n_maps + levels[m]]  with respect to every map, in one launch:
+    mask ? clamp(d - gt, -1, 1) * grad_loss * scale / count_level : 0, each of its map's shape.  grad_loss is a device scalar."""
+    gt, mk = _ground_truth_args(depth_gt, mask, "depth_loss_backward")
+    n = len(maps)
+    if len(levels) != n or not 1 <= n <= DEPTH_LOSS_MAX_MAPS:
+        raise RuntimeError(f"depth_loss_backward: 1..{DEPTH_LOSS_MAX_MAPS} maps, one level each")
+    ms = _level_maps(maps, levels, tuple(gt.shape), gt.device, "depth_loss_backward")
+    if terms.dtype != torch.float64 or tuple(terms.shape) != (n + 4,) or terms.device != gt.device:
+        raise RuntimeError(f"depth_loss_backward: terms must be float64 [{n + 4}] on {gt.device}")
+    g = _require(grad_loss.reshape(()), "depth_loss_backward (grad_loss)")
+    import ctypes
+
+    B, H, W = gt.shape
+    grads = [torch.empty_like(m) for m in ms]
+    lv = (ctypes.c_int * n)(*[int(l) for l in levels])
+    with _device_guard(gt):
+        ptrs, keep_m = _native.pointer_array([m.data_ptr() for m in ms])
+        gptrs, keep_g = _native.pointer_array([t.data_ptr() for t in grads])
+        rc = _native.lib().pmb200_depth_loss_backward(ptrs, lv, n, gt.data_ptr(), mk.data_ptr(), B, H, W, terms.contiguous().data_ptr(),
+                                                      g.data_ptr(), float(scale), gptrs, _stream(gt))
+    _native.check(rc, "depth_loss_backward")
+    return [t.view_as(m) for t, m in zip(grads, maps)]
+
+
+def depth_metrics(maps: Sequence[Tensor], depth_gt: Tensor, mask: Tensor, thresholds: Sequence[float] = (1.0, 2.0, 4.0, 8.0)) -> Tensor:
+    """Per-image sums behind the reference's absolute_depth_error_metrics and threshold_metrics (utils.py:187-221), without a
+    host synchronisation.  maps: the four maps of levels 0..3 (float32 [B, H >> l, W >> l]); -> float64 [B, 8 + n_thr]:
+    the sum of |d - gt| over the masked pixels of levels 0..3, the mask counts of levels 0..3, and per threshold the number
+    of masked level-0 pixels with float32 |d - gt| > t.  Exact counts: rates formed from them match the reference bit for bit."""
+    import ctypes
+
+    gt, mk = _ground_truth_args(depth_gt, mask, "depth_metrics")
+    if len(maps) != 4:
+        raise RuntimeError("depth_metrics: one map for each of the levels 0..3")
+    if len(thresholds) > DEPTH_METRICS_MAX_THRESHOLDS:
+        raise RuntimeError(f"depth_metrics: at most {DEPTH_METRICS_MAX_THRESHOLDS} thresholds")
+    ms = _level_maps(maps, range(4), tuple(gt.shape), gt.device, "depth_metrics")
+    B, H, W = gt.shape
+    thr = (ctypes.c_float * max(len(thresholds), 1))(*[float(t) for t in thresholds])
+    out = torch.empty((B, 8 + len(thresholds)), dtype=torch.float64, device=gt.device)
+    with _device_guard(gt):
+        ptrs, keep = _native.pointer_array([m.data_ptr() for m in ms])
+        rc = _native.lib().pmb200_depth_metrics(ptrs, gt.data_ptr(), mk.data_ptr(), B, H, W, thr, len(thresholds), out.data_ptr(),
+                                                _stream(gt))
+    _native.check(rc, "depth_metrics")
+    return out
