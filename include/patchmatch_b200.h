@@ -177,6 +177,14 @@ int pmb200_conv2d_nhwc(const float *x, const float *filter_frag, const float *bi
                        int relu, int precision, int transposed2x, int y_channel_stride, int y_channel_offset,
                        int rows_per_warp, void *stream);
 
+/* One source view of a ragged pack (the *_views entry points): the view's first float is src_flat + offset, and batch item b
+ * of it is [height, width(, C)] row-major starting at src_flat + offset + b * height * width (* C). */
+typedef struct pmb200_view_extent {
+    int64_t offset; /* floats from src_flat to (view v, batch 0); K-A: a multiple of 4 */
+    int height;
+    int width;
+} pmb200_view_extent;
+
 /* ------------------------------------------------------------------------------------
  * Geometric-consistency filtering of one reference depth map against V source depth maps, one launch
  * (SURVEY.md 8f row f4).  Replaces reproject_with_depth (eval.py:86-146), check_geometric_consistency (eval.py:149-190)
@@ -196,6 +204,15 @@ int pmb200_geometric_filter(const float *ref_depth, const float *confidence, con
                             float geo_depth_thres, float photo_thres, int geo_mask_thres, int *geo_mask_sum_out,
                             unsigned char *photo_mask_out, unsigned char *final_mask_out, double *depth_avg_out,
                             void *stream);
+/* pmb200_geometric_filter with source depth maps of different sizes (V <= 64): src_depths [V,Hs,Ws] replaced by src_flat and
+ * one host extent per view; source view v's map is [height_v, width_v] at src_flat + offset_v, sampled at its own size
+ * (eval.py:129 remaps each source on its own map).  PMB200_EINVAL when a view has a non-positive size, more than 2^31
+ * pixels, or a negative offset. */
+int pmb200_geometric_filter_views(const float *ref_depth, const float *confidence, const float *src_flat,
+                                  const pmb200_view_extent *views_host, const double *cams, int V, int H, int W,
+                                  double geo_pixel_thres, float geo_depth_thres, float photo_thres, int geo_mask_thres,
+                                  int *geo_mask_sum_out, unsigned char *photo_mask_out, unsigned char *final_mask_out,
+                                  double *depth_avg_out, void *stream);
 
 /* Point-cloud half of the fusion for one reference view (reference eval.py:273-296): the pixels of final_mask, in row-major
  * order, back-projected with the averaged depth into the world frame, with their colours, written as the 15-byte vertex
@@ -413,6 +430,37 @@ int pmb200_warp_corr_view_weights(const float *ref_nhwc, const float *src_nhwc, 
                                   float *view_weights_out, float *sims_out,
                                   int V, int B, int C, int G, int H, int W, int Hs, int Ws, int D,
                                   void *stream);
+
+/* ------------------------------------------------------------------------------------
+ * K-A with a size per source view (views of different resolutions or orientations; the
+ * reference's differentiable_warping samples each source at its own size).
+ * A ragged source pack is one float buffer `src_flat` plus one extent per view:
+ *   source view v, batch item b, is [height_v, width_v, C] channels-last starting at
+ *   src_flat + offset_v + b * height_v * width_v * C.
+ * offset_v counts floats and must be a multiple of 4 (16-byte aligned gathers); src_flat is
+ * 32-byte aligned on the (C,G) fast paths.  views_host is a HOST array of V extents, copied into
+ * the kernel parameter block (a captured CUDA graph keeps its own copy, like head_host).
+ * Each view is exactly what the uniform entry point computes for a pack of that view's size:
+ * the align_corners=True scale (width_v - 1) / (W - 1), (height_v - 1) / (H - 1), zero padding
+ * at that view's borders and the behind-the-camera rule.  PMB200_EINVAL, output untouched,
+ * when V is outside 1..PMB200_MAX_VIEWS, a view has a non-positive size or height*width >= 2^29,
+ * an offset is negative or not a multiple of 4, or the pack reaches 2^31 float4 elements.
+ * Always runs the third-generation kernel (the generic kernel for other (C,G)).
+ */
+/* pmb200_warp_corr with (Hs, Ws) replaced by per-view extents */
+int pmb200_warp_corr_views(const float *ref_nhwc, const float *src_flat, const pmb200_view_extent *views_host,
+                           const float *rt, const float *depth, const float *view_weights, float *out,
+                           int V, int B, int C, int G, int H, int W, int D, void *stream);
+/* pmb200_warp_corr_score with (Hs, Ws) replaced by per-view extents */
+int pmb200_warp_corr_score_views(const float *ref_nhwc, const float *src_flat, const pmb200_view_extent *views_host,
+                                 const float *rt, const float *depth, const float *view_weights,
+                                 const pmb200_mlp *head_host, float *score_out, int score_stride,
+                                 int V, int B, int C, int G, int H, int W, int D, void *stream);
+/* pmb200_warp_corr_view_weights with (Hs, Ws) replaced by per-view extents */
+int pmb200_warp_corr_view_weights_views(const float *ref_nhwc, const float *src_flat, const pmb200_view_extent *views_host,
+                                        const float *rt, const float *depth, const pmb200_mlp *head_host,
+                                        float *view_weights_out, float *sims_out,
+                                        int V, int B, int C, int G, int H, int W, int D, void *stream);
 
 /* View-weighted aggregation of stored per-view similarities + SimilarityNet head:
  *   score_out [B,D,H,W] = MLP( sum_v sims[v]*w[:,v] / (1e-5 + sum_v w[:,v]) ).  G in {4,8}. */

@@ -102,6 +102,15 @@ class MapInfo(ctypes.Structure):
 
 _PMAP = POINTER(MapInfo)
 
+
+class ViewExtent(ctypes.Structure):
+    """pmb200_view_extent (include/patchmatch_b200.h): one source view of a ragged pack."""
+
+    _fields_ = [("offset", c_int64), ("height", c_int), ("width", c_int)]
+
+
+_PVIEW = POINTER(ViewExtent)
+
 _SIGNATURES = {
     "pmb200_abi_version": (c_int, []),
     "pmb200_last_error": (c_char_p, []),
@@ -146,6 +155,12 @@ _SIGNATURES = {
     "pmb200_offset_corr": (c_int, [c_void_p] * 2 + [c_int, c_void_p] + [c_int] * 7 + [c_void_p]),
     "pmb200_warp_corr_score": (c_int, [c_void_p] * 5 + [_PMLP, c_void_p] + [c_int] * 10 + [c_void_p]),
     "pmb200_warp_corr_view_weights": (c_int, [c_void_p] * 4 + [_PMLP, c_void_p, c_void_p] + [c_int] * 9 + [c_void_p]),
+    "pmb200_warp_corr_views": (c_int, [c_void_p, c_void_p, _PVIEW] + [c_void_p] * 4 + [c_int] * 7 + [c_void_p]),
+    "pmb200_warp_corr_score_views": (c_int, [c_void_p, c_void_p, _PVIEW] + [c_void_p] * 3 + [_PMLP, c_void_p] + [c_int] * 8 + [c_void_p]),
+    "pmb200_warp_corr_view_weights_views": (c_int, [c_void_p, c_void_p, _PVIEW] + [c_void_p] * 2 + [_PMLP, c_void_p, c_void_p]
+                                            + [c_int] * 7 + [c_void_p]),
+    "pmb200_geometric_filter_views": (c_int, [c_void_p] * 3 + [_PVIEW, c_void_p] + [c_int] * 3 + [c_double, c_float, c_float, c_int]
+                                      + [c_void_p] * 5),
     "pmb200_aggregate_views_score": (c_int, [c_void_p] * 2 + [_PMLP, c_void_p] + [c_int] * 7 + [c_void_p]),
     "pmb200_offset_corr_weight": (c_int, [c_void_p] * 2 + [c_int, _PMLP, c_void_p] + [c_int] * 7 + [c_void_p]),
     "pmb200_init_propagate": (c_int, [c_void_p] * 2 + [c_int] + [c_void_p] * 4 + [c_int] * 8 + [c_float, c_void_p]),

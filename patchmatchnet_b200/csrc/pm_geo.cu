@@ -51,6 +51,31 @@ __global__ void __launch_bounds__(256) geometric_filter_kernel(const GeoParams p
     p.depth_avg[n] = r.depth_avg;
 }
 
+// Source depth maps of different sizes (pmb200_geometric_filter_views): the extents travel in the parameter block and are
+// staged in shared memory behind the cameras.
+constexpr int kGeoMaxViews = 64;
+struct GeoViews {
+    pmgeo::SourceMap v[kGeoMaxViews];
+};
+
+__global__ void __launch_bounds__(256) geometric_filter_views_kernel(const GeoParams p, const GeoViews views) {
+    extern __shared__ double s_cam[];  // [V][60], then V SourceMap
+    pmgeo::SourceMap *s_views = reinterpret_cast<pmgeo::SourceMap *>(s_cam + p.V * kCamDoubles);
+    for (int i = threadIdx.x; i < p.V * kCamDoubles; i += blockDim.x) s_cam[i] = p.cams[i];
+    for (int i = threadIdx.x; i < p.V; i += blockDim.x) s_views[i] = views.v[i];
+    __syncthreads();
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n >= p.H * p.W) return;
+    const int x = n % p.W, y = n / p.W;
+    const pmgeo::PixelResult r = pmgeo::filter_pixel(s_cam, p.src_depths, s_views, p.V, x, y, __ldg(p.ref_depth + n),
+                                                     __ldg(p.confidence + n), p.pixel_thres, p.depth_thres, p.photo_thres,
+                                                     p.mask_thres);
+    p.mask_sum[n] = r.count;
+    p.photo_mask[n] = r.photo ? 1 : 0;
+    p.final_mask[n] = r.final ? 1 : 0;
+    p.depth_avg[n] = r.depth_avg;
+}
+
 // ---- fusion half (reference eval.py:273-296): masked back-projection + colour gather + ORDER-PRESERVING compaction ----------
 // Three small launches: per-block survivor counts, one-block exclusive scan of the counts, write.  A survivor's position is
 // scan[block] + (survivors before it in the block), so the records come out in row-major pixel order exactly as the
@@ -150,4 +175,35 @@ extern "C" int pmb200_geometric_filter(const float *ref_depth, const float *conf
     const int blocks = (int)(((long long)H * W + threads - 1) / threads);
     geometric_filter_kernel<<<blocks, threads, (size_t)V * kCamDoubles * sizeof(double), reinterpret_cast<cudaStream_t>(stream)>>>(p);
     return pmb200_internal_launch_status("geometric_filter");
+}
+
+extern "C" int pmb200_geometric_filter_views(const float *ref_depth, const float *confidence, const float *src_flat,
+                                             const pmb200_view_extent *views_host, const double *cams, int V, int H, int W,
+                                             double geo_pixel_thres, float geo_depth_thres, float photo_thres, int geo_mask_thres,
+                                             int *geo_mask_sum_out, unsigned char *photo_mask_out, unsigned char *final_mask_out,
+                                             double *depth_avg_out, void *stream) {
+    if (!ref_depth || !confidence || !src_flat || !views_host || !cams || !geo_mask_sum_out || !photo_mask_out || !final_mask_out ||
+        !depth_avg_out)
+        return pmb200_internal_fail(PMB200_EINVAL, "geometric_filter_views: null pointer");
+    if (V < 1 || V > kGeoMaxViews || H < 1 || W < 1 || (long long)H * W >= (1ll << 31))
+        return pmb200_internal_fail(PMB200_EINVAL, "geometric_filter_views: bad size (1 <= V <= 64)");
+    GeoViews views;
+    for (int v = 0; v < V; ++v) {
+        const pmb200_view_extent &e = views_host[v];
+        if (e.height < 1 || e.width < 1 || (long long)e.height * e.width >= (1ll << 31) || e.offset < 0)
+            return pmb200_internal_fail(PMB200_EINVAL, "geometric_filter_views: bad source extent");
+        views.v[v].offset = e.offset;
+        views.v[v].rows = e.height;
+        views.v[v].cols = e.width;
+    }
+    GeoParams p;
+    p.ref_depth = ref_depth; p.confidence = confidence; p.src_depths = src_flat; p.cams = cams;
+    p.V = V; p.H = H; p.W = W; p.Hs = views.v[0].rows; p.Ws = views.v[0].cols;
+    p.pixel_thres = geo_pixel_thres; p.depth_thres = geo_depth_thres; p.photo_thres = photo_thres; p.mask_thres = geo_mask_thres;
+    p.mask_sum = geo_mask_sum_out; p.photo_mask = photo_mask_out; p.final_mask = final_mask_out; p.depth_avg = depth_avg_out;
+    const int threads = 256;
+    const int blocks = (int)(((long long)H * W + threads - 1) / threads);
+    const size_t smem = (size_t)V * kCamDoubles * sizeof(double) + (size_t)V * sizeof(pmgeo::SourceMap);
+    geometric_filter_views_kernel<<<blocks, threads, smem, reinterpret_cast<cudaStream_t>(stream)>>>(p, views);
+    return pmb200_internal_launch_status("geometric_filter_views");
 }

@@ -130,6 +130,33 @@ PMG_HD PixelResult filter_pixel(const double *cams, const float *src_depths, int
     return r;
 }
 
+// One source depth map of a ragged pack: [rows, cols] at src_flat + offset
+struct SourceMap {
+    long long offset;
+    int rows, cols;
+};
+
+// filter_pixel with a size per source view: view v samples its own [rows_v, cols_v] map (eval.py:129 remaps each source at
+// its own size).  Same arithmetic, same order as filter_pixel.
+PMG_HD PixelResult filter_pixel(const double *cams, const float *src_flat, const SourceMap *views, int V, int x, int y, float dref,
+                                float confidence, double pixel_thres, float depth_thres, float photo_thres, int mask_thres) {
+    float sum = 0.0f;
+    int cnt = 0;
+    for (int v = 0; v < V; ++v) {
+        float drep;
+        const bool ok = check_view(cams + v * kCamDoubles, src_flat + views[v].offset, views[v].rows, views[v].cols, x, y, dref,
+                                   pixel_thres, depth_thres, &drep);
+        sum = add32(sum, ok ? drep : 0.0f);
+        cnt += ok ? 1 : 0;
+    }
+    PixelResult r;
+    r.count = cnt;
+    r.photo = confidence > photo_thres;
+    r.final = r.photo && cnt >= mask_thres;
+    r.depth_avg = (double)add32(sum, dref) / (double)(cnt + 1);
+    return r;
+}
+
 // One fused point (reference eval.py:273-281).  cam: Kref^-1 (9, row-major) | Eref^-1 (16): float32 inverses widened to double,
 // composed on the host the way numpy composes them (ops.compose_fusion_camera).  The reference multiplies (x, y, 1) by the
 // float64 averaged depth first, then applies the two matrices in float64 (BLAS: one fused multiply-add chain per output, k

@@ -9,6 +9,8 @@
 //   warp_corr3_kernel<C,G,EPI,DC,PIPE,MINB>  K-A, third generation: register/L1 gather; taken for shapes generation 4
 //                                  declines and selectable for A/B measurements (pmb200_set_tuning("ka_gen", 3));
 //                                  warp_corr_generic_kernel: any C % G == 0
+//   warp_corr3_views_kernel / warp_corr_generic_views_kernel   the same bodies with a size per source view (ragged pack)
+//                                  pmb200_warp_corr_views / _score_views / _view_weights_views
 //   aggregate_views_kernel / aggregate_score_kernel   weighted view average of stored similarities (+ head)
 //   offset_corr_kernel<C,G,HEAD>   K-A': reference self-correlation at the learned evaluation neighbours (+ head)
 //   init_propagate_kernel<NPAD>    K-C: hypothesis init + neighbour gather + warp-shuffle bitonic sort
@@ -201,6 +203,16 @@ struct WarpCorrParams {
     int ostride = 1;  // element stride of the score epilogue's output (2: the .y lane of an (xnorm, score) buffer)
 };
 
+// Per-view source extents of a ragged source pack (the *_views entry points): view v, batch b starts at float4 index
+// base4[v] + b * hs[v] * ws[v] * C / 4 of p.src; sx / sy are that view's align_corners=True scales.  Passed as a kernel
+// parameter of its own so that the uniform instantiations keep the parameter block (and the code) they always had; the
+// per-view instantiations read p.Hs / p.Ws / p.sx / p.sy from here instead.
+struct ViewTable {
+    unsigned base4[PMB200_MAX_VIEWS];
+    int hs[PMB200_MAX_VIEWS], ws[PMB200_MAX_VIEWS];
+    float sx[PMB200_MAX_VIEWS], sy[PMB200_MAX_VIEWS];
+};
+
 // Epilogue of the fused warp+correlation kernel
 constexpr int kEpiSims = 0;    // per-view similarities                 out [V,B,G,D,H,W]
 constexpr int kEpiAgg = 1;     // view-weighted average                 out [B,G,D,H,W]
@@ -271,9 +283,11 @@ __device__ __forceinline__ void dot_store(const float4 (&t)[8], const float (&r)
     }
 }
 
-template <int C, int G, int EPI, int DC, int PIPE, int MINB>
-__global__ void __launch_bounds__(kWarps2 * 32, MINB) warp_corr3_kernel(const WarpCorrParams p, const MlpParams mlp,
-                                                                  float *__restrict__ sims_out) {
+// The body of both third-generation kernels.  VIEWS = false: one (Hs, Ws) for every source view, read from p (the uniform
+// entry points; vt is null).  VIEWS = true: view v's extent and scales come from vt (the *_views entry points).
+template <int C, int G, int EPI, int DC, int PIPE, bool VIEWS>
+__device__ __forceinline__ void warp_corr3_body(const WarpCorrParams &p, const ViewTable *vt, const MlpParams &mlp,
+                                                float *__restrict__ sims_out) {
     using M = LaneMap<C, G>;
     constexpr int EPW = M::PPW * DC;   // footprints per warp pass
     static_assert(EPW % 32 == 0, "PPW * DC must be a multiple of the warp size");
@@ -327,6 +341,8 @@ __global__ void __launch_bounds__(kWarps2 * 32, MINB) warp_corr3_kernel(const Wa
         const pm::Ray ray = pm::pixel_ray(rt, px_x, px_y);
         // issued here so that its latency hides behind phase 1 (it was 10 % of the stall samples right before its use)
         const float wv = kWeighted ? __ldg(p.vw + ((size_t)b * p.V + v) * HW + nc) : 1.0f;
+        const int Hs = VIEWS ? vt->hs[v] : p.Hs, Ws = VIEWS ? vt->ws[v] : p.Ws;
+        const float sx = VIEWS ? vt->sx[v] : p.sx, sy = VIEWS ? vt->sy[v] : p.sy;
 
         // ---- phase 1: footprints, per-pixel layered numbering of the unique cells ----
         float4 w[NE];
@@ -340,8 +356,8 @@ __global__ void __launch_bounds__(kWarps2 * 32, MINB) warp_corr3_kernel(const Wa
             c.key = pm::kKeyNone;
             if (ev[k]) {
                 float uu, vv;
-                pm::project_fast(ray, rt, dep[k], p.W, p.H, p.sx, p.sy, &uu, &vv);
-                c = pm::zero_pad_cell_fast(uu, vv, p.Hs, p.Ws);
+                pm::project_fast(ray, rt, dep[k], p.W, p.H, sx, sy, &uu, &vv);
+                c = pm::zero_pad_cell_fast(uu, vv, Hs, Ws);
             }
             w[k] = make_float4(c.w00, c.w01, c.w10, c.w11);
             key[k] = c.key;
@@ -365,8 +381,9 @@ __global__ void __launch_bounds__(kWarps2 * 32, MINB) warp_corr3_kernel(const Wa
 
         // ---- phase 2a: gather layer by layer, two layers in flight ----
         const float4 *pack = reinterpret_cast<const float4 *>(p.src);
-        const unsigned row_stride = (unsigned)p.Ws * (C / 4);
-        const unsigned sv = (unsigned)(v * p.B + b) * ((unsigned)p.Hs * row_stride) + li * 2;  // float4 index of this lane's channels
+        const unsigned row_stride = (unsigned)Ws * (C / 4);
+        const unsigned sv = (VIEWS ? vt->base4[v] + (unsigned)b * ((unsigned)Hs * row_stride)
+                                   : (unsigned)(v * p.B + b) * ((unsigned)Hs * row_stride)) + li * 2;  // float4 index of this lane's channels
         const int maxc = __reduce_max_sync(full, cg);
         if constexpr (PIPE) {
             float4 ta[8], tb[8];
@@ -467,6 +484,19 @@ __global__ void __launch_bounds__(kWarps2 * 32, MINB) warp_corr3_kernel(const Wa
     }
 }
 
+template <int C, int G, int EPI, int DC, int PIPE, int MINB>
+__global__ void __launch_bounds__(kWarps2 * 32, MINB) warp_corr3_kernel(const WarpCorrParams p, const MlpParams mlp,
+                                                                  float *__restrict__ sims_out) {
+    warp_corr3_body<C, G, EPI, DC, PIPE, false>(p, nullptr, mlp, sims_out);
+}
+
+// per-view source extents (pmb200_warp_corr*_views)
+template <int C, int G, int EPI, int DC, int PIPE, int MINB>
+__global__ void __launch_bounds__(kWarps2 * 32, MINB) warp_corr3_views_kernel(const WarpCorrParams p, const ViewTable vt,
+                                                                        const MlpParams mlp, float *__restrict__ sims_out) {
+    warp_corr3_body<C, G, EPI, DC, PIPE, true>(p, &vt, mlp, sims_out);
+}
+
 // sum_v sims[v]*w_v / (1e-5 + sum_v w_v) -> SimilarityNet head -> score [B,D,H,W]   (first stage-3 iteration, eval)
 template <int G>
 __global__ void aggregate_score_kernel(const float *__restrict__ sims, const float *__restrict__ vw,
@@ -495,8 +525,9 @@ __global__ void aggregate_score_kernel(const float *__restrict__ sims, const flo
     score[idx * ostride] = mlp_eval<G>(mlp, x);
 }
 
-// Any C % G == 0: one thread per (batch, hypothesis, pixel), scalar channel loop.  Slow path.
-__global__ void warp_corr_generic_kernel(const WarpCorrParams p, int C, int G) {
+// Any C % G == 0: one thread per (batch, hypothesis, pixel), scalar channel loop.  Slow path.  VIEWS as in warp_corr3_body.
+template <bool VIEWS>
+__device__ __forceinline__ void warp_corr_generic_body(const WarpCorrParams &p, const ViewTable *vt, int C, int G) {
     const int HW = p.H * p.W;
     const size_t total = (size_t)p.B * p.D * HW;
     const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -514,15 +545,17 @@ __global__ void warp_corr_generic_kernel(const WarpCorrParams p, int C, int G) {
         for (int v = 0; v < p.V; ++v) {
             float rt[12];
             for (int i = 0; i < 12; ++i) rt[i] = p.rt[((size_t)v * p.B + b) * 12 + i];
+            const int Hs = VIEWS ? vt->hs[v] : p.Hs, Ws = VIEWS ? vt->ws[v] : p.Ws;
             float u, w;
-            pm::project(pm::pixel_ray(rt, x, y), rt, dep, p.W, p.H, p.sx, p.sy, &u, &w);
-            const pm::Cell c = pm::zero_pad_cell(u, w, p.Hs, p.Ws);
+            pm::project(pm::pixel_ray(rt, x, y), rt, dep, p.W, p.H, VIEWS ? vt->sx[v] : p.sx, VIEWS ? vt->sy[v] : p.sy, &u, &w);
+            const pm::Cell c = pm::zero_pad_cell(u, w, Hs, Ws);
             float sim = 0.0f;
             if (c.key != pm::kKeyNone) {
-                const float *base = p.src + ((size_t)v * p.B + b) * p.Hs * p.Ws * C;
+                const float *base = VIEWS ? p.src + (size_t)vt->base4[v] * 4 + (size_t)b * Hs * Ws * C
+                                          : p.src + ((size_t)v * p.B + b) * Hs * Ws * C;
                 const float *t0 = base + (size_t)pm::cell_r0(c.key) * C;
                 const float *t1 = t0 + pm::cell_dx(c.key) * C;
-                const float *t2 = t0 + (size_t)pm::cell_dy(c.key) * p.Ws * C;
+                const float *t2 = t0 + (size_t)pm::cell_dy(c.key) * Ws * C;
                 const float *t3 = t2 + pm::cell_dx(c.key) * C;
                 for (int k = g * cpg; k < (g + 1) * cpg; ++k)
                     sim += ref[k] * (c.w00 * t0[k] + c.w01 * t1[k] + c.w10 * t2[k] + c.w11 * t3[k]);
@@ -538,6 +571,12 @@ __global__ void warp_corr_generic_kernel(const WarpCorrParams p, int C, int G) {
         }
         if (fused) p.out[(((size_t)b * G + g) * p.D + d) * HW + n] = acc / wsum;
     }
+}
+
+__global__ void warp_corr_generic_kernel(const WarpCorrParams p, int C, int G) { warp_corr_generic_body<false>(p, nullptr, C, G); }
+
+__global__ void warp_corr_generic_views_kernel(const WarpCorrParams p, const ViewTable vt, int C, int G) {
+    warp_corr_generic_body<true>(p, &vt, C, G);
 }
 
 struct OffsetCorrParams {
@@ -1129,6 +1168,23 @@ const int kTuneDefaults[kTuneCount] = {3, 0, 0, -1, 0, 0, 0, 0, 0, 0, 0, 0, 2};
 int g_tune[kTuneCount] = {3, 0, 0, -1, 0, 0, 0, 0, 0, 0, 0, 0, 2};
 inline int tune(Tune t) { return __atomic_load_n(&g_tune[t], __ATOMIC_RELAXED); }
 
+// Shared memory per CTA (s_T + s_key) decides how many CTAs of the plain-gather kernel fit; asking ptxas for more than
+// that only caps the registers for nothing.
+template <int C, int G, int DC>
+constexpr int wc3_min_blocks() {
+    constexpr int kSmem = kWarps2 * LaneMap<C, G>::PPW * DC * ((4 * G + 4) * 4 + 4);
+    constexpr int kFit = (227 * 1024) / (kSmem + 1024);
+    return kFit >= 6 ? 6 : (kFit >= 5 ? 5 : 4);
+}
+
+// Rows per warp pass of the default third-generation launch
+template <int C, int G, int EPI>
+constexpr int wc3_default_dc() {
+    constexpr int PPW = LaneMap<C, G>::PPW;
+    constexpr int kDefault = PPW == 4 ? 16 : (PPW == 8 ? 8 : 4);
+    return EPI == kEpiScore ? kDefault : (PPW == 4 ? 8 : kDefault);
+}
+
 // Third-generation K-A launch (kept for shapes generation 4 does not take and for A/B measurements).
 template <int C, int G, int EPI, int DC>
 void launch_wc3(const WarpCorrParams &p, const MlpParams &m, float *sims_out, cudaStream_t st) {
@@ -1148,19 +1204,13 @@ void launch_wc3(const WarpCorrParams &p, const MlpParams &m, float *sims_out, cu
     }
     if (pipe) warp_corr3_kernel<C, G, EPI, DC, 1, 4><<<grid, kWarps2 * 32, 0, st>>>(p, m, sims_out);
     else {
-        // shared memory per CTA (s_T + s_key) decides how many CTAs fit; asking ptxas for more than that only caps the
-        // registers for nothing
-        constexpr int kSmem = kWarps2 * LaneMap<C, G>::PPW * DC * ((4 * G + 4) * 4 + 4);
-        constexpr int kFit = (227 * 1024) / (kSmem + 1024);
-        constexpr int kMinB = kFit >= 6 ? 6 : (kFit >= 5 ? 5 : 4);
-        warp_corr3_kernel<C, G, EPI, DC, 0, kMinB><<<grid, kWarps2 * 32, 0, st>>>(p, m, sims_out);
+        warp_corr3_kernel<C, G, EPI, DC, 0, wc3_min_blocks<C, G, DC>()><<<grid, kWarps2 * 32, 0, st>>>(p, m, sims_out);
     }
 }
 
 template <int C, int G, int EPI>
 void launch_wc3_auto(const WarpCorrParams &p, const MlpParams &m, float *sims_out, cudaStream_t st) {
     constexpr int PPW = LaneMap<C, G>::PPW;
-    constexpr int kDefault = PPW == 4 ? 16 : (PPW == 8 ? 8 : 4);
     if constexpr (EPI == kEpiScore || EPI == kEpiViewW) {
         const int d = tune(EPI == kEpiScore ? kTuneKa3Dc : kTuneKa3DcVw);
 #define PMB200_TRY3(DD)                                                                                  \
@@ -1173,7 +1223,17 @@ void launch_wc3_auto(const WarpCorrParams &p, const MlpParams &m, float *sims_ou
         PMB200_TRY3(4) PMB200_TRY3(8) PMB200_TRY3(16)
 #undef PMB200_TRY3
     }
-    launch_wc3<C, G, EPI, (EPI == kEpiScore ? kDefault : (PPW == 4 ? 8 : kDefault))>(p, m, sims_out, st);
+    launch_wc3<C, G, EPI, wc3_default_dc<C, G, EPI>()>(p, m, sims_out, st);
+}
+
+// Per-view K-A launch (the *_views entry points): generation 3 at its default launch shape.  The ka3_* knobs choose among
+// the uniform instantiations only; generation 4 does not take per-view extents.
+template <int C, int G, int EPI>
+void launch_wc3_views(const WarpCorrParams &p, const ViewTable &vt, const MlpParams &m, float *sims_out, cudaStream_t st) {
+    constexpr int DC = wc3_default_dc<C, G, EPI>();
+    constexpr int pix_per_block = kWarps2 * LaneMap<C, G>::PPW;
+    dim3 grid((p.H * p.W + pix_per_block - 1) / pix_per_block, (p.D + DC - 1) / DC, p.B);
+    warp_corr3_views_kernel<C, G, EPI, DC, 0, wc3_min_blocks<C, G, DC>()><<<grid, kWarps2 * 32, 0, st>>>(p, vt, m, sims_out);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1483,6 +1543,92 @@ int pmb200_warp_corr_view_weights(const float *ref_nhwc, const float *src_nhwc, 
                                   int C, int G, int H, int W, int Hs, int Ws, int D, void *stream) {
     return warp_corr_head("warp_corr_view_weights", kEpiViewW, ref_nhwc, src_nhwc, rt, depth, nullptr, head_host,
                           view_weights_out, sims_out, 1, V, B, C, G, H, W, Hs, Ws, D, stream);
+}
+
+namespace {
+// The three *_views entry points: K-A over a ragged source pack, one extent per view.  epi: kEpiSims / kEpiAgg (no head;
+// kEpiAgg when view_weights is given), kEpiScore, kEpiViewW.  Every check runs before anything is written.
+int warp_corr_views(const char *what, int epi, const float *ref_nhwc, const float *src_flat, const pmb200_view_extent *views_host,
+                    const float *rt, const float *depth, const float *view_weights, const pmb200_mlp *head_host, float *out,
+                    float *sims_out, int out_stride, int V, int B, int C, int G, int H, int W, int D, void *stream) {
+    const bool head = epi == kEpiScore || epi == kEpiViewW;
+    if (!ref_nhwc || !src_flat || !views_host || !rt || !depth || !out || (head && !head_host))
+        return fail(PMB200_EINVAL, "warp_corr views: null pointer");
+    if (epi == kEpiScore && !view_weights) return fail(PMB200_EINVAL, "warp_corr_score_views: view_weights missing");
+    if (V < 1 || V > PMB200_MAX_VIEWS || B < 1 || B > 65535 || H < 1 || W < 1 || D < 1 || (D + 3) / 4 > 65535)
+        return fail(PMB200_EINVAL, "warp_corr views: bad size");
+    if (C < 1 || G < 1 || C % G != 0) return fail(PMB200_EINVAL, "warp_corr views: C must be a multiple of G");
+    const bool fast = (C == 64 && G == 8) || (C == 32 && G == 8) || (C == 16 && G == 4);
+    if (head && !fast) return fail(PMB200_EUNSUPPORTED, "warp_corr views: fused heads exist for (C,G) in {(64,8),(32,8),(16,4)} only");
+    if (fast && (misaligned32(ref_nhwc) || misaligned32(src_flat)))
+        return fail(PMB200_EINVAL, "warp_corr views: feature packs must be 32-byte aligned (256-bit loads)");
+    ViewTable vt;
+    for (int v = 0; v < V; ++v) {
+        const pmb200_view_extent &e = views_host[v];
+        if (e.height < 1 || e.width < 1) return fail(PMB200_EINVAL, "warp_corr views: a view has a non-positive size");
+        if ((long long)e.height * e.width >= (1LL << pm::kKeyDxShift)) return fail(PMB200_EINVAL, "warp_corr views: source map too large");
+        if (e.offset < 0 || e.offset % 4 != 0) return fail(PMB200_EINVAL, "warp_corr views: offsets must be non-negative multiples of 4 floats");
+        if (e.offset / 4 >= (1LL << 31) || (e.offset + (long long)B * e.height * e.width * C) / 4 >= (1LL << 31))
+            return fail(PMB200_EINVAL, "warp_corr views: source pack too large (32-bit tap indices)");
+        vt.base4[v] = (unsigned)(e.offset / 4);
+        vt.hs[v] = e.height;
+        vt.ws[v] = e.width;
+        // F.grid_sample(align_corners=True) maps the normalised coordinate onto each source's own extent
+        vt.sx[v] = (W > 1) ? (float)(e.width - 1) / (float)(W - 1) : 1.0f;
+        vt.sy[v] = (H > 1) ? (float)(e.height - 1) / (float)(H - 1) : 1.0f;
+    }
+    WarpCorrParams p;
+    p.ref = ref_nhwc; p.src = src_flat; p.rt = rt; p.depth = depth; p.vw = view_weights; p.out = out;
+    p.V = V; p.B = B; p.H = H; p.W = W; p.Hs = vt.hs[0]; p.Ws = vt.ws[0]; p.D = D;
+    p.sx = vt.sx[0]; p.sy = vt.sy[0];
+    p.ostride = out_stride < 1 ? 1 : out_stride;
+    const MlpParams m = head ? to_device_layout(head_host) : MlpParams();
+    cudaStream_t st = as_stream(stream);
+    if (epi == kEpiViewW) {  // atomic max target starts at 0 (weights are sigmoids, > 0)
+        cudaError_t e = cudaMemsetAsync(out, 0, (size_t)B * V * H * W * sizeof(float), st);
+        if (e != cudaSuccess) return fail((int)e, "warp_corr_view_weights_views: memset failed");
+    }
+    if (epi == kEpiSims && view_weights) epi = kEpiAgg;
+#define PMB200_LAUNCH_WV(CC, GG)                                                                   \
+    do {                                                                                           \
+        if (epi == kEpiSims) launch_wc3_views<CC, GG, kEpiSims>(p, vt, m, nullptr, st);            \
+        else if (epi == kEpiAgg) launch_wc3_views<CC, GG, kEpiAgg>(p, vt, m, nullptr, st);         \
+        else if (epi == kEpiScore) launch_wc3_views<CC, GG, kEpiScore>(p, vt, m, nullptr, st);     \
+        else launch_wc3_views<CC, GG, kEpiViewW>(p, vt, m, sims_out, st);                          \
+    } while (0)
+    if (C == 64 && G == 8) PMB200_LAUNCH_WV(64, 8);
+    else if (C == 32 && G == 8) PMB200_LAUNCH_WV(32, 8);
+    else if (C == 16 && G == 4) PMB200_LAUNCH_WV(16, 4);
+    else {
+        const size_t total = (size_t)B * D * H * W;
+        warp_corr_generic_views_kernel<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(p, vt, C, G);
+    }
+#undef PMB200_LAUNCH_WV
+    return launch_status(what);
+}
+}  // namespace
+
+int pmb200_warp_corr_views(const float *ref_nhwc, const float *src_flat, const pmb200_view_extent *views_host, const float *rt,
+                           const float *depth, const float *view_weights, float *out, int V, int B, int C, int G, int H, int W,
+                           int D, void *stream) {
+    return warp_corr_views("warp_corr_views", kEpiSims, ref_nhwc, src_flat, views_host, rt, depth, view_weights, nullptr, out,
+                           nullptr, 1, V, B, C, G, H, W, D, stream);
+}
+
+int pmb200_warp_corr_score_views(const float *ref_nhwc, const float *src_flat, const pmb200_view_extent *views_host,
+                                 const float *rt, const float *depth, const float *view_weights, const pmb200_mlp *head_host,
+                                 float *score_out, int score_stride, int V, int B, int C, int G, int H, int W, int D,
+                                 void *stream) {
+    return warp_corr_views("warp_corr_score_views", kEpiScore, ref_nhwc, src_flat, views_host, rt, depth, view_weights, head_host,
+                           score_out, nullptr, score_stride, V, B, C, G, H, W, D, stream);
+}
+
+int pmb200_warp_corr_view_weights_views(const float *ref_nhwc, const float *src_flat, const pmb200_view_extent *views_host,
+                                        const float *rt, const float *depth, const pmb200_mlp *head_host,
+                                        float *view_weights_out, float *sims_out, int V, int B, int C, int G, int H, int W,
+                                        int D, void *stream) {
+    return warp_corr_views("warp_corr_view_weights_views", kEpiViewW, ref_nhwc, src_flat, views_host, rt, depth, nullptr,
+                           head_host, view_weights_out, sims_out, 1, V, B, C, G, H, W, D, stream);
 }
 
 int pmb200_aggregate_views_score(const float *sims, const float *view_weights, const pmb200_mlp *head_host,

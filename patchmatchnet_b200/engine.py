@@ -12,11 +12,16 @@ async copies on a copy stream so uploads overlap compute.
 
 The stage-3 random initialisation of each request slot draws from the slot's own generator, seeded with ``seed`` + slot
 index, so the same sequence of requests gives the same maps every run.  There is no CPU path: construction fails without CUDA.
+
+Views of different sizes (several cameras, portrait and landscape shots) take ``view_sizes``, one (H, W) per view with the
+reference first; ``height, width`` stay the reference's size, which is the size of the outputs:
+
+    eng = DepthEngine(net, 1, 3, 1200, 1600, view_sizes=[(1200, 1600), (1600, 1200), (1200, 1600)])
 """
 from __future__ import annotations
 
 import contextlib
-from typing import Dict, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -24,6 +29,8 @@ Tensor = torch.Tensor
 
 
 class DepthEngine:
+    view_sizes: Optional[List[Tuple[int, int]]] = None  # None: every view has the reference's size
+
     def __init__(
         self,
         net: torch.nn.Module,
@@ -36,9 +43,15 @@ class DepthEngine:
         warmup: int = 3,
         n_slots: int = 3,
         seed: int = 0,
+        view_sizes: Optional[Sequence[Tuple[int, int]]] = None,
     ) -> None:
         if not torch.cuda.is_available():
             raise RuntimeError("DepthEngine needs a CUDA device (H100); there is no CPU fallback")
+        # without view sizes the images of a slot are one [N,B,3,H,W] buffer, with them one [B,3,H_v,W_v] buffer per view
+        if view_sizes is not None:
+            self.view_sizes = [(int(h), int(w)) for h, w in view_sizes]
+            if len(self.view_sizes) != n_views or self.view_sizes[0] != (height, width):
+                raise ValueError("view_sizes: one (H, W) per view, the reference's (height, width) first")
         self.device = torch.device(device)
         self.net = net.eval().to(self.device)
         self.shape = (batch, n_views, height, width)
@@ -79,8 +92,12 @@ class DepthEngine:
         params = torch.zeros(n_i + n_e + 2 * B, device=dev)
         params[n_i + n_e:n_i + n_e + B] = 1.0
         params[n_i + n_e + B:] = 2.0
+        if self.view_sizes is None:
+            images = torch.zeros(N, B, 3, H, W, device=dev)
+        else:  # one buffer per view, at that view's size
+            images = [torch.zeros(B, 3, h, w, device=dev) for h, w in self.view_sizes]
         blk = dict(
-            images=torch.zeros(N, B, 3, H, W, device=dev),
+            images=images,
             params=params,
             intrinsics=params[:n_i].view(B, N, 3, 3),
             extrinsics=params[n_i:n_i + n_e].view(B, N, 4, 4),
@@ -255,7 +272,7 @@ class DepthEngine:
                 images = req["images"]
                 with torch.cuda.stream(self.copy_stream):
                     first = images[0]
-                    if len(images) == buf["images"].shape[0] and _adjacent_views(images):
+                    if self.view_sizes is None and len(images) == buf["images"].shape[0] and _adjacent_views(images):
                         stacked = torch.as_strided(first, (len(images),) + tuple(first.shape), (first.numel(),) + tuple(first.stride()))
                         buf["images"].copy_(stacked, non_blocking=True)
                         h2d += stacked.numel() * stacked.element_size()
@@ -272,7 +289,11 @@ class DepthEngine:
                 st = slot["stream"]
                 with torch.cuda.stream(st):
                     st.wait_event(buf["uploaded"])
-                    slot["images"].copy_(buf["images"], non_blocking=True)
+                    if self.view_sizes is None:
+                        slot["images"].copy_(buf["images"], non_blocking=True)
+                    else:
+                        for dst, src in zip(slot["images"], buf["images"]):
+                            dst.copy_(src, non_blocking=True)
                     slot["params"].copy_(buf["params"], non_blocking=True)
                     buf["free"].record(st)
                     depth, conf = self.run_slot(k)

@@ -9,7 +9,7 @@ an error (there is no fallback path).
 from __future__ import annotations
 
 import os
-from typing import Optional, Sequence
+from typing import List, Optional, Sequence, Tuple, Union
 
 import torch
 
@@ -125,6 +125,64 @@ def pack_nhwc(maps: Sequence[Tensor]) -> Tensor:
         rc = _native.lib().pmb200_pack_nhwc(arr, len(srcs), B, C, H, W, out.data_ptr(), _stream(first))
     _native.check(rc, "pack_nhwc")
     return out
+
+
+class ViewPack:
+    """A ragged channels-last source pack: source view v, batch item b, is [heights[v], widths[v], C] starting at float
+    offsets[v] + b * heights[v] * widths[v] * C of `data` (flat float32).  What the *_views entry points take
+    (pmb200_view_extent)."""
+
+    # every view starts on a 256-byte boundary: the gathers need 16 bytes, whole 128-byte lines keep a texel in one line
+    ALIGN_FLOATS = 64
+
+    def __init__(self, data: Tensor, offsets: Sequence[int], heights: Sequence[int], widths: Sequence[int], B: int, C: int) -> None:
+        self.data, self.B, self.C = data, int(B), int(C)
+        self.offsets, self.heights, self.widths = [int(o) for o in offsets], [int(h) for h in heights], [int(w) for w in widths]
+        ext = (_native.ViewExtent * len(self.offsets))()
+        for v, (o, h, w) in enumerate(zip(self.offsets, self.heights, self.widths)):
+            ext[v].offset, ext[v].height, ext[v].width = o, h, w
+        self.extents = ext  # host array, read by the entry points at call time
+
+    def __len__(self) -> int:
+        return len(self.offsets)
+
+    @property
+    def device(self):
+        return self.data.device
+
+    @staticmethod
+    def layout(shapes: Sequence[Tuple[int, int]], B: int, C: int) -> Tuple[List[int], int]:
+        """(float offset of every view, total floats) of a pack of views of the given (H, W)."""
+        offsets, n = [], 0
+        for h, w in shapes:
+            offsets.append(n)
+            n += -(-(B * h * w * C) // ViewPack.ALIGN_FLOATS) * ViewPack.ALIGN_FLOATS
+        return offsets, n
+
+    def view(self, v: int) -> Tensor:
+        """[B,H_v,W_v,C] view of source v (no copy)."""
+        h, w = self.heights[v], self.widths[v]
+        n = self.B * h * w * self.C
+        return self.data[self.offsets[v]:self.offsets[v] + n].view(self.B, h, w, self.C)
+
+
+def pack_nhwc_views(maps: Sequence[Tensor]) -> ViewPack:
+    """Ragged channels-last pack of n NCHW maps [B,C,H_v,W_v] that share B and C but not their size: one pmb200_pack_nhwc
+    launch per map into its slice of one buffer.  Views start on ViewPack.ALIGN_FLOATS-float boundaries."""
+    srcs = [_require(m, "feature map", 4) for m in maps]
+    B, C = srcs[0].shape[:2]
+    if any(m.shape[:2] != (B, C) for m in srcs):
+        raise RuntimeError("pack_nhwc_views: maps must share batch size and channels")
+    shapes = [tuple(m.shape[2:]) for m in srcs]
+    offsets, total = ViewPack.layout(shapes, B, C)
+    data = torch.empty(total, dtype=torch.float32, device=srcs[0].device)
+    pack = ViewPack(data, offsets, [h for h, _ in shapes], [w for _, w in shapes], B, C)
+    with _device_guard(srcs[0]):
+        for v, m in enumerate(srcs):
+            arr, keep = _native.pointer_array([m.data_ptr()])
+            rc = _native.lib().pmb200_pack_nhwc(arr, 1, B, C, shapes[v][0], shapes[v][1], data.data_ptr() + 4 * offsets[v], _stream(m))
+            _native.check(rc, "pack_nhwc_views")
+    return pack
 
 
 def photometric_confidence(prob: Tensor, out_h: int, out_w: int) -> Tensor:
@@ -503,12 +561,15 @@ def conv2d_nhwc(x: Tensor, filter_frag: Tensor, bias: Optional[Tensor], cout: in
 
 
 def warp_corr(
-    ref_nhwc: Tensor, src_nhwc: Tensor, rt: Tensor, depth: Tensor, G: int, view_weights: Optional[Tensor] = None
+    ref_nhwc: Tensor, src_nhwc: Union[Tensor, ViewPack], rt: Tensor, depth: Tensor, G: int, view_weights: Optional[Tensor] = None
 ) -> Tensor:
-    """K-A.  ref [B,H,W,C], src [V,B,Hs,Ws,C], rt [V,B,12], depth [B,D,H,W].
+    """K-A.  ref [B,H,W,C], src [V,B,Hs,Ws,C] or a ViewPack (sources of different sizes, pack_nhwc_views), rt [V,B,12],
+    depth [B,D,H,W].
 
     Without view weights: per-view similarities [V,B,G,D,H,W].  With view_weights [B,V,H,W]:
     the weighted average over views [B,G,D,H,W] (reference patchmatch.py:192-217)."""
+    if isinstance(src_nhwc, ViewPack):
+        return _warp_corr_views(ref_nhwc, src_nhwc, rt, depth, G, view_weights)
     ref = _require(ref_nhwc, "ref_nhwc", 4)
     src = _require(src_nhwc, "src_nhwc", 5)
     rt = _require(rt, "rt", 3)
@@ -533,6 +594,39 @@ def warp_corr(
             V, B, C, G, H, W, Hs, Ws, D, _stream(ref),
         )
     _native.check(rc, "warp_corr")
+    return out
+
+
+def _views_args(ref_nhwc, pack: ViewPack, rt, depth):
+    ref = _require(ref_nhwc, "ref_nhwc", 4)
+    if not _on_device(pack.data) or pack.data.dtype != torch.float32:
+        raise RuntimeError("warp_corr: the view pack must hold CUDA float32 data")
+    rt = _require(rt, "rt", 3)
+    depth = _require(depth, "depth", 4)
+    B, H, W, C = ref.shape
+    V, D = len(pack), depth.shape[1]
+    if pack.B != B or pack.C != C or rt.shape != (V, B, 12) or depth.shape != (B, D, H, W):
+        raise RuntimeError("warp_corr: inconsistent shapes")
+    return ref, rt, depth, (V, B, C, H, W, D)
+
+
+def _warp_corr_views(ref_nhwc, pack: ViewPack, rt, depth, G: int, view_weights: Optional[Tensor]) -> Tensor:
+    ref, rt, depth, (V, B, C, H, W, D) = _views_args(ref_nhwc, pack, rt, depth)
+    vw_ptr = None
+    if view_weights is not None:
+        vw = _require(view_weights, "view_weights", 4)
+        if vw.shape != (B, V, H, W):
+            raise RuntimeError("warp_corr: view_weights must be [B,V,H,W]")
+        out = torch.empty((B, G, D, H, W), dtype=torch.float32, device=ref.device)
+        vw_ptr = vw.data_ptr()
+    else:
+        out = torch.empty((V, B, G, D, H, W), dtype=torch.float32, device=ref.device)
+    with _device_guard(ref):
+        rc = _native.lib().pmb200_warp_corr_views(
+            ref.data_ptr(), pack.data.data_ptr(), pack.extents, rt.data_ptr(), depth.data_ptr(), vw_ptr, out.data_ptr(),
+            V, B, C, G, H, W, D, _stream(ref),
+        )
+    _native.check(rc, "warp_corr_views")
     return out
 
 
@@ -561,7 +655,21 @@ def _score_target(xs: Optional[Tensor], B: int, D: int, H: int, W: int, device):
 def warp_corr_score(ref_nhwc: Tensor, src_nhwc: Tensor, rt: Tensor, depth: Tensor, G: int, view_weights: Tensor,
                     head: "_native.MlpStruct", xs: Optional[Tensor] = None) -> Tensor:
     """K-A with the SimilarityNet head fused (eval mode): -> raw score [B,D,H,W]; the similarity
-    tensor is never written.  `head` holds the BN-folded weights (host struct, see PointwiseHead.folded)."""
+    tensor is never written.  `head` holds the BN-folded weights (host struct, see PointwiseHead.folded).  src_nhwc may be a
+    ViewPack (sources of different sizes)."""
+    if isinstance(src_nhwc, ViewPack):
+        ref, rt, depth, (V, B, C, H, W, D) = _views_args(ref_nhwc, src_nhwc, rt, depth)
+        vw = _require(view_weights, "view_weights", 4)
+        if vw.shape != (B, V, H, W):
+            raise RuntimeError("warp_corr_score: view_weights must be [B,V,H,W]")
+        out, out_ptr, stride = _score_target(xs, B, D, H, W, ref.device)
+        with _device_guard(ref):
+            rc = _native.lib().pmb200_warp_corr_score_views(
+                ref.data_ptr(), src_nhwc.data.data_ptr(), src_nhwc.extents, rt.data_ptr(), depth.data_ptr(), vw.data_ptr(), head,
+                out_ptr, stride, V, B, C, G, H, W, D, _stream(ref),
+            )
+        _native.check(rc, "warp_corr_score_views")
+        return out
     ref, src, rt, depth, (V, B, C, H, W, Hs, Ws, D) = _warp_args(ref_nhwc, src_nhwc, rt, depth)
     vw = _require(view_weights, "view_weights", 4)
     if vw.shape != (B, V, H, W):
@@ -579,7 +687,18 @@ def warp_corr_score(ref_nhwc: Tensor, src_nhwc: Tensor, rt: Tensor, depth: Tenso
 def warp_corr_view_weights(ref_nhwc: Tensor, src_nhwc: Tensor, rt: Tensor, depth: Tensor, G: int,
                            head: "_native.MlpStruct", keep_sims: bool = False):
     """K-A with PixelwiseNet fused (eval mode): -> pixel-wise view weights [B,V,H,W]
-    (and, keep_sims, the per-view similarities [V,B,G,D,H,W] for aggregate_views_score)."""
+    (and, keep_sims, the per-view similarities [V,B,G,D,H,W] for aggregate_views_score).  src_nhwc may be a ViewPack."""
+    if isinstance(src_nhwc, ViewPack):
+        ref, rt, depth, (V, B, C, H, W, D) = _views_args(ref_nhwc, src_nhwc, rt, depth)
+        out = torch.empty((B, V, H, W), dtype=torch.float32, device=ref.device)
+        sims = torch.empty((V, B, G, D, H, W), dtype=torch.float32, device=ref.device) if keep_sims else None
+        with _device_guard(ref):
+            rc = _native.lib().pmb200_warp_corr_view_weights_views(
+                ref.data_ptr(), src_nhwc.data.data_ptr(), src_nhwc.extents, rt.data_ptr(), depth.data_ptr(), head, out.data_ptr(),
+                None if sims is None else sims.data_ptr(), V, B, C, G, H, W, D, _stream(ref),
+            )
+        _native.check(rc, "warp_corr_view_weights_views")
+        return (out, sims) if keep_sims else out
     ref, src, rt, depth, (V, B, C, H, W, Hs, Ws, D) = _warp_args(ref_nhwc, src_nhwc, rt, depth)
     out = torch.empty((B, V, H, W), dtype=torch.float32, device=ref.device)
     sims = torch.empty((V, B, G, D, H, W), dtype=torch.float32, device=ref.device) if keep_sims else None
@@ -777,12 +896,16 @@ def compose_filter_cameras(ref_K, ref_E, src_Ks, src_Es) -> Tensor:
     return torch.from_numpy(np.stack(rows))
 
 
-def geometric_filter(ref_depth: Tensor, confidence: Tensor, src_depths: Tensor, cams: Tensor, geo_pixel_thres: float = 1.0,
-                     geo_depth_thres: float = 0.01, photo_thres: float = 0.8, geo_mask_thres: int = 3):
+def geometric_filter(ref_depth: Tensor, confidence: Tensor, src_depths: Union[Tensor, Sequence[Tensor]], cams: Tensor,
+                     geo_pixel_thres: float = 1.0, geo_depth_thres: float = 0.01, photo_thres: float = 0.8, geo_mask_thres: int = 3):
     """Geometric-consistency filtering of one reference view against V source views in one launch (reference
-    eval.py:86-190, :220-256).  ref_depth / confidence [H,W], src_depths [V,Hs,Ws] CUDA float32; cams [V,60] float64 from
+    eval.py:86-190, :220-256).  ref_depth / confidence [H,W], src_depths [V,Hs,Ws] CUDA float32, or a list of V source maps
+    [Hs_v,Ws_v] of different sizes (pmb200_geometric_filter_views); cams [V,60] float64 from
     compose_filter_cameras (moved to the device here).  -> (photo_mask bool [H,W], geo_mask_sum int32 [H,W],
     final_mask bool [H,W], depth_averaged float64 [H,W])."""
+    if not isinstance(src_depths, torch.Tensor):
+        return _geometric_filter_views(ref_depth, confidence, list(src_depths), cams, geo_pixel_thres, geo_depth_thres,
+                                       photo_thres, geo_mask_thres)
     ref = _require(ref_depth, "ref_depth", 2)
     conf = _require(confidence, "confidence", 2)
     src = _require(src_depths, "src_depths", 3)
@@ -804,6 +927,38 @@ def geometric_filter(ref_depth: Tensor, confidence: Tensor, src_depths: Tensor, 
             final.data_ptr(), avg.data_ptr(), _stream(ref),
         )
     _native.check(rc, "geometric_filter")
+    return photo.bool(), mask_sum, final.bool(), avg
+
+
+def _geometric_filter_views(ref_depth: Tensor, confidence: Tensor, src_depths: List[Tensor], cams: Tensor, geo_pixel_thres: float,
+                            geo_depth_thres: float, photo_thres: float, geo_mask_thres: int):
+    ref = _require(ref_depth, "ref_depth", 2)
+    conf = _require(confidence, "confidence", 2)
+    srcs = [_require(s, "src_depths", 2) for s in src_depths]
+    H, W = ref.shape
+    V = len(srcs)
+    if conf.shape != (H, W):
+        raise RuntimeError("geometric_filter: confidence must match ref_depth")
+    if V < 1 or cams.shape != (V, 60) or cams.dtype != torch.float64:
+        raise RuntimeError("geometric_filter: cams must be a [V,60] float64 tensor (compose_filter_cameras)")
+    flat = torch.cat([s.reshape(-1) for s in srcs])
+    ext = (_native.ViewExtent * V)()
+    off = 0
+    for v, s in enumerate(srcs):
+        ext[v].offset, ext[v].height, ext[v].width = off, s.shape[0], s.shape[1]
+        off += s.numel()
+    cams = cams.to(ref.device).contiguous()
+    mask_sum = torch.empty((H, W), dtype=torch.int32, device=ref.device)
+    photo = torch.empty((H, W), dtype=torch.uint8, device=ref.device)
+    final = torch.empty((H, W), dtype=torch.uint8, device=ref.device)
+    avg = torch.empty((H, W), dtype=torch.float64, device=ref.device)
+    with _device_guard(ref):
+        rc = _native.lib().pmb200_geometric_filter_views(
+            ref.data_ptr(), conf.data_ptr(), flat.data_ptr(), ext, cams.data_ptr(), V, H, W, float(geo_pixel_thres),
+            float(geo_depth_thres), float(photo_thres), int(geo_mask_thres), mask_sum.data_ptr(), photo.data_ptr(),
+            final.data_ptr(), avg.data_ptr(), _stream(ref),
+        )
+    _native.check(rc, "geometric_filter_views")
     return photo.bool(), mask_sum, final.bool(), avg
 
 

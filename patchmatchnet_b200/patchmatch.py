@@ -453,6 +453,10 @@ class PatchMatch(nn.Module):
         elif same_size:
             pack = ops.pack_nhwc([ref_feature] + list(src_features))
             ref_nhwc, src_nhwc = pack[0], pack[1:]
+        elif any(f.shape != src_features[0].shape for f in src_features[1:]):
+            # source views of different sizes (several cameras, mixed orientations): a ragged pack, one extent per view
+            ref_nhwc = ops.pack_nhwc([ref_feature])[0]
+            src_nhwc = ops.pack_nhwc_views(list(src_features))
         else:
             ref_nhwc = ops.pack_nhwc([ref_feature])[0]
             src_nhwc = ops.pack_nhwc(list(src_features))

@@ -11,18 +11,23 @@ Without --scan-list the input folder is one scene; with it, every line names a s
 
 Depth stage, per scan: the requests are the pair.txt entries in file order, each the reference view plus its first
 `--num-views` source views.  Every image the scan needs is decoded once (data_io.read_image) and uploaded once into a
-device-resident image bank; a request is assembled on the device (DepthEngine.set_device_inputs).  There is one DepthEngine
-per distinct (views, H, W); request j of an engine runs on slot j % n_slots, each slot on its own stream, so requests
-overlap.  Depth and confidence are copied out of the graph-owned outputs on the slot's stream into a device map bank and then
-written with data_io.save_map_from_device.  The network call is the one DepthEngine makes for any request, so the maps are
-bit-identical to a direct engine run with the same seed, slot count and request order.  Engines live for the whole call, so
-the stage-3 random initialisation continues its per-slot sequences from one scan to the next.
+device-resident image bank; a request is assembled on the device (DepthEngine.set_device_inputs).  Requests are grouped by
+their size signature, the (H, W) of every view in request order (group_requests).  There is one DepthEngine per distinct
+signature; request j of a group runs on slot j % n_slots, each slot on its own stream, so requests overlap.  Depth and
+confidence are copied out of the graph-owned outputs on the slot's stream into a device map bank and then written with
+data_io.save_map_from_device.  The network call is the one DepthEngine makes for any request, so the maps are bit-identical
+to a direct engine run with the same seed, slot count and request order.  Engines of uniform signatures (every view the
+reference's size) live for the whole call, so the stage-3 random initialisation continues its per-slot sequences from one
+scan to the next.  A signature that mixes sizes (several cameras, portrait and landscape shots) gets an engine with
+DepthEngine(view_sizes=...) and min(n_slots, group size) slots, released when its group is done, so a scene with many
+signatures does not hold one engine per signature.
 
 Fusion stage, per scan: the reference's filter_depth (eval.py:193-297) for every reference view in pair order, with every
 source view pair.txt lists for it (not only --num-views): ops.compose_filter_cameras -> ops.geometric_filter
-(pmb200_geometric_filter) -> the three mask PNGs -> ops.compose_fusion_camera -> ops.fuse_points (pmb200_fuse_points).  The
-vertex records stay on the device until data_io.save_ply writes the scan's fused.ply once.  With --output-type both the maps
-come from the map bank; with --output-type fusion each map file is read once per scan (data_io.read_map_to_device).
+(pmb200_geometric_filter; pmb200_geometric_filter_views when the source maps differ in size) -> the three mask PNGs ->
+ops.compose_fusion_camera -> ops.fuse_points (pmb200_fuse_points).  The vertex records stay on the device until
+data_io.save_ply writes the scan's fused.ply once.  With --output-type both the maps come from the map bank; with
+--output-type fusion each map file is read once per scan (data_io.read_map_to_device).
 
 Device memory held besides the engines, for a scan of n_img images of H x W and n_ref reference views:
     image bank   n_img * 3 * H * W * 4 bytes
@@ -195,42 +200,64 @@ def load_network(args: argparse.Namespace) -> PatchmatchNet:
     return net.eval()
 
 
+Signature = Tuple[Tuple[int, int], ...]
+
+
+def group_requests(signatures: Sequence[Signature]) -> Dict[Signature, List[int]]:
+    """Request indices grouped by size signature (the (H, W) of every view of a request, reference first), groups in order of
+    first appearance and requests in their order within a group."""
+    groups: Dict[Signature, List[int]] = {}
+    for j, sig in enumerate(signatures):
+        groups.setdefault(tuple(sig), []).append(j)
+    return groups
+
+
+def is_uniform(sig: Signature) -> bool:
+    """Every view of the signature has the reference view's size."""
+    return all(hw == sig[0] for hw in sig[1:])
+
+
 class DepthStage:
-    """The network side of the command: one DepthEngine (and one stream per slot) per distinct (views, H, W), kept across
-    scans."""
+    """The network side of the command: one DepthEngine (and one stream per slot) per size signature.  Engines of uniform
+    signatures are kept across scans; an engine of a mixed signature is released when its group is done."""
 
     def __init__(self, net: PatchmatchNet, device: torch.device, n_slots: int = 3, seed: int = 0) -> None:
         self.net, self.device, self.n_slots, self.seed = net, device, n_slots, seed
         self.engines: Dict[Tuple[int, int, int], Tuple[DepthEngine, List[torch.cuda.Stream]]] = {}
         self.setup_seconds = 0.0
+        self.engines_built = 0
 
-    def _engine(self, key, fill: Callable[[DepthEngine, int], None]):
+    def _build(self, sig: Signature, n_slots: int, fill: Callable[[DepthEngine, int], None]):
+        t0 = time.perf_counter()
+        h, w = sig[0]
+        eng = DepthEngine(self.net, 1, len(sig), h, w, device=str(self.device), n_slots=n_slots, seed=self.seed,
+                          view_sizes=None if is_uniform(sig) else sig)
+        for k in range(eng.n_slots):  # warm-up and capture need valid cameras in every slot
+            fill(eng, k)
+        torch.cuda.current_stream(self.device).synchronize()
+        eng.prepare()
+        self.setup_seconds += time.perf_counter() - t0
+        self.engines_built += 1
+        return eng, [torch.cuda.Stream(device=self.device) for _ in range(eng.n_slots)]
+
+    def _engine(self, sig: Signature, group_size: int, fill: Callable[[DepthEngine, int], None]):
+        if not is_uniform(sig):
+            return self._build(sig, min(self.n_slots, group_size), fill)
+        key = (len(sig),) + sig[0]
         if key not in self.engines:
-            t0 = time.perf_counter()
-            n, h, w = key
-            eng = DepthEngine(self.net, 1, n, h, w, device=str(self.device), n_slots=self.n_slots, seed=self.seed)
-            for k in range(eng.n_slots):  # warm-up and capture need valid cameras in every slot
-                fill(eng, k)
-            torch.cuda.current_stream(self.device).synchronize()
-            eng.prepare()
-            self.engines[key] = (eng, [torch.cuda.Stream(device=self.device) for _ in range(eng.n_slots)])
-            self.setup_seconds += time.perf_counter() - t0
+            self.engines[key] = self._build(sig, self.n_slots, fill)
         return self.engines[key]
 
     def run(self, bank: SceneBank, requests: Sequence[List[int]]) -> Dict[int, Tuple[Tensor, Tensor]]:
         """All requests of a scan -> {reference view: (depth [H,W], confidence [H,W])} on the device, in the map bank."""
-        groups: Dict[Tuple[int, int, int], List[int]] = {}
-        for j, views in enumerate(requests):
+        for views in requests:
             if not bank.has_range[views[0]]:
                 raise ValueError(f"view {views[0]}: its cam file has no depth range (line 12), which a depth request needs")
-            h, w = bank.shape(views[0])
-            if any(bank.shape(v) != (h, w) for v in views[1:]):
-                raise ValueError(f"request for view {views[0]}: the source images must have the reference image's size {h}x{w}")
-            groups.setdefault((len(views), h, w), []).append(j)
+        groups = group_requests([tuple(bank.shape(v) for v in views) for views in requests])
         cur = torch.cuda.current_stream(self.device)
         maps: Dict[int, Tuple[Tensor, Tensor]] = {}
-        for key, js in groups.items():
-            _, h, w = key
+        for sig, js in groups.items():
+            h, w = sig[0]
             rows = torch.tensor([[bank.row[v] for v in requests[j]] for j in js], dtype=torch.int64).to(self.device)
             out = torch.empty((len(js), 2, h, w), dtype=torch.float32, device=self.device)
 
@@ -240,7 +267,7 @@ class DepthStage:
                 eng.set_device_inputs(slot, [bank.images[v] for v in requests[js[i]]], bank.K.index_select(0, r).unsqueeze(0),
                                       bank.E.index_select(0, r).unsqueeze(0), depth_range[:, 0], depth_range[:, 1])
 
-            eng, streams = self._engine(key, fill)
+            eng, streams = self._engine(sig, len(js), fill)
             for st in streams:
                 st.wait_stream(cur)  # the banks were filled on the current stream
             for i, j in enumerate(js):
@@ -253,6 +280,11 @@ class DepthStage:
                 maps[requests[j][0]] = (out[i, 0], out[i, 1])
             for st in streams:
                 cur.wait_stream(st)
+            if not is_uniform(sig):
+                # the graphs' private memory goes back to the allocator with the engine: let the replays finish first
+                for st in streams:
+                    st.synchronize()
+                del eng, streams
         return maps
 
 
@@ -294,7 +326,9 @@ def fuse_scan(args: argparse.Namespace, scan: str, bank: SceneBank, pairs: Seque
     bodies = []
     for ref, srcs in pairs:
         ref_depth, conf = maps[ref]
-        src_depths = torch.stack([maps[s][0] for s in srcs])
+        src_list = [maps[s][0] for s in srcs]
+        same = all(d.shape == src_list[0].shape for d in src_list[1:])
+        src_depths = torch.stack(src_list) if same else src_list  # sources of different sizes: the per-view filter
         cams = ops.compose_filter_cameras(bank.intrinsics[ref], bank.extrinsics[ref], [bank.intrinsics[s] for s in srcs],
                                           [bank.extrinsics[s] for s in srcs])
         photo, mask_sum, final, avg = ops.geometric_filter(ref_depth, conf, src_depths, cams, args.geo_pixel_thres,
@@ -318,7 +352,7 @@ def reconstruct(args: argparse.Namespace, *, device: str = "cuda:0", n_slots: in
                 log: Callable[..., None] = print) -> Dict[str, float]:
     """The command's library call.  `args` as parse_args returns it.  -> seconds of the depth stage (image decoding and
     upload, engine set-up, network, map files), of the fusion stage (filter, masks, fusion, fused.ply) and end to end, plus
-    counts.  Raises before it creates any output when the arguments are invalid or there is no CUDA device."""
+    counts (scans, depth maps, points, engines built and their set-up seconds).  Raises before it creates any output when the arguments are invalid or there is no CUDA device."""
     scans = check_args(args)
     if not torch.cuda.is_available():
         raise RuntimeError("reconstruct needs a CUDA device (H100); there is no CPU fallback")
@@ -326,8 +360,8 @@ def reconstruct(args: argparse.Namespace, *, device: str = "cuda:0", n_slots: in
     do_depth = args.output_type in ("depth", "both")
     do_fusion = args.output_type in ("fusion", "both")
     os.makedirs(args.output_folder, exist_ok=True)
-    stats = {"depth_seconds": 0.0, "fusion_seconds": 0.0, "engine_setup_seconds": 0.0, "scans": len(scans), "depth_maps": 0,
-             "points": 0}
+    stats = {"depth_seconds": 0.0, "fusion_seconds": 0.0, "engine_setup_seconds": 0.0, "engines_built": 0, "scans": len(scans),
+             "depth_maps": 0, "points": 0}
     t_start = time.perf_counter()
     with precision(args.tf32), torch.cuda.device(dev), torch.no_grad():
         stage = DepthStage(load_network(args).to(dev), dev, n_slots=n_slots, seed=args.seed) if do_depth else None
@@ -355,6 +389,7 @@ def reconstruct(args: argparse.Namespace, *, device: str = "cuda:0", n_slots: in
             del bank, maps
         if stage is not None:
             stats["engine_setup_seconds"] = stage.setup_seconds
+            stats["engines_built"] = stage.engines_built
     stats["total_seconds"] = time.perf_counter() - t_start
     return stats
 
