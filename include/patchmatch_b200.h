@@ -534,6 +534,17 @@ int pmb200_warp_corr_backward(const float *ref_nhwc, const float *src_nhwc, cons
                               float *d_ref_nhwc, float *d_src_nhwc,
                               int V, int B, int C, int G, int H, int W, int Hs, int Ws, int D,
                               void *stream);
+/* pmb200_warp_corr_backward over a ragged source pack (the backward of pmb200_warp_corr_views): (Hs, Ws) replaced by one
+ * HOST extent per view.  d_src_flat has the layout of src_flat (same offsets); the call zeroes it from src_flat's first
+ * float to the end of the last view, padding between views included, then scatters into it.  Each view is exactly what
+ * pmb200_warp_corr_backward computes for a pack of that view's size.  PMB200_EINVAL, nothing written, on the forward's
+ * extent rules (V outside 1..PMB200_MAX_VIEWS, null extents, a non-positive size, height*width >= 2^29, an offset that
+ * is negative or not a multiple of 4, a pack at or beyond 2^31 float4 elements); PMB200_EUNSUPPORTED for (C,G) other
+ * than (64,8), (32,8), (16,4). */
+int pmb200_warp_corr_views_backward(const float *ref_nhwc, const float *src_flat, const pmb200_view_extent *views_host,
+                                    const float *rt, const float *depth, const float *view_weights,
+                                    const float *grad_out, float *d_ref_nhwc, float *d_src_flat,
+                                    int V, int B, int C, int G, int H, int W, int D, void *stream);
 
 /* aggregate_views backward: d_sims [V,B,G,D,H,W], d_view_weights [B,V,H,W]. */
 int pmb200_aggregate_views_backward(const float *sims, const float *view_weights, const float *grad_out,

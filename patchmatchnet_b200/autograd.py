@@ -9,7 +9,7 @@ reference feature (patchmatch.py:475).  The 1x1x1 heads stay ordinary torch modu
 """
 from __future__ import annotations
 
-from typing import Optional
+from typing import Optional, Tuple
 
 import torch
 
@@ -64,6 +64,65 @@ class WarpCorr(torch.autograd.Function):
             )
         _native.check(rc, "warp_corr_backward")
         return d_ref, d_src, None, None, None, None
+
+
+class PackNHWCViews(torch.autograd.Function):
+    """n NCHW maps [B,C,H_v,W_v] -> the flat data of their ragged channels-last pack (ops.pack_nhwc_views; rebuild the pack
+    with ops.ViewPack.from_shapes); backward hands every map its slice of the flat gradient, re-viewed as NCHW."""
+
+    @staticmethod
+    def forward(ctx, *maps: Tensor) -> Tensor:
+        pack = ops.pack_nhwc_views([m.detach() for m in maps])
+        ctx.slices = [(o, m.shape) for o, m in zip(pack.offsets, maps)]
+        return pack.data
+
+    @staticmethod
+    def backward(ctx, g: Tensor):
+        return tuple(g[o:o + s.numel()].view(s[0], s[2], s[3], s[1]).permute(0, 3, 1, 2) for o, s in ctx.slices)
+
+
+class WarpCorrViews(torch.autograd.Function):
+    """K-A over a ragged source pack: `src_flat` is the pack's data (PackNHWCViews), `shapes` the (H, W) of every source
+    view.  Gradients: reference feature, the source pack."""
+
+    @staticmethod
+    def forward(ctx, ref_nhwc: Tensor, src_flat: Tensor, rt: Tensor, depth: Tensor, view_weights: Optional[Tensor], G: int,
+                shapes: Tuple[Tuple[int, int], ...]):
+        B, _, _, C = ref_nhwc.shape
+        pack = ops.ViewPack.from_shapes(src_flat.detach(), shapes, B, C)
+        out = ops.warp_corr(ref_nhwc.detach(), pack, rt, depth.detach(), G, None if view_weights is None else view_weights.detach())
+        ctx.G, ctx.pack = G, pack
+        ctx.has_w = view_weights is not None
+        ctx.save_for_backward(ref_nhwc, rt, depth, *([view_weights] if view_weights is not None else []))
+        return out
+
+    @staticmethod
+    def backward(ctx, g: Tensor):
+        saved = ctx.saved_tensors
+        ref, rt, depth = [t.detach().contiguous() for t in saved[:3]]
+        vw = saved[3].detach().contiguous() if ctx.has_w else None
+        pack = ctx.pack
+        d_ref, d_src = warp_corr_views_backward(ref, pack, rt, depth, vw, g.contiguous(), ctx.G)
+        return d_ref, d_src, None, None, None, None, None
+
+
+def warp_corr_views_backward(ref: Tensor, pack: "ops.ViewPack", rt: Tensor, depth: Tensor, vw: Optional[Tensor], g: Tensor,
+                             G: int) -> Tuple[Tensor, Tensor]:
+    """pmb200_warp_corr_views_backward -> (d_ref [B,H,W,C], d_src: the flat gradient, laid out like pack.data)."""
+    B, H, W, C = ref.shape
+    V, D = len(pack), depth.shape[1]
+    d_ref = torch.empty_like(ref)
+    d_src = torch.empty_like(pack.data)
+    with ops._device_guard(ref):
+        rc = _native.lib().pmb200_warp_corr_views_backward(
+            ref.data_ptr(), pack.data.data_ptr(), pack.extents, rt.data_ptr(), depth.data_ptr(), _ptr(vw), g.data_ptr(),
+            d_ref.data_ptr(), d_src.data_ptr(), V, B, C, G, H, W, D, ops._stream(ref),
+        )
+    _native.check(rc, "warp_corr_views_backward")
+    end = max(o + B * h * w * C for o, h, w in zip(pack.offsets, pack.heights, pack.widths))
+    if end < d_src.numel():  # the alignment padding after the last view, which the entry point does not know about
+        d_src[end:].zero_()
+    return d_ref, d_src
 
 
 class AggregateViews(torch.autograd.Function):

@@ -85,11 +85,22 @@ struct BwdMap {
     static constexpr int GPL = CPL / CPG;
 };
 
+// Per-view source extents of a ragged source pack (pmb200_warp_corr_views_backward): view v, batch b starts at float
+// base[v] + b * hs[v] * ws[v] * C of p.src (and of p.dsrc); sx / sy are that view's align_corners=True scales.  A kernel
+// parameter of its own, so that the uniform instantiations keep the parameter block (and the code) they always had.
+struct BwdViewTable {
+    long long base[PMB200_MAX_VIEWS];
+    int hs[PMB200_MAX_VIEWS], ws[PMB200_MAX_VIEWS];
+    float sx[PMB200_MAX_VIEWS], sy[PMB200_MAX_VIEWS];
+};
+
 // One lane group (C/8 lanes) per reference pixel, all hypotheses and all views in the group.
 // d_ref is owned by the group (plain stores); d_src is scattered with 128-bit vector atomics, accumulated
 // in registers while consecutive hypotheses stay in the same source cell.
-template <int C, int G>
-__global__ void __launch_bounds__(128) warp_corr_backward_kernel(const WarpCorrBwdParams p) {
+// VIEWS = false: one (Hs, Ws) for every source view, read from p (vt is null).  VIEWS = true: view v's extent, base and
+// scales come from vt.
+template <int C, int G, bool VIEWS>
+__device__ __forceinline__ void warp_corr_backward_body(const WarpCorrBwdParams &p, const BwdViewTable *vt) {
     using M = BwdMap<C, G>;
     constexpr int V4 = C / 4;
     const int lane = threadIdx.x & 31;
@@ -123,8 +134,11 @@ __global__ void __launch_bounds__(128) warp_corr_backward_kernel(const WarpCorrB
         for (int i = 0; i < 12; ++i) rt[i] = __ldg(p.rt + ((size_t)v * p.B + b) * 12 + i);
         const pm::Ray ray = pm::pixel_ray(rt, x, y);
         const float vscale = p.vw ? __ldg(p.vw + ((size_t)b * p.V + v) * HW + n) / wsum : 1.0f;
-        const float4 *sv = reinterpret_cast<const float4 *>(p.src + ((size_t)v * p.B + b) * p.Hs * p.Ws * C) + li * 2;
-        float4 *dv = reinterpret_cast<float4 *>(p.dsrc + ((size_t)v * p.B + b) * p.Hs * p.Ws * C) + li * 2;
+        const int Hs = VIEWS ? vt->hs[v] : p.Hs, Ws = VIEWS ? vt->ws[v] : p.Ws;
+        const float sx = VIEWS ? vt->sx[v] : p.sx, sy = VIEWS ? vt->sy[v] : p.sy;
+        const size_t vbase = VIEWS ? (size_t)vt->base[v] + (size_t)b * Hs * Ws * C : ((size_t)v * p.B + b) * Hs * Ws * C;
+        const float4 *sv = reinterpret_cast<const float4 *>(p.src + vbase) + li * 2;
+        float4 *dv = reinterpret_cast<float4 *>(p.dsrc + vbase) + li * 2;
 
         int pkey = pm::kKeyNone;
         float ta[4][8], tg[4][8];
@@ -136,7 +150,7 @@ __global__ void __launch_bounds__(128) warp_corr_backward_kernel(const WarpCorrB
         auto flush = [&](int key) {
             const int r0 = pm::cell_r0(key), dx = pm::cell_dx(key), dy = pm::cell_dy(key);
             float4 *t0 = dv + (size_t)r0 * V4;
-            float4 *tp[4] = {t0, t0 + dx * V4, t0 + (size_t)dy * p.Ws * V4, t0 + (size_t)dy * p.Ws * V4 + dx * V4};
+            float4 *tp[4] = {t0, t0 + dx * V4, t0 + (size_t)dy * Ws * V4, t0 + (size_t)dy * Ws * V4 + dx * V4};
 #pragma unroll
             for (int t = 0; t < 4; ++t) {
                 atomicAdd(tp[t], make_float4(tg[t][0], tg[t][1], tg[t][2], tg[t][3]));
@@ -147,8 +161,8 @@ __global__ void __launch_bounds__(128) warp_corr_backward_kernel(const WarpCorrB
         for (int d = 0; d < p.D; ++d) {
             const float dep = __ldg(p.depth + ((size_t)b * p.D + d) * HW + n);
             float uu, vv;
-            pm::project(ray, rt, dep, p.W, p.H, p.sx, p.sy, &uu, &vv);
-            const pm::Cell c = pm::zero_pad_cell(uu, vv, p.Hs, p.Ws);
+            pm::project(ray, rt, dep, p.W, p.H, sx, sy, &uu, &vv);
+            const pm::Cell c = pm::zero_pad_cell(uu, vv, Hs, Ws);
             if (c.key == pm::kKeyNone) continue;
             float gs[M::GPL];
 #pragma unroll
@@ -161,7 +175,7 @@ __global__ void __launch_bounds__(128) warp_corr_backward_kernel(const WarpCorrB
                 if (pkey != pm::kKeyNone) flush(pkey);
                 const int r0 = pm::cell_r0(c.key), dx = pm::cell_dx(c.key), dy = pm::cell_dy(c.key);
                 const float4 *t0 = sv + (size_t)r0 * V4;
-                const float4 *tq[4] = {t0, t0 + dx * V4, t0 + (size_t)dy * p.Ws * V4, t0 + (size_t)dy * p.Ws * V4 + dx * V4};
+                const float4 *tq[4] = {t0, t0 + dx * V4, t0 + (size_t)dy * Ws * V4, t0 + (size_t)dy * Ws * V4 + dx * V4};
 #pragma unroll
                 for (int t = 0; t < 4; ++t) {
                     const float4 a = __ldg(tq[t]), bq = __ldg(tq[t] + 1);
@@ -188,6 +202,17 @@ __global__ void __launch_bounds__(128) warp_corr_backward_kernel(const WarpCorrB
     float4 *dp = reinterpret_cast<float4 *>(p.dref + ((size_t)b * HW + n) * C) + li * 2;
     dp[0] = make_float4(dref[0], dref[1], dref[2], dref[3]);
     dp[1] = make_float4(dref[4], dref[5], dref[6], dref[7]);
+}
+
+template <int C, int G>
+__global__ void __launch_bounds__(128) warp_corr_backward_kernel(const WarpCorrBwdParams p) {
+    warp_corr_backward_body<C, G, false>(p, nullptr);
+}
+
+// per-view source extents (pmb200_warp_corr_views_backward)
+template <int C, int G>
+__global__ void __launch_bounds__(128) warp_corr_backward_views_kernel(const WarpCorrBwdParams p, const BwdViewTable vt) {
+    warp_corr_backward_body<C, G, true>(p, &vt);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -525,6 +550,60 @@ int pmb200_warp_corr_backward(const float *ref_nhwc, const float *src_nhwc, cons
     else return pmb200_internal_fail(PMB200_EUNSUPPORTED, "warp_corr_backward: (C,G) must be (64,8), (32,8) or (16,4)");
 #undef PMB200_LAUNCH_WB
     return pmb200_internal_launch_status("warp_corr_backward");
+}
+
+int pmb200_warp_corr_views_backward(const float *ref_nhwc, const float *src_flat, const pmb200_view_extent *views_host,
+                                    const float *rt, const float *depth, const float *view_weights, const float *grad_out,
+                                    float *d_ref_nhwc, float *d_src_flat, int V, int B, int C, int G, int H, int W, int D,
+                                    void *stream) {
+    if (!ref_nhwc || !src_flat || !views_host || !rt || !depth || !grad_out || !d_ref_nhwc || !d_src_flat)
+        return pmb200_internal_fail(PMB200_EINVAL, "warp_corr_views_backward: null pointer");
+    if (V < 1 || V > PMB200_MAX_VIEWS || B < 1 || B > 65535 || H < 1 || W < 1 || D < 1)
+        return pmb200_internal_fail(PMB200_EINVAL, "warp_corr_views_backward: bad size");
+    if (!((C == 64 && G == 8) || (C == 32 && G == 8) || (C == 16 && G == 4)))
+        return pmb200_internal_fail(PMB200_EUNSUPPORTED, "warp_corr_views_backward: (C,G) must be (64,8), (32,8) or (16,4)");
+    // every check runs before anything is written: a rejected call leaves d_ref / d_src untouched
+    BwdViewTable vt;
+    long long end = 0;  // floats of the pack: the zero fill covers every view and the padding between views
+    for (int v = 0; v < V; ++v) {
+        const pmb200_view_extent &e = views_host[v];
+        if (e.height < 1 || e.width < 1)
+            return pmb200_internal_fail(PMB200_EINVAL, "warp_corr_views_backward: a view has a non-positive size");
+        if ((long long)e.height * e.width >= (1LL << pm::kKeyDxShift))
+            return pmb200_internal_fail(PMB200_EINVAL, "warp_corr_views_backward: source map too large");
+        if (e.offset < 0 || e.offset % 4 != 0)
+            return pmb200_internal_fail(PMB200_EINVAL, "warp_corr_views_backward: offsets must be non-negative multiples of 4 floats");
+        const long long view_end = e.offset + (long long)B * e.height * e.width * C;
+        if (e.offset / 4 >= (1LL << 31) || view_end / 4 >= (1LL << 31))
+            return pmb200_internal_fail(PMB200_EINVAL, "warp_corr_views_backward: source pack too large (2^31 float4 elements)");
+        end = view_end > end ? view_end : end;
+        vt.base[v] = e.offset;
+        vt.hs[v] = e.height;
+        vt.ws[v] = e.width;
+        // F.grid_sample(align_corners=True) maps the normalised coordinate onto each source's own extent
+        vt.sx[v] = (W > 1) ? (float)(e.width - 1) / (float)(W - 1) : 1.0f;
+        vt.sy[v] = (H > 1) ? (float)(e.height - 1) / (float)(H - 1) : 1.0f;
+    }
+    WarpCorrBwdParams p;
+    p.ref = ref_nhwc; p.src = src_flat; p.rt = rt; p.depth = depth; p.vw = view_weights; p.gout = grad_out;
+    p.dref = d_ref_nhwc; p.dsrc = d_src_flat;
+    p.V = V; p.B = B; p.H = H; p.W = W; p.Hs = vt.hs[0]; p.Ws = vt.ws[0]; p.D = D;
+    p.sx = vt.sx[0]; p.sy = vt.sy[0];
+    cudaStream_t st = as_stream(stream);
+    cudaError_t e = cudaMemsetAsync(d_src_flat, 0, (size_t)end * sizeof(float), st);
+    if (e != cudaSuccess) return pmb200_internal_fail((int)e, "warp_corr_views_backward: memset failed");
+    const int HW = H * W;
+#define PMB200_LAUNCH_WBV(CC, GG)                                                        \
+    do {                                                                                 \
+        const int pix_per_block = 4 * BwdMap<CC, GG>::PPW;                               \
+        dim3 grid((HW + pix_per_block - 1) / pix_per_block, B);                          \
+        warp_corr_backward_views_kernel<CC, GG><<<grid, 128, 0, st>>>(p, vt);            \
+    } while (0)
+    if (C == 64 && G == 8) PMB200_LAUNCH_WBV(64, 8);
+    else if (C == 32 && G == 8) PMB200_LAUNCH_WBV(32, 8);
+    else PMB200_LAUNCH_WBV(16, 4);
+#undef PMB200_LAUNCH_WBV
+    return pmb200_internal_launch_status("warp_corr_views_backward");
 }
 
 int pmb200_aggregate_views_backward(const float *sims, const float *view_weights, const float *grad_out, float *d_sims,

@@ -18,7 +18,7 @@ There is no Python fallback: without libpmb200.so every call raises ``NativeLibr
 from __future__ import annotations
 
 import os
-from typing import List
+from typing import Dict, List
 from typing import Tuple
 
 import numpy as np
@@ -111,6 +111,18 @@ def save_image(filename: str, image: np.ndarray) -> None:
     else:
         image = image.astype(np.uint8)
     Image.fromarray(image).save(filename)
+
+
+def read_image_dictionary(filename: str) -> Dict[int, str]:
+    """data_io.py:67-83 -> {image id: image file name} from an ETH3D index2prefix.txt: a count line, then "<id> <name>"
+    lines, split on single spaces."""
+    image_dict: Dict[int, str] = {}
+    with open(filename) as f:
+        num_entries = int(f.readline().strip())
+        for _ in range(num_entries):
+            parts = f.readline().strip().split(" ")
+            image_dict[int(parts[0].strip())] = parts[1].strip()
+    return image_dict
 
 
 def read_cam_file(filename: str) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:

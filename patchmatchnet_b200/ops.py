@@ -159,6 +159,12 @@ class ViewPack:
             n += -(-(B * h * w * C) // ViewPack.ALIGN_FLOATS) * ViewPack.ALIGN_FLOATS
         return offsets, n
 
+    @classmethod
+    def from_shapes(cls, data: Tensor, shapes: Sequence[Tuple[int, int]], B: int, C: int) -> "ViewPack":
+        """The pack of views of the given (H, W) over `data`, laid out by `layout` (what pack_nhwc_views builds)."""
+        offsets, _ = cls.layout(shapes, B, C)
+        return cls(data, offsets, [h for h, _ in shapes], [w for _, w in shapes], B, C)
+
     def view(self, v: int) -> Tensor:
         """[B,H_v,W_v,C] view of source v (no copy)."""
         h, w = self.heights[v], self.widths[v]
@@ -176,7 +182,7 @@ def pack_nhwc_views(maps: Sequence[Tensor]) -> ViewPack:
     shapes = [tuple(m.shape[2:]) for m in srcs]
     offsets, total = ViewPack.layout(shapes, B, C)
     data = torch.empty(total, dtype=torch.float32, device=srcs[0].device)
-    pack = ViewPack(data, offsets, [h for h, _ in shapes], [w for _, w in shapes], B, C)
+    pack = ViewPack.from_shapes(data, shapes, B, C)
     with _device_guard(srcs[0]):
         for v, m in enumerate(srcs):
             arr, keep = _native.pointer_array([m.data_ptr()])

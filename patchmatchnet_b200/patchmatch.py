@@ -443,13 +443,22 @@ class PatchMatch(nn.Module):
 
         # channels-last feature pack [1+V,B,H,W,C] (zero-copy if the producer already emitted it)
         same_size = all(f.shape == ref_feature.shape for f in src_features)
+        src_shapes: Optional[Tuple[Tuple[int, int], ...]] = None  # training over a ragged source pack: each view's (H, W)
         if need_grad:
             from . import autograd as ag  # training configuration: native forward + native backward kernels
 
-            if not same_size:
-                raise NotImplementedError("training with source maps of a different size than the reference map")
-            pack = ag.PackNHWC.apply(ref_feature, *src_features)
-            ref_nhwc, src_nhwc = pack[0], pack[1:]
+            if same_size:
+                pack = ag.PackNHWC.apply(ref_feature, *src_features)
+                ref_nhwc, src_nhwc = pack[0], pack[1:]
+            elif any(f.shape != src_features[0].shape for f in src_features[1:]):
+                # source views of different sizes: the flat data of a ragged pack travels through autograd, the
+                # per-view sizes beside it (WarpCorrViews rebuilds the pack)
+                ref_nhwc = ag.PackNHWC.apply(ref_feature)[0]
+                src_nhwc = ag.PackNHWCViews.apply(*src_features)
+                src_shapes = tuple(tuple(f.shape[2:]) for f in src_features)
+            else:
+                ref_nhwc = ag.PackNHWC.apply(ref_feature)[0]
+                src_nhwc = ag.PackNHWC.apply(*src_features)
         elif same_size:
             pack = ops.pack_nhwc([ref_feature] + list(src_features))
             ref_nhwc, src_nhwc = pack[0], pack[1:]
@@ -519,8 +528,12 @@ class PatchMatch(nn.Module):
                     )
                 score0 = None
             elif need_grad:
+                if src_shapes is None:
+                    warp_corr = lambda vw: ag.WarpCorr.apply(ref_nhwc, src_nhwc, rt, hyp, vw, self.G)
+                else:
+                    warp_corr = lambda vw: ag.WarpCorrViews.apply(ref_nhwc, src_nhwc, rt, hyp, vw, self.G, src_shapes)
                 if is_empty(view_weights):
-                    sims = ag.WarpCorr.apply(ref_nhwc, src_nhwc, rt, hyp, None, self.G)  # [V,B,G,D,H,W]
+                    sims = warp_corr(None)  # [V,B,G,D,H,W]
                     if self.training:
                         view_weights = torch.cat([self.evaluation.pixel_wise_net(sims[v]) for v in range(V)], dim=1)
                     else:
@@ -528,7 +541,7 @@ class PatchMatch(nn.Module):
                         view_weights = vw.view(V, B, H, W).permute(1, 0, 2, 3).contiguous()
                     score0 = self.evaluation.similarity_net(ag.AggregateViews.apply(sims, view_weights))
                 else:
-                    score0 = self.evaluation.similarity_net(ag.WarpCorr.apply(ref_nhwc, src_nhwc, rt, hyp, view_weights, self.G))
+                    score0 = self.evaluation.similarity_net(warp_corr(view_weights))
             elif is_empty(view_weights):
                 sims = ops.warp_corr(ref_nhwc, src_nhwc, rt, hyp, self.G)  # [V,B,G,D,H,W]
                 if self.training:

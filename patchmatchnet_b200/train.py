@@ -4,7 +4,7 @@
         --test-list lists/dtu/val.txt --num-views 4 --batch-size 4 --epochs 8 --num-light-idx 7
     python -m torch.distributed.run --nproc-per-node 8 -m patchmatchnet_b200.train ...        # one process per GPU (NCCL)
 
-Input per scan (datasets/mvs.py): pair.txt, images/[light/]%08d.jpg, cams/%08d_cam.txt, depth_gt/%08d.pfm.  Output in the
+Input per scan (datasets/mvs.py): pair.txt, images/[light/]%08d.jpg (--image-extension), cams/%08d_cam.txt, depth_gt/%08d.pfm.  Output in the
 output folder: params_%06d.ckpt ({"epoch", "model", "optimizer"}; model keys carry the reference's DataParallel "module."
 prefix, in its named_parameters order), module_%06d.pt (a TorchScript archive of the eval-mode network's state dict) and
 train_log.jsonl (one line per scalar: {"tag", "step", "value"}, the reference's TensorBoard tags).
@@ -79,6 +79,8 @@ def build_parser() -> argparse.ArgumentParser:
                     help="num of neighbors for adaptive matching cost aggregation of adaptive evaluation on stages 1,2,3")
     ap.add_argument("--tf32", action="store_true", help="TF32 operands in the convolutions (default: fp32-accurate)")
     ap.add_argument("--num-workers", type=int, default=8, help="training loader workers (validation uses half)")
+    ap.add_argument("--image-extension", type=str, default=".jpg",
+                    help="extension of the files under images/ (.png for convert_eth3d's output)")
     return ap
 
 
@@ -114,9 +116,11 @@ class MVSDataset(Dataset):
     `num_views` source views; intrinsics scaled to the read image; depth_gt/%08d.pfm read with max_dim; mask = depth_gt >=
     depth_min.  A missing ground-truth file is an error naming the path."""
 
-    def __init__(self, data_path: str, num_views: int = 10, max_dim: int = -1, scan_list: str = "", num_light_idx: int = -1) -> None:
+    def __init__(self, data_path: str, num_views: int = 10, max_dim: int = -1, scan_list: str = "", num_light_idx: int = -1,
+                 image_extension: str = ".jpg") -> None:
         super().__init__()
         self.data_path, self.num_views, self.max_dim = data_path, num_views, max_dim
+        self.image_extension = image_extension
         self.metas: List[Tuple[str, str, int, List[int]]] = []
         if os.path.isfile(scan_list):
             with open(scan_list) as f:
@@ -140,7 +144,7 @@ class MVSDataset(Dataset):
         depth_gt = mask = None
         for i, v in enumerate(view_ids):
             image, original_h, original_w = data_io.read_image(
-                os.path.join(self.data_path, scan, "images", light, "{:0>8}.jpg".format(v)), self.max_dim)
+                os.path.join(self.data_path, scan, "images", light, "{:0>8}{}".format(v, self.image_extension)), self.max_dim)
             images.append(image.transpose([2, 0, 1]))
             k, e, depth_params = data_io.read_cam_file(os.path.join(self.data_path, scan, "cams", "{:0>8}_cam.txt".format(v)))
             intrinsics.append(data_io.scale_intrinsics(k, image.shape[:2], original_h, original_w))
@@ -191,9 +195,25 @@ class GlobalBatchSampler(Sampler):
         return self.n // self.batch_size if self.drop_last else (self.n + self.batch_size - 1) // self.batch_size
 
 
+def check_view_sizes(samples: Sequence[Dict[str, object]]) -> None:
+    """Samples batched together must agree view by view in size (views may differ from each other within a sample).
+    RuntimeError naming the two sizes otherwise, instead of default_collate's stack error."""
+    first = samples[0]["images"]
+    for s in samples[1:]:
+        for v, (a, b) in enumerate(zip(first, s["images"])):
+            if tuple(a.shape[-2:]) != tuple(b.shape[-2:]):
+                raise RuntimeError(
+                    "the samples of one batch disagree in the size of view {}: {}x{} and {}x{}; data whose samples differ "
+                    "in size trains with one sample per rank (--batch-size equal to the number of processes)".format(
+                        v, a.shape[-2], a.shape[-1], b.shape[-2], b.shape[-1]))
+
+
 def collate(samples):
-    """default_collate, and None for a rank's empty share of a small last batch."""
-    return default_collate(samples) if samples else None
+    """default_collate after check_view_sizes, and None for a rank's empty share of a small last batch."""
+    if not samples:
+        return None
+    check_view_sizes(samples)
+    return default_collate(samples)
 
 
 def make_loader(dataset: Dataset, batch_size: int, shuffle: bool, num_workers: int, seed: int, rank: int, world: int) -> DataLoader:
@@ -450,8 +470,10 @@ def _run(args: argparse.Namespace, sess: Session) -> Dict[str, object]:
     torch.manual_seed(args.rand_seed)
     torch.cuda.manual_seed(args.rand_seed)
     torch.backends.cudnn.benchmark = True
-    train_set = MVSDataset(args.input_folder, args.num_views, args.image_max_dim, args.train_list, args.num_light_idx)
-    test_set = MVSDataset(args.input_folder, args.num_views, args.image_max_dim, args.test_list, args.num_light_idx)
+    train_set = MVSDataset(args.input_folder, args.num_views, args.image_max_dim, args.train_list, args.num_light_idx,
+                           args.image_extension)
+    test_set = MVSDataset(args.input_folder, args.num_views, args.image_max_dim, args.test_list, args.num_light_idx,
+                          args.image_extension)
     train_loader = make_loader(train_set, args.batch_size, True, args.num_workers, args.rand_seed, sess.rank, sess.world)
     test_loader = make_loader(test_set, args.batch_size, False, args.num_workers // 2, args.rand_seed, sess.rank, sess.world)
     result: Dict[str, object] = {"start_epoch": 0, "final": None}
