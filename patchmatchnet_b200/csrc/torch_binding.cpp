@@ -51,10 +51,11 @@ Tensor offsets_arg(const Tensor &off, int64_t B, int64_t K, int64_t H, int64_t W
     return off.contiguous();
 }
 
-// A scripted module keeps its packed offset-conv filters as CPU tensors (state-dict keys stay the reference's).  Uploading them
+// A scripted module keeps its packed / folded filters as CPU tensors (state-dict keys stay the reference's).  Uploading them
 // on every forward is an implicit host sync from pageable memory and makes the scripted model impossible to capture in a CUDA
 // graph, so device copies are cached per (source storage, version, device).  The cache holds the SOURCE tensor too: its address
-// cannot be recycled for other contents while the entry lives.  Bounded (a model has two such filters per stage).
+// cannot be recycled for other contents while the entry lives.  Bounded: a scripted PatchmatchNet holds about 50 such tensors
+// (filters and biases of FeatureNet, Refinement and the offset convs), so 512 entries serve several devices without eviction.
 Tensor device_copy_cached(const Tensor &t, const c10::Device &dev) {
     if (t.device() == dev) return t.contiguous();
     struct Entry { Tensor src, copy; };
@@ -64,8 +65,8 @@ Tensor device_copy_cached(const Tensor &t, const c10::Device &dev) {
     std::lock_guard<std::mutex> lock(mu);
     auto it = cache->find(key);
     if (it != cache->end() && it->second.src.numel() == t.numel()) return it->second.copy;
-    if (cache->size() >= 64) cache->clear();
-    Entry e{t, t.to(dev).contiguous()};
+    if (cache->size() >= 512) cache->clear();
+    Entry e{t, t.to(dev)};  // memory format preserved: ATen's convolutions get the folded filter in the layout eager hands them
     (*cache)[key] = e;
     return e.copy;
 }
@@ -384,6 +385,312 @@ Tensor conv2d_nhwc(const Tensor &x, const Tensor &filter_frag, const c10::option
     return out;
 }
 
+// ---- the rest of the eval-mode network (reference models/net.py): what a scripted PatchmatchNet calls --------------------------
+
+// optional [cout] bias on x's device (a scripted module may hold a folded bias on the CPU: cached like the filters)
+const float *bias_arg(const c10::optional<Tensor> &bias, int64_t cout, const c10::Device &dev, Tensor &keep, const char *name) {
+    if (!bias.has_value() || !bias->defined()) return nullptr;
+    TORCH_CHECK(bias->scalar_type() == at::kFloat && bias->numel() == cout, name, ": bias must have Cout float32 elements");
+    keep = device_copy_cached(*bias, dev);
+    return keep.data_ptr<float>();
+}
+
+// `out`: channels-last CUDA float32 [N,C,Ho,Wo] with C >= out_channel_offset + cout
+void check_conv_out(const Tensor &out, const Tensor &x, int64_t Ho, int64_t Wo, int64_t cout, int64_t offset, const char *name) {
+    TORCH_CHECK(out.is_cuda() && out.scalar_type() == at::kFloat && out.dim() == 4 && out.device() == x.device() &&
+                    out.size(0) == x.size(0) && out.size(2) == Ho && out.size(3) == Wo &&
+                    out.is_contiguous(at::MemoryFormat::ChannelsLast),
+                name, ": out must be a channels-last CUDA float32 [N,C,", Ho, ",", Wo, "] tensor on x's device");
+    TORCH_CHECK(offset >= 0 && offset + cout <= out.size(1), name, ": channels ", offset, "..", offset + cout,
+                " do not fit in out's ", out.size(1));
+}
+
+Tensor conv_x(const Tensor &x, const char *name) {
+    TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kFloat && x.dim() == 4,
+                name, ": x must be a 4-D CUDA float32 tensor; there is no CPU fallback");
+    return x.contiguous(at::MemoryFormat::ChannelsLast);
+}
+
+// conv2d_nhwc with every argument of pmb200_conv2d_nhwc: the bilinear x2 upsample-add epilogue (FeatureNet's top-down path),
+// the zero-stuffed transposed form (Refinement's ConvTranspose2d) and a channel window of a wider `out` (concat fusion)
+void conv2d_nhwc_out(const Tensor &x, const Tensor &filter_frag, const c10::optional<Tensor> &bias, int64_t cout, int64_t ks,
+                     int64_t stride, int64_t pad, int64_t dil, bool relu, int64_t precision, bool transposed2x,
+                     const c10::optional<Tensor> &add_up2x, Tensor &out, int64_t out_channel_offset) {
+    const Tensor xc = conv_x(x, "conv2d_nhwc_out");
+    const int64_t N = xc.size(0), cin = xc.size(1), H = xc.size(2), W = xc.size(3);
+    const int want = pmb200_conv2d_filter_floats((int)cin, (int)cout, (int)ks, (int)precision);
+    TORCH_CHECK(want > 0 && filter_frag.scalar_type() == at::kFloat && filter_frag.numel() == want,
+                "conv2d_nhwc_out: filter must be ", want, " float32 values in fragment order for this precision (pack_conv_filter)");
+    const int64_t Hv = transposed2x ? 2 * H : H, Wv = transposed2x ? 2 * W : W;
+    const int64_t Ho = (Hv + 2 * pad - dil * (ks - 1) - 1) / stride + 1, Wo = (Wv + 2 * pad - dil * (ks - 1) - 1) / stride + 1;
+    TORCH_CHECK(Ho >= 1 && Wo >= 1, "conv2d_nhwc_out: empty output");
+    check_conv_out(out, xc, Ho, Wo, cout, out_channel_offset, "conv2d_nhwc_out");
+    const float *up_ptr = nullptr;
+    if (add_up2x.has_value() && add_up2x->defined()) {
+        const Tensor &u = *add_up2x;
+        TORCH_CHECK(u.is_cuda() && u.scalar_type() == at::kFloat && u.dim() == 4 && u.is_contiguous(at::MemoryFormat::ChannelsLast),
+                    "conv2d_nhwc_out: add_up2x must be a channels-last CUDA float32 tensor");
+        TORCH_CHECK(u.size(0) == N && u.size(1) == cout && u.size(2) == Ho / 2 && u.size(3) == Wo / 2,
+                    "conv2d_nhwc_out: add_up2x must be [N,cout,Ho/2,Wo/2]");
+        up_ptr = u.data_ptr<float>();
+    }
+    c10::cuda::CUDAGuard guard(xc.device());
+    const Tensor frag = device_copy_cached(filter_frag, xc.device());
+    Tensor b;
+    const float *b_ptr = bias_arg(bias, cout, xc.device(), b, "conv2d_nhwc_out");
+    check(pmb200_conv2d_nhwc(xc.data_ptr<float>(), frag.data_ptr<float>(), b_ptr, up_ptr, out.data_ptr<float>(), (int)N, (int)H, (int)W,
+                             (int)cin, (int)cout, (int)ks, (int)stride, (int)pad, (int)dil, relu ? 1 : 0, (int)precision,
+                             transposed2x ? 1 : 0, (int)out.size(1), (int)out_channel_offset, 0, stream_of(xc)),
+          "conv2d_nhwc_out");
+}
+
+// K-D5 / K-D5h (csrc/pm_conv5.cu): the wgmma convolution, tap form (any stride) or halo-tile form (halo = true, stride 1)
+void conv2d_tc5_out(const Tensor &x, const Tensor &filter_tc5, const c10::optional<Tensor> &bias, int64_t cout, int64_t ks,
+                    int64_t stride, int64_t pad, int64_t dil, bool relu, bool halo, Tensor &out, int64_t out_channel_offset) {
+    TORCH_CHECK(!halo || stride == 1, "conv2d_tc5: the halo-tile form serves stride 1");
+    const Tensor xc = conv_x(x, "conv2d_tc5");
+    const int64_t N = xc.size(0), cin = xc.size(1), H = xc.size(2), W = xc.size(3);
+    const int want = pmb200_conv2d_tc5_filter_floats((int)cin, (int)cout, (int)ks);
+    TORCH_CHECK(want > 0 && filter_tc5.scalar_type() == at::kFloat && filter_tc5.numel() == want,
+                "conv2d_tc5: filter must be ", want, " float32 values (pack_conv_filter_tc5 / pack_conv_filter_tc5h)");
+    const int64_t Ho = (H + 2 * pad - dil * (ks - 1) - 1) / stride + 1, Wo = (W + 2 * pad - dil * (ks - 1) - 1) / stride + 1;
+    TORCH_CHECK(Ho >= 1 && Wo >= 1, "conv2d_tc5: empty output");
+    check_conv_out(out, xc, Ho, Wo, cout, out_channel_offset, "conv2d_tc5");
+    c10::cuda::CUDAGuard guard(xc.device());
+    const Tensor filt = device_copy_cached(filter_tc5, xc.device());
+    Tensor b;
+    const float *b_ptr = bias_arg(bias, cout, xc.device(), b, "conv2d_tc5");
+    if (halo) {
+        check(pmb200_conv2d_tc5h(xc.data_ptr<float>(), filt.data_ptr<float>(), b_ptr, out.data_ptr<float>(), (int)N, (int)H, (int)W,
+                                 (int)cin, (int)cout, (int)ks, (int)pad, (int)dil, relu ? 1 : 0, (int)out.size(1),
+                                 (int)out_channel_offset, stream_of(xc)),
+              "conv2d_tc5h");
+    } else {
+        check(pmb200_conv2d_tc5(xc.data_ptr<float>(), filt.data_ptr<float>(), b_ptr, out.data_ptr<float>(), (int)N, (int)H, (int)W,
+                                (int)cin, (int)cout, (int)ks, (int)stride, (int)pad, (int)dil, relu ? 1 : 0, (int)out.size(1),
+                                (int)out_channel_offset, stream_of(xc)),
+              "conv2d_tc5");
+    }
+}
+
+Tensor conv2d_tc5(const Tensor &x, const Tensor &filter_tc5, const c10::optional<Tensor> &bias, int64_t cout, int64_t ks,
+                  int64_t stride, int64_t pad, int64_t dil, bool relu, bool halo) {
+    TORCH_CHECK(x.is_cuda() && x.dim() == 4, "conv2d_tc5: x must be a 4-D CUDA float32 tensor; there is no CPU fallback");
+    const int64_t Ho = (x.size(2) + 2 * pad - dil * (ks - 1) - 1) / stride + 1, Wo = (x.size(3) + 2 * pad - dil * (ks - 1) - 1) / stride + 1;
+    TORCH_CHECK(Ho >= 1 && Wo >= 1 && stride >= 1, "conv2d_tc5: empty output");
+    Tensor out = at::empty({x.size(0), cout, Ho, Wo}, x.options().dtype(at::kFloat).memory_format(at::MemoryFormat::ChannelsLast));
+    conv2d_tc5_out(x, filter_tc5, bias, cout, ks, stride, pad, dil, relu, halo, out, 0);
+    return out;
+}
+
+// host weights of K-S / K-R: they travel in the kernel parameter block, so they must be contiguous float32 CPU tensors
+const float *host_arg(const Tensor &t, std::initializer_list<int64_t> shape, const char *what, const char *name) {
+    TORCH_CHECK(t.device().is_cpu() && t.scalar_type() == at::kFloat && t.is_contiguous() && t.sizes() == at::IntArrayRef(shape),
+                what, ": ", name, " must be a contiguous float32 HOST tensor of shape ", at::IntArrayRef(shape));
+    return t.data_ptr<float>();
+}
+
+Tensor per_image(const Tensor &t, int64_t N, const char *what, const char *name) {
+    const Tensor r = dev_f32(t.reshape({-1}), name, 1);
+    TORCH_CHECK(r.numel() == N, what, ": ", name, " must have one value per image");
+    return r;
+}
+
+// K-S: relu(conv1(relu(conv0(x)))) of FeatureNet (reference models/net.py:18-19, :44) -> [N,8,H,W] channels-last
+Tensor conv_stem(const Tensor &x_, const Tensor &w0, const Tensor &b0, const Tensor &w1, const Tensor &b1) {
+    TORCH_CHECK(x_.is_cuda() && x_.scalar_type() == at::kFloat && x_.dim() == 4 && x_.size(1) == 3,
+                "conv_stem: x must be a CUDA float32 [N,3,H,W] tensor; there is no CPU fallback");
+    const Tensor x = x_.contiguous();
+    const float *pw0 = host_arg(w0, {8, 3, 3, 3}, "conv_stem", "w0"), *pb0 = host_arg(b0, {8}, "conv_stem", "b0");
+    const float *pw1 = host_arg(w1, {8, 8, 3, 3}, "conv_stem", "w1"), *pb1 = host_arg(b1, {8}, "conv_stem", "b1");
+    c10::cuda::CUDAGuard guard(x.device());
+    Tensor y = at::empty({x.size(0), 8, x.size(2), x.size(3)}, x.options().memory_format(at::MemoryFormat::ChannelsLast));
+    check(pmb200_conv_stem(x.data_ptr<float>(), pw0, pb0, pw1, pb1, y.data_ptr<float>(), (int)x.size(0), (int)x.size(2),
+                           (int)x.size(3), stream_of(x)),
+          "conv_stem");
+    return y;
+}
+
+// K-R, half resolution (reference models/net.py:104-110) -> [N,8,h,w] channels-last
+Tensor refine_low(const Tensor &depth_half, const Tensor &depth_min, const Tensor &depth_max, const Tensor &w1, const Tensor &b1,
+                  const Tensor &w2, const Tensor &b2) {
+    const Tensor dh = dev_f32(depth_half, "depth_half", 4);
+    TORCH_CHECK(dh.size(1) == 1, "refine_low: depth_half must be [N,1,h,w]");
+    const int64_t N = dh.size(0), h = dh.size(2), w = dh.size(3);
+    const Tensor lo = per_image(depth_min, N, "refine_low", "depth_min"), hi = per_image(depth_max, N, "refine_low", "depth_max");
+    const float *pw1 = host_arg(w1, {8, 1, 3, 3}, "refine_low", "w1"), *pb1 = host_arg(b1, {8}, "refine_low", "b1");
+    const float *pw2 = host_arg(w2, {8, 8, 3, 3}, "refine_low", "w2"), *pb2 = host_arg(b2, {8}, "refine_low", "b2");
+    c10::cuda::CUDAGuard guard(dh.device());
+    Tensor y = at::empty({N, 8, h, w}, dh.options().memory_format(at::MemoryFormat::ChannelsLast));
+    check(pmb200_refine_low(dh.data_ptr<float>(), lo.data_ptr<float>(), hi.data_ptr<float>(), pw1, pb1, pw2, pb2, y.data_ptr<float>(),
+                            (int)N, (int)h, (int)w, stream_of(dh)),
+          "refine_low");
+    return y;
+}
+
+// K-R, full resolution (reference models/net.py:103, :112-120) -> depth [N,1,2h,2w]
+Tensor refine_full(const Tensor &low, const Tensor &img_, const Tensor &depth_half, const Tensor &depth_min, const Tensor &depth_max,
+                   const Tensor &wd, const Tensor &bd, const Tensor &w0, const Tensor &b0, const Tensor &w3, const Tensor &b3,
+                   const Tensor &wr) {
+    TORCH_CHECK(low.is_cuda() && low.scalar_type() == at::kFloat && low.dim() == 4 && low.size(1) == 8 &&
+                    low.is_contiguous(at::MemoryFormat::ChannelsLast),
+                "refine_full: low must be a channels-last CUDA float32 [N,8,h,w] tensor; there is no CPU fallback");
+    const int64_t N = low.size(0), h = low.size(2), w = low.size(3);
+    const Tensor img = dev_f32(img_, "img", 4), dh = dev_f32(depth_half, "depth_half", 4);
+    TORCH_CHECK(img.size(0) == N && img.size(1) == 3 && img.size(2) == 2 * h && img.size(3) == 2 * w,
+                "refine_full: img must be [", N, ",3,", 2 * h, ",", 2 * w, "]");
+    TORCH_CHECK(dh.size(0) == N && dh.size(1) == 1 && dh.size(2) == h && dh.size(3) == w,
+                "refine_full: depth_half must be [", N, ",1,", h, ",", w, "]");
+    const Tensor lo = per_image(depth_min, N, "refine_full", "depth_min"), hi = per_image(depth_max, N, "refine_full", "depth_max");
+    const float *pwd = host_arg(wd, {8, 8, 3, 3}, "refine_full", "wd"), *pbd = host_arg(bd, {8}, "refine_full", "bd");
+    const float *pw0 = host_arg(w0, {8, 3, 3, 3}, "refine_full", "w0"), *pb0 = host_arg(b0, {8}, "refine_full", "b0");
+    const float *pw3 = host_arg(w3, {8, 16, 3, 3}, "refine_full", "w3"), *pb3 = host_arg(b3, {8}, "refine_full", "b3");
+    const float *pwr = host_arg(wr, {1, 8, 3, 3}, "refine_full", "wr");
+    c10::cuda::CUDAGuard guard(low.device());
+    Tensor out = at::empty({N, 1, 2 * h, 2 * w}, low.options().memory_format(at::MemoryFormat::Contiguous));
+    check(pmb200_refine_full(low.data_ptr<float>(), img.data_ptr<float>(), dh.data_ptr<float>(), lo.data_ptr<float>(), hi.data_ptr<float>(),
+                             pwd, pbd, pw0, pb0, pw3, pb3, pwr, out.data_ptr<float>(), (int)N, (int)(2 * h), (int)(2 * w), stream_of(low)),
+          "refine_full");
+    return out;
+}
+
+// bilinear x2 upsample of x plus y (plus a per-channel bias), channels-last (FeatureNet's top-down step, models/net.py:60-66)
+Tensor upsample2x_add(const Tensor &x_, const Tensor &y_, const c10::optional<Tensor> &bias) {
+    TORCH_CHECK(x_.is_cuda() && y_.is_cuda() && x_.scalar_type() == at::kFloat && y_.scalar_type() == at::kFloat && x_.dim() == 4 &&
+                    y_.dim() == 4, "upsample2x_add: x and y must be 4-D CUDA float32 tensors; there is no CPU fallback");
+    const int64_t N = x_.size(0), C = x_.size(1), h = x_.size(2), w = x_.size(3);
+    TORCH_CHECK(y_.size(0) == N && y_.size(1) == C && y_.size(2) == 2 * h && y_.size(3) == 2 * w, "upsample2x_add: y must be [N,C,2h,2w]");
+    const Tensor x = x_.contiguous(at::MemoryFormat::ChannelsLast), y = y_.contiguous(at::MemoryFormat::ChannelsLast);
+    c10::cuda::CUDAGuard guard(x.device());
+    Tensor b;
+    const float *b_ptr = bias_arg(bias, C, x.device(), b, "upsample2x_add");
+    Tensor out = at::empty_like(y, y.options().memory_format(at::MemoryFormat::ChannelsLast));
+    check(pmb200_upsample2x_add_nhwc(x.data_ptr<float>(), y.data_ptr<float>(), b_ptr, out.data_ptr<float>(), (int)N, (int)h, (int)w, (int)C,
+                                     stream_of(x)),
+          "upsample2x_add_nhwc");
+    return out;
+}
+
+// ---- ragged source packs: views of different sizes (the *_views entry points of K-A) --------------------------------------------
+constexpr int64_t kViewAlignFloats = 64;  // every view starts on a 256-byte boundary (ops.ViewPack.ALIGN_FLOATS)
+
+// NCHW maps [B,C,H_v,W_v] sharing B and C -> (flat channels-last data, CPU int64 [V,3] extents (offset, height, width))
+std::tuple<Tensor, Tensor> pack_nhwc_views(at::TensorList maps) {
+    TORCH_CHECK(!maps.empty(), "pack_nhwc_views: no maps");
+    const Tensor &first = maps[0];
+    TORCH_CHECK(first.is_cuda() && first.scalar_type() == at::kFloat && first.dim() == 4,
+                "pack_nhwc_views: expected CUDA float32 [B,C,H,W] maps; there is no CPU fallback");
+    const int64_t V = (int64_t)maps.size(), B = first.size(0), C = first.size(1);
+    Tensor extents = at::empty({V, 3}, at::TensorOptions().dtype(at::kLong));
+    auto e = extents.accessor<int64_t, 2>();
+    int64_t total = 0;
+    std::vector<Tensor> keep;
+    for (int64_t v = 0; v < V; ++v) {
+        const Tensor &m = maps[v];
+        TORCH_CHECK(m.is_cuda() && m.scalar_type() == at::kFloat && m.dim() == 4 && m.device() == first.device() && m.size(0) == B &&
+                        m.size(1) == C, "pack_nhwc_views: maps must share batch size, channels, dtype and device");
+        keep.push_back(m.contiguous());
+        e[v][0] = total;
+        e[v][1] = m.size(2);
+        e[v][2] = m.size(3);
+        total += (B * m.size(2) * m.size(3) * C + kViewAlignFloats - 1) / kViewAlignFloats * kViewAlignFloats;
+    }
+    c10::cuda::CUDAGuard guard(first.device());
+    Tensor data = at::empty({total}, first.options().memory_format(at::MemoryFormat::Contiguous));
+    for (int64_t v = 0; v < V; ++v) {
+        const float *ptr = keep[v].data_ptr<float>();
+        check(pmb200_pack_nhwc(&ptr, 1, (int)B, (int)C, (int)e[v][1], (int)e[v][2], data.data_ptr<float>() + e[v][0], stream_of(first)),
+              "pack_nhwc_views");
+    }
+    return std::make_tuple(data, extents);
+}
+
+struct ViewsShape {
+    int V, B, C, H, W, D;
+    std::vector<pmb200_view_extent> ext;
+};
+
+ViewsShape views_shape(const Tensor &ref, const Tensor &src_flat, const Tensor &extents, const Tensor &rt, const Tensor &depth) {
+    TORCH_CHECK(src_flat.is_cuda() && src_flat.scalar_type() == at::kFloat && src_flat.dim() == 1 && src_flat.is_contiguous(),
+                "src_flat: expected the contiguous CUDA float32 data of a view pack (pack_nhwc_views)");
+    TORCH_CHECK(extents.device().is_cpu() && extents.scalar_type() == at::kLong && extents.dim() == 2 && extents.size(1) == 3,
+                "extents: expected a CPU int64 [V,3] tensor of (offset, height, width) (pack_nhwc_views)");
+    ViewsShape s;
+    s.B = (int)ref.size(0); s.H = (int)ref.size(1); s.W = (int)ref.size(2); s.C = (int)ref.size(3);
+    s.V = (int)extents.size(0); s.D = (int)depth.size(1);
+    TORCH_CHECK(rt.size(0) == s.V && rt.size(1) == s.B && rt.size(2) == 12 && depth.size(0) == s.B && depth.size(2) == s.H &&
+                    depth.size(3) == s.W, "warp_corr: inconsistent shapes");
+    const Tensor ex = extents.contiguous();
+    const int64_t *p = ex.data_ptr<int64_t>();
+    for (int v = 0; v < s.V; ++v) {
+        const int64_t off = p[3 * v], h = p[3 * v + 1], w = p[3 * v + 2];
+        TORCH_CHECK(off >= 0 && h > 0 && w > 0 && off + (int64_t)s.B * h * w * s.C <= src_flat.numel(),
+                    "warp_corr: view ", v, " (offset ", off, ", ", h, "x", w, ") does not lie inside the pack's ", src_flat.numel(), " floats");
+        s.ext.push_back(pmb200_view_extent{off, (int)h, (int)w});
+    }
+    return s;
+}
+
+Tensor warp_corr_views(const Tensor &ref_nhwc, const Tensor &src_flat, const Tensor &extents, const Tensor &rt_, const Tensor &depth_,
+                       const c10::optional<Tensor> &view_weights, int64_t G) {
+    const Tensor ref = dev_f32(ref_nhwc, "ref_nhwc", 4), rt = dev_f32(rt_, "rt", 3), depth = dev_f32(depth_, "depth", 4);
+    const ViewsShape s = views_shape(ref, src_flat, extents, rt, depth);
+    c10::cuda::CUDAGuard guard(ref.device());
+    Tensor vw, out;
+    if (view_weights.has_value() && view_weights->numel() > 0) {
+        vw = dev_f32(*view_weights, "view_weights", 4);
+        TORCH_CHECK(vw.size(0) == s.B && vw.size(1) == s.V && vw.size(2) == s.H && vw.size(3) == s.W,
+                    "warp_corr: view_weights must be [B,V,H,W]");
+        out = at::empty({s.B, G, s.D, s.H, s.W}, ref.options());
+    } else {
+        out = at::empty({s.V, s.B, G, s.D, s.H, s.W}, ref.options());
+    }
+    check(pmb200_warp_corr_views(ref.data_ptr<float>(), src_flat.data_ptr<float>(), s.ext.data(), rt.data_ptr<float>(),
+                                 depth.data_ptr<float>(), vw.defined() ? vw.data_ptr<float>() : nullptr, out.data_ptr<float>(), s.V,
+                                 s.B, s.C, (int)G, s.H, s.W, s.D, stream_of(ref)),
+          "warp_corr_views");
+    return out;
+}
+
+std::tuple<Tensor, Tensor> warp_corr_view_weights_views(const Tensor &ref_nhwc, const Tensor &src_flat, const Tensor &extents,
+                                                        const Tensor &rt_, const Tensor &depth_, const Tensor &head, int64_t G) {
+    const Tensor ref = dev_f32(ref_nhwc, "ref_nhwc", 4), rt = dev_f32(rt_, "rt", 3), depth = dev_f32(depth_, "depth", 4);
+    const ViewsShape s = views_shape(ref, src_flat, extents, rt, depth);
+    const Head h(head);
+    c10::cuda::CUDAGuard guard(ref.device());
+    Tensor vw = at::empty({s.B, s.V, s.H, s.W}, ref.options());
+    Tensor sims = at::empty({s.V, s.B, G, s.D, s.H, s.W}, ref.options());
+    check(pmb200_warp_corr_view_weights_views(ref.data_ptr<float>(), src_flat.data_ptr<float>(), s.ext.data(), rt.data_ptr<float>(),
+                                              depth.data_ptr<float>(), h.ptr, vw.data_ptr<float>(), sims.data_ptr<float>(), s.V, s.B,
+                                              s.C, (int)G, s.H, s.W, s.D, stream_of(ref)),
+          "warp_corr_view_weights_views");
+    return std::make_tuple(vw, sims);
+}
+
+void warp_corr_score_views_(const Tensor &ref_nhwc, const Tensor &src_flat, const Tensor &extents, const Tensor &rt_, const Tensor &depth_,
+                            const Tensor &view_weights, const Tensor &head, int64_t G, Tensor &xs) {
+    const Tensor ref = dev_f32(ref_nhwc, "ref_nhwc", 4), rt = dev_f32(rt_, "rt", 3), depth = dev_f32(depth_, "depth", 4);
+    const ViewsShape s = views_shape(ref, src_flat, extents, rt, depth);
+    const Tensor vw = dev_f32(view_weights, "view_weights", 4);
+    TORCH_CHECK(vw.size(0) == s.B && vw.size(1) == s.V && vw.size(2) == s.H && vw.size(3) == s.W,
+                "warp_corr_score: view_weights must be [B,V,H,W]");
+    check_xs(xs, s.B, s.D, s.H, s.W);
+    const Head h(head);
+    c10::cuda::CUDAGuard guard(ref.device());
+    check(pmb200_warp_corr_score_views(ref.data_ptr<float>(), src_flat.data_ptr<float>(), s.ext.data(), rt.data_ptr<float>(),
+                                       depth.data_ptr<float>(), vw.data_ptr<float>(), h.ptr, xs.data_ptr<float>() + 1, 2, s.V, s.B,
+                                       s.C, (int)G, s.H, s.W, s.D, stream_of(ref)),
+          "warp_corr_score_views");
+}
+
+// the cached device copy of a host-held tensor: the folded filters a scripted network hands to ATen's convolutions
+Tensor device_copy(const Tensor &t, const Tensor &like) {
+    TORCH_CHECK(like.is_cuda(), "device_copy: `like` must be a CUDA tensor");
+    c10::cuda::CUDAGuard guard(like.device());
+    if (t.device() == like.device()) return t;
+    return device_copy_cached(t, like.device());
+}
+
 int64_t abi_version() { return pmb200_abi_version(); }
 
 }  // namespace
@@ -404,10 +711,23 @@ TORCH_LIBRARY(pmb200, m) {
     m.def("adaptive_eval_planar(Tensor score0, Tensor xnorm, Tensor depth_sample, Tensor offsets, Tensor feature_weight, Tensor depth_min, Tensor depth_max, int dilation, float interval_scale, bool is_inverse) -> (Tensor, Tensor)");
     m.def("photometric_confidence(Tensor prob, int out_h, int out_w) -> Tensor");
     m.def("conv2d_nhwc(Tensor x, Tensor filter_frag, Tensor? bias, int cout, int ks, int stride, int pad, int dil, bool relu, int precision) -> Tensor");
+    m.def("conv2d_nhwc_out(Tensor x, Tensor filter_frag, Tensor? bias, int cout, int ks, int stride, int pad, int dil, bool relu, int precision, bool transposed2x, Tensor? add_up2x, Tensor(a!) out, int out_channel_offset) -> ()");
+    m.def("conv2d_tc5(Tensor x, Tensor filter_tc5, Tensor? bias, int cout, int ks, int stride, int pad, int dil, bool relu, bool halo) -> Tensor");
+    m.def("conv2d_tc5_out(Tensor x, Tensor filter_tc5, Tensor? bias, int cout, int ks, int stride, int pad, int dil, bool relu, bool halo, Tensor(a!) out, int out_channel_offset) -> ()");
+    m.def("conv_stem(Tensor x, Tensor w0, Tensor b0, Tensor w1, Tensor b1) -> Tensor");
+    m.def("refine_low(Tensor depth_half, Tensor depth_min, Tensor depth_max, Tensor w1, Tensor b1, Tensor w2, Tensor b2) -> Tensor");
+    m.def("refine_full(Tensor low, Tensor img, Tensor depth_half, Tensor depth_min, Tensor depth_max, Tensor wd, Tensor bd, Tensor w0, Tensor b0, Tensor w3, Tensor b3, Tensor wr) -> Tensor");
+    m.def("upsample2x_add(Tensor x, Tensor y, Tensor? bias) -> Tensor");
+    m.def("pack_nhwc_views(Tensor[] maps) -> (Tensor, Tensor)");
+    m.def("warp_corr_views(Tensor ref_nhwc, Tensor src_flat, Tensor extents, Tensor rt, Tensor depth, Tensor? view_weights, int G) -> Tensor");
+    m.def("warp_corr_view_weights_views(Tensor ref_nhwc, Tensor src_flat, Tensor extents, Tensor rt, Tensor depth, Tensor head, int G) -> (Tensor, Tensor)");
+    m.def("warp_corr_score_views_(Tensor ref_nhwc, Tensor src_flat, Tensor extents, Tensor rt, Tensor depth, Tensor view_weights, Tensor head, int G, Tensor(a!) xs) -> ()");
+    m.def("device_copy(Tensor t, Tensor like) -> Tensor");
 }
 
 // CUDA is the only backend: a CPU tensor reaches no kernel and the dispatcher raises, there is no fallback.
-// relative_projection / pack_nhwc take tensor lists, which dispatch on their first element.
+// relative_projection / pack_nhwc / pack_nhwc_views take tensor lists, which dispatch on their first element; the ops that take
+// host weights (conv_stem, refine_*, device_copy) dispatch on their CUDA arguments.
 TORCH_LIBRARY_IMPL(pmb200, CUDA, m) {
     m.impl("relative_projection", &relative_projection);
     m.impl("pack_nhwc", &pack_nhwc);
@@ -423,4 +743,16 @@ TORCH_LIBRARY_IMPL(pmb200, CUDA, m) {
     m.impl("adaptive_eval_planar", &adaptive_eval_planar);
     m.impl("photometric_confidence", &photometric_confidence);
     m.impl("conv2d_nhwc", &conv2d_nhwc);
+    m.impl("conv2d_nhwc_out", &conv2d_nhwc_out);
+    m.impl("conv2d_tc5", &conv2d_tc5);
+    m.impl("conv2d_tc5_out", &conv2d_tc5_out);
+    m.impl("conv_stem", &conv_stem);
+    m.impl("refine_low", &refine_low);
+    m.impl("refine_full", &refine_full);
+    m.impl("upsample2x_add", &upsample2x_add);
+    m.impl("pack_nhwc_views", &pack_nhwc_views);
+    m.impl("warp_corr_views", &warp_corr_views);
+    m.impl("warp_corr_view_weights_views", &warp_corr_view_weights_views);
+    m.impl("warp_corr_score_views_", &warp_corr_score_views_);
+    m.impl("device_copy", &device_copy);
 }

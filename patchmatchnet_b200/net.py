@@ -15,13 +15,19 @@ same shell by tests and by bench.py's CPU-baseline leg.
 """
 from __future__ import annotations
 
-from typing import Dict, List, Tuple, Type
+import os
+from typing import Dict, List, Optional, Tuple, Type
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
 Tensor = torch.Tensor
+
+
+def _freeze_after_load(module, incompatible_keys) -> None:
+    if not module.training and _freezing():
+        module.freeze_script()
 
 
 def _fold_bn(weight: Tensor, bn: nn.BatchNorm2d, out_dim: int = 0):
@@ -83,6 +89,64 @@ def ops_prefers(conv: nn.Conv2d) -> bool:
     return ops.conv_prefers_native(conv.in_channels, conv.out_channels, conv.kernel_size[0])
 
 
+# ---- TorchScript -------------------------------------------------------------------------------------------------------------
+# A scripted network runs the eval-mode launch sequence of the eager one through `torch.ops.pmb200.*` (csrc/torch_binding.cpp).
+# What eager decides per call from module-level switches (ops.NATIVE_CONVS, ops.conv_precision(), ops.conv_tc5_mode, ...) and
+# the folded / packed weights it caches are frozen when the module goes to eval mode (eval(), or load_state_dict in eval mode):
+# the call the reference makes right before torch.jit.script (train.py:52-53).  Frozen values are plain HOST tensors and Python
+# scalars, never state-dict entries; the operators keep device copies of the host tensors (one upload per device).
+# Native conv forms: 0 = the mma.sync kernel (conv2d_nhwc, fragment-ordered filter), 1 = the wgmma tap form, 2 = the wgmma
+# halo-tile form (conv2d_tc5).  Layer modes: 0 = the reference op sequence, 1 = ATen's convolution on the folded weights, 2 = native.
+
+
+def _freezing() -> bool:
+    """False in a process that must not map the native libraries (PMB200_SKIP_TORCH_OPS=1, bench.py's reference arm): the
+    freeze asks the library which conv forms it serves."""
+    return os.environ.get("PMB200_SKIP_TORCH_OPS") != "1"
+
+
+def _host(t: Tensor) -> Tensor:
+    return t.detach().float().cpu()
+
+
+def _freeze_native(weight: Tensor, stride: int, transposed: bool = False) -> Tuple[int, Tensor]:
+    """(form, host filter image) of the native conv eager runs for this filter."""
+    from . import ops
+
+    cout, cin, ks = weight.shape[0], weight.shape[1], weight.shape[2]
+    mode = "" if transposed else ops.conv_tc5_mode(cin, cout, ks, stride)
+    with torch.no_grad():
+        if mode:
+            return (2 if mode == "halo" else 1), _host(ops.pack_conv_filter_tc5_for(weight, mode))
+        return 0, _host(ops.pack_conv_filter(weight, ops.conv_precision(), transposed=transposed))
+
+
+def _script_conv(x: Tensor, form: int, filt: Tensor, bias: Optional[Tensor], cout: int, ks: int, stride: int, pad: int, dil: int,
+                 relu: bool, precision: int, out: Optional[Tensor] = None, out_channel_offset: int = 0,
+                 add_up2x: Optional[Tensor] = None, transposed2x: bool = False) -> Tensor:
+    """A native conv in the scripted forward: ops.conv2d_nhwc (form 0) or ops.conv2d_tc5 (forms 1, 2), written into `out` at a
+    channel offset when given, else into a new channels-last tensor."""
+    H, W = x.size(2), x.size(3)
+    if transposed2x:
+        H, W = 2 * H, 2 * W
+    if out is None:
+        Ho = (H + 2 * pad - dil * (ks - 1) - 1) // stride + 1
+        Wo = (W + 2 * pad - dil * (ks - 1) - 1) // stride + 1
+        out = torch.empty([x.size(0), cout, Ho, Wo], dtype=torch.float32, device=x.device, memory_format=torch.channels_last)
+    if form == 0:
+        torch.ops.pmb200.conv2d_nhwc_out(x, filt, bias, cout, ks, stride, pad, dil, relu, precision, transposed2x, add_up2x, out,
+                                         out_channel_offset)
+    else:
+        torch.ops.pmb200.conv2d_tc5_out(x, filt, bias, cout, ks, stride, pad, dil, relu, form == 2, out, out_channel_offset)
+    return out
+
+
+def _nonempty(t: Tensor) -> Optional[Tensor]:
+    if t.numel() == 0:
+        return None
+    return t
+
+
 class _PackedConv:
     """Fragment-ordered filter (+ bias) of a plain nn.Conv2d, cached until the weights change or move."""
 
@@ -122,6 +186,49 @@ class _ConvBnReLU2d(nn.Module):
         self._cache = _FoldCache()
         self._frag_cache = _FoldCache()
         self._tc5_cache = _FoldCache()
+        self._k, self._stride, self._pad, self._cout = k, stride, pad, cout
+        # scripted forward, frozen by freeze_script (see "TorchScript" above)
+        self._s_mode = 0
+        self._s_fused_relu = _FUSED_CONV_RELU
+        self._s_form = 0  # native form
+        self._s_precision = 3
+        self._s_native_w = torch.zeros(0)  # folded filter image for the native form, folded bias
+        self._s_native_b = torch.zeros(0)
+        self._s_lib_w = torch.zeros(0)  # folded channels-last filter and bias for ATen's convolution
+        self._s_lib_b = torch.zeros(0)
+
+    def freeze_script(self) -> None:
+        """Freeze the layer's eval-mode decisions and folded weights for the scripted forward."""
+        from . import ops
+
+        native = ops.NATIVE_CONVS and ops_prefers(self.conv)
+        self._s_mode = 0 if not LIBRARY_FAST_PATH else (2 if native else 1)
+        self._s_precision = ops.conv_precision()
+        with torch.no_grad():
+            if ops.NATIVE_CONVS:  # Refinement's native tail calls the native form whatever the layer prefers
+                mode = ops.conv_tc5_mode(self.conv.in_channels, self.conv.out_channels, self._k, self._stride)
+                frag, b = self.folded_tc5(mode) if mode else self.folded_frag()
+                self._s_form = (2 if mode == "halo" else 1) if mode else 0
+                self._s_native_w, self._s_native_b = _host(frag), _host(b)
+            if self._s_mode == 1:
+                w, b = self.folded()
+                self._s_lib_w, self._s_lib_b = _host(w), _host(b)
+
+    def native_script(self, x: Tensor, out: Optional[Tensor] = None, out_channel_offset: int = 0) -> Tensor:
+        return _script_conv(x, self._s_form, self._s_native_w, self._s_native_b, self._cout, self._k, self._stride, self._pad, 1, True,
+                            self._s_precision, out, out_channel_offset)
+
+    def _forward_script(self, x: Tensor) -> Tensor:
+        if self._s_mode == 2:
+            return self.native_script(x)
+        if self._s_mode == 1:
+            w = torch.ops.pmb200.device_copy(self._s_lib_w, x)
+            b = torch.ops.pmb200.device_copy(self._s_lib_b, x)
+            s, p = [self._stride, self._stride], [self._pad, self._pad]
+            if self._s_fused_relu:
+                return torch.cudnn_convolution_relu(x, w, b, s, p, [1, 1], 1)
+            return F.relu_(F.conv2d(x, w, b, s, p, [1, 1]))
+        return F.relu(self.bn(self.conv(x)), inplace=True)
 
     def folded_frag(self):
         """(fragment-ordered folded filter, folded bias) for the native conv."""
@@ -175,6 +282,12 @@ class _ConvBnReLU2d(nn.Module):
         return self._cache.get(srcs, make)
 
     def forward(self, x: Tensor) -> Tensor:
+        if torch.jit.is_scripting():
+            return self._forward_script(x)
+        return self._forward_eager(x)
+
+    @torch.jit.unused
+    def _forward_eager(self, x: Tensor) -> Tensor:
         if self.training or not _fast(x):
             return F.relu(self.bn(self.conv(x)), inplace=True)
         c = self.conv
@@ -210,6 +323,101 @@ class FeatureNet(nn.Module):
         self._composed_cache = _FoldCache()
         self._stem_cache = _FoldCache()
         self.fuse_top_down = True  # eval mode on CUDA: composed 1x1 heads (see composed_heads); False = layer by layer
+        # scripted forward, frozen by freeze_script (see "TorchScript" above)
+        self._s_fast = True
+        self._s_native = True
+        self._s_stem_fused = False
+        self._s_stem = [torch.zeros(0)] * 4  # stem_weights()
+        self._s_top_down = 0  # 0 = the reference's, 1 = layer by layer (native or ATen lateral conv), 2 = composed heads
+        self._s_precision = 3
+        self._s_plain_form: Dict[str, int] = {}  # the plain 1x1 convs (_plain), by name: form, filter image, bias (empty: none)
+        self._s_plain_w: Dict[str, Tensor] = {}
+        self._s_plain_b: Dict[str, Tensor] = {}
+        self._s_composed: Dict[str, Tensor] = {}  # composed_heads(), filters packed
+        self.register_load_state_dict_post_hook(_freeze_after_load)
+
+    def train(self, mode: bool = True):
+        super().train(mode)
+        if not mode and _freezing():
+            self.freeze_script()
+        return self
+
+    def freeze_script(self) -> None:
+        """Freeze the eval-mode decisions and folded weights of the scripted forward: the stem, each layer's conv form, the
+        top-down path (following fuse_top_down) and its filters."""
+        from . import ops
+
+        for i in range(11):
+            getattr(self, f"conv{i}").freeze_script()
+        self._s_fast = LIBRARY_FAST_PATH
+        self._s_native = LIBRARY_FAST_PATH and ops.NATIVE_CONVS
+        self._s_precision = ops.conv_precision()
+        self._s_stem_fused = self._s_native and ops.STEM_FUSED and self._s_precision == 3
+        self._s_stem = [_host(t) for t in self.stem_weights()] if self._s_stem_fused else [torch.zeros(0)] * 4
+        self._s_top_down = 0 if not LIBRARY_FAST_PATH else (2 if self._s_native and self.fuse_top_down else 1)
+        self._s_plain_form, self._s_plain_w, self._s_plain_b, self._s_composed = {}, {}, {}, {}
+        if self._s_native:
+            for name in ("output1", "inner1", "inner2", "output2", "output3"):
+                conv = getattr(self, name)
+                self._s_plain_form[name], self._s_plain_w[name] = _freeze_native(conv.weight, 1)
+                self._s_plain_b[name] = torch.zeros(0) if conv.bias is None else _host(conv.bias)
+        if self._s_top_down == 2:
+            with torch.no_grad():
+                for k, v in self.composed_heads().items():
+                    self._s_composed[k] = _host(ops.pack_conv_filter(v, self._s_precision) if v.dim() == 4 else v)
+
+    def _forward_script(self, x: Tensor) -> Dict[int, Tensor]:
+        if self.training:
+            raise RuntimeError("a scripted patchmatchnet_b200 network is inference-only; call eval() before torch.jit.script")
+        if self._s_stem_fused and x.dim() == 4 and x.size(1) == 3 and x.dtype == torch.float32:
+            y = torch.ops.pmb200.conv_stem(x, self._s_stem[0], self._s_stem[1], self._s_stem[2], self._s_stem[3])
+        else:
+            if self._s_fast and not x.is_contiguous(memory_format=torch.channels_last):
+                x = x.contiguous(memory_format=torch.channels_last)
+            y = self.conv1(self.conv0(x))
+        half = self.conv4(self.conv3(self.conv2(y)))
+        quarter = self.conv7(self.conv6(self.conv5(half)))
+        eighth = self.conv10(self.conv9(self.conv8(quarter)))
+        out: Dict[int, Tensor] = {3: self._plain_script("output1", eighth)}
+        if self._s_top_down == 2:  # _fused_top_down
+            w, p = self._s_composed, self._s_precision
+            u_o = _script_conv(eighth, 0, w["u_o"], None, 32, 1, 1, 0, 1, False, p)
+            u_t = _script_conv(eighth, 0, w["u_t"], None, 16, 1, 1, 0, 1, False, p)
+            out[2] = _script_conv(quarter, 0, w["l2_o"], w["c2_o"], 32, 1, 1, 0, 1, False, p, add_up2x=u_o)
+            t = _script_conv(quarter, 0, w["l2_t"], w["c2_t"], 16, 1, 1, 0, 1, False, p, add_up2x=u_t)
+            out[1] = _script_conv(half, 0, w["l1"], w["c1"], 16, 1, 1, 0, 1, False, p, add_up2x=t)
+            return out
+        top = self._top_down_script(eighth, "inner1", quarter)
+        out[2] = self._plain_script("output2", top)
+        top = self._top_down_script(top, "inner2", half)
+        out[1] = self._plain_script("output3", top)
+        return out
+
+    def _plain_script(self, name: str, x: Tensor) -> Tensor:
+        if self._s_native:
+            cout = 64 if name == "output1" else (32 if name == "output2" else 16)
+            return _script_conv(x, self._s_plain_form[name], self._s_plain_w[name], _nonempty(self._s_plain_b[name]), cout, 1, 1, 0, 1,
+                                False, self._s_precision)
+        if name == "output1":
+            return self.output1(x)
+        if name == "output2":
+            return self.output2(x)
+        return self.output3(x)
+
+    def _top_down_script(self, coarse: Tensor, lateral_name: str, fine: Tensor) -> Tensor:
+        if lateral_name == "inner1":
+            weight, bias = self.inner1.weight, self.inner1.bias
+        else:
+            weight, bias = self.inner2.weight, self.inner2.bias
+        if self._s_top_down == 0:
+            lateral = self.inner1(fine) if lateral_name == "inner1" else self.inner2(fine)
+            return F.interpolate(coarse, scale_factor=2.0, mode="bilinear", align_corners=False) + lateral
+        if self._s_native:
+            lateral = _script_conv(fine, self._s_plain_form[lateral_name], self._s_plain_w[lateral_name], None, 64, 1, 1, 0, 1, False,
+                                   self._s_precision)
+        else:
+            lateral = F.conv2d(fine, weight, None)
+        return torch.ops.pmb200.upsample2x_add(coarse, lateral, bias)
 
     def _plain(self, name: str, x: Tensor) -> Tensor:
         """One of the bias-free / lateral 1x1 convs: native in eval mode on CUDA, else the module itself."""
@@ -286,6 +494,12 @@ class FeatureNet(nn.Module):
         return self._trunk(x, 0, 1)
 
     def forward(self, x: Tensor) -> Dict[int, Tensor]:
+        if torch.jit.is_scripting():
+            return self._forward_script(x)
+        return self._forward_eager(x)
+
+    @torch.jit.unused
+    def _forward_eager(self, x: Tensor) -> Dict[int, Tensor]:
         half = self._trunk(self._stem(x), 2, 4)
         quarter = self._trunk(half, 5, 7)
         eighth = self._trunk(quarter, 8, 10)
@@ -330,6 +544,80 @@ class Refinement(nn.Module):
         self._deconv_frag = _FoldCache()
         self._host_cache = _FoldCache()
         self._res_packed = _PackedConv()
+        # scripted forward, frozen by freeze_script (see "TorchScript" above)
+        self._s_fast = True
+        self._s_native = True
+        self._s_fused = False
+        self._s_host = [torch.zeros(0)] * 11  # host_weights() for K-R
+        self._s_precision = 3
+        self._s_deconv_w = torch.zeros(0)  # native tail: transposed conv (fragment order) and bias, residual conv form and filter
+        self._s_deconv_b = torch.zeros(0)
+        self._s_res_form = 0
+        self._s_res_w = torch.zeros(0)
+        self._s_up_w = torch.zeros(0)  # ATen tail: folded transposed conv
+        self._s_up_b = torch.zeros(0)
+        self.register_load_state_dict_post_hook(_freeze_after_load)
+
+    def train(self, mode: bool = True):
+        super().train(mode)
+        if not mode and _freezing():
+            self.freeze_script()
+        return self
+
+    def freeze_script(self) -> None:
+        """Freeze the eval-mode decisions and folded weights of the scripted forward: K-R, or the conv-family tail."""
+        from . import ops
+
+        for m in (self.conv0, self.conv1, self.conv2, self.conv3):
+            m.freeze_script()
+        self._s_fast = LIBRARY_FAST_PATH
+        self._s_native = LIBRARY_FAST_PATH and ops.NATIVE_CONVS
+        self._s_precision = ops.conv_precision()
+        self._s_fused = self._s_native and ops.REFINE_FUSED and self._s_precision == 3 and self.res.bias is None
+        self._s_host = [_host(t) for t in self.host_weights()] if self._s_fused else [torch.zeros(0)] * 11
+        with torch.no_grad():
+            if self._s_native:
+                w, b = _fold_bn(self.deconv.weight, self.bn, out_dim=1)
+                self._s_deconv_w, self._s_deconv_b = _host(ops.pack_conv_filter(w, self._s_precision, transposed=True)), _host(b)
+                self._s_res_form, self._s_res_w = _freeze_native(self.res.weight, 1)
+            if self._s_fast:
+                w, b = _fold_bn(self.deconv.weight, self.bn, out_dim=1)
+                self._s_up_w, self._s_up_b = _host(w), _host(b)
+
+    def _forward_script(self, img: Tensor, depth_half: Tensor, depth_min: Tensor, depth_max: Tensor) -> Tensor:
+        if self.training:
+            raise RuntimeError("a scripted patchmatchnet_b200 network is inference-only; call eval() before torch.jit.script")
+        if (self._s_fused and img.dtype == torch.float32 and img.size(-2) == 2 * depth_half.size(-2)
+                and img.size(-1) == 2 * depth_half.size(-1)):
+            hw = self._s_host
+            dh, lo, hi = depth_half.float(), depth_min.float(), depth_max.float()
+            low = torch.ops.pmb200.refine_low(dh, lo, hi, hw[0], hw[1], hw[2], hw[3])
+            return torch.ops.pmb200.refine_full(low, img, dh, lo, hi, hw[4], hw[5], hw[6], hw[7], hw[8], hw[9], hw[10])
+        B = depth_min.size(0)
+        lo = depth_min.view(B, 1, 1, 1)
+        span = (depth_max - depth_min).view(B, 1, 1, 1)
+        d = (depth_half - lo) / span
+        if self._s_fast:
+            img = img.contiguous(memory_format=torch.channels_last)
+        if self._s_native and img.size(-2) == 2 * d.size(-2) and img.size(-1) == 2 * d.size(-1):  # _native_tail
+            low = self.conv2.native_script(self.conv1.native_script(d))
+            both = torch.empty([low.size(0), 16, 2 * low.size(2), 2 * low.size(3)], dtype=torch.float32, device=low.device,
+                               memory_format=torch.channels_last)
+            _script_conv(low, 0, self._s_deconv_w, self._s_deconv_b, 8, 3, 1, 1, 1, True, self._s_precision, both, 0,
+                         transposed2x=True)
+            self.conv0.native_script(img, both, 8)
+            res = _script_conv(self.conv3.native_script(both), self._s_res_form, self._s_res_w, None, 1, 3, 1, 1, 1, False,
+                               self._s_precision)
+        else:
+            x = self.conv2(self.conv1(d))
+            if self._s_fast:
+                up = F.relu_(F.conv_transpose2d(x, torch.ops.pmb200.device_copy(self._s_up_w, x),
+                                                torch.ops.pmb200.device_copy(self._s_up_b, x), stride=2, padding=1, output_padding=1))
+            else:
+                up = F.relu(self.bn(self.deconv(x)), inplace=True)
+            res = self.res(self.conv3(torch.cat((up, self.conv0(img)), dim=1)))
+        d = F.interpolate(d, scale_factor=2.0, mode="nearest") + res
+        return d * span + lo
 
     def _native_tail(self, img: Tensor, d: Tensor) -> Tensor:
         """conv1 -> conv2 -> transposed conv (BatchNorm folded, ReLU) and conv0(img) written straight into the two
@@ -389,6 +677,12 @@ class Refinement(nn.Module):
         return ops.refine_full(low, img, depth_half, depth_min, depth_max, *hw[4:])
 
     def forward(self, img: Tensor, depth_half: Tensor, depth_min: Tensor, depth_max: Tensor) -> Tensor:
+        if torch.jit.is_scripting():
+            return self._forward_script(img, depth_half, depth_min, depth_max)
+        return self._forward_eager(img, depth_half, depth_min, depth_max)
+
+    @torch.jit.unused
+    def _forward_eager(self, img: Tensor, depth_half: Tensor, depth_min: Tensor, depth_max: Tensor) -> Tensor:
         from . import ops
 
         if (not self.training and _native_convs(img) and ops.REFINE_FUSED and ops.conv_precision() == 3 and img.dtype == torch.float32
@@ -445,6 +739,8 @@ class PatchmatchNet(nn.Module):
 
     GROUPS = (4, 8, 8)  # net.py:158
     FEATURES = (16, 32, 64)  # net.py:153
+    # not part of a scripted network (a scripted module's state dict would list the buffer); it uses _s_stage_scales instead
+    __jit_ignored_attributes__ = ["_stage_scales"]
 
     def __init__(
         self,
@@ -486,6 +782,25 @@ class PatchmatchNet(nn.Module):
         self.register_buffer("_stage_scales", torch.tensor([0.125, 0.25, 0.5]).view(3, 1, 1, 1, 1), persistent=False)
         # eval mode: push all views through FeatureNet as one batch (set False to go view by view)
         self.stack_views = True
+        # scripted forward, frozen by freeze_script (see "TorchScript" above)
+        self._s_fast = True
+        self._s_ref_channels_last = False  # extract_features' channels-last copy of the reference image
+        self._s_stage_scales = torch.tensor([0.125, 0.25, 0.5]).view(3, 1, 1, 1, 1)
+        self.register_load_state_dict_post_hook(_freeze_after_load)
+
+    def train(self, mode: bool = True):
+        super().train(mode)
+        if not mode and _freezing():
+            self.freeze_script()
+        return self
+
+    def freeze_script(self) -> None:
+        """Freeze the network-level eval-mode decisions of the scripted forward (FeatureNet, Refinement and the stages freeze
+        their own)."""
+        from . import ops
+
+        self._s_fast = LIBRARY_FAST_PATH
+        self._s_ref_channels_last = LIBRARY_FAST_PATH and not (ops.REFINE_FUSED and ops.NATIVE_CONVS and ops.conv_precision() == 3)
 
     def extract_features(self, images: List[Tensor]) -> List[Dict[int, Tensor]]:
         """One FeatureNet pass per view (reference net.py:203-208).  In eval mode the
@@ -510,6 +825,117 @@ class PatchmatchNet(nn.Module):
         return [{k: v[i * b:(i + 1) * b] for k, v in stacked.items()} for i in range(n)]
 
     def forward(
+        self,
+        images: List[Tensor],
+        intrinsics: Tensor,
+        extrinsics: Tensor,
+        depth_min: Tensor,
+        depth_max: Tensor,
+    ) -> Tuple[Tensor, Tensor, Dict[int, List[Tensor]]]:
+        if torch.jit.is_scripting():
+            return self._forward_script(images, intrinsics, extrinsics, depth_min, depth_max)
+        return self._forward_eager(images, intrinsics, extrinsics, depth_min, depth_max)
+
+    def _forward_script(
+        self,
+        images: List[Tensor],
+        intrinsics: Tensor,
+        extrinsics: Tensor,
+        depth_min: Tensor,
+        depth_max: Tensor,
+    ) -> Tuple[Tensor, Tensor, Dict[int, List[Tensor]]]:
+        """The eval-mode forward of `_forward_eager` in the TorchScript subset: the same launches under the decisions frozen at
+        eval() time.  Views of one size are always concatenated into one batch (TorchScript cannot see whether they already
+        share one buffer, which eager passes on without a copy).  Inference only, as scripting is in the reference."""
+        if self.training:
+            raise RuntimeError("a scripted patchmatchnet_b200 network is inference-only; call eval() before torch.jit.script")
+        assert len(images) == intrinsics.size(1), "Different number of images and intrinsic matrices"
+        assert len(images) == extrinsics.size(1), "Different number of images and extrinsic matrices"
+        images = list(images)
+        H0, W0 = images[0].size(-2), images[0].size(-1)
+        for i in range(len(images)):  # _round_dims_to_8
+            h, w = images[i].size(-2), images[i].size(-1)
+            nh, nw = int(round(h / 8)) * 8, int(round(w / 8)) * 8
+            if nh != h or nw != w:
+                intrinsics[:, i, 0] *= nw / w
+                intrinsics[:, i, 1] *= nh / h
+                images[i] = F.interpolate(images[i], size=[nh, nw], mode="bilinear", align_corners=False)
+        ref_image = images[0]
+        Hr, Wr = ref_image.size(-2), ref_image.size(-1)
+
+        same = True
+        for im in images:
+            if im.size() != images[0].size():
+                same = False
+        feats: List[Dict[int, Tensor]] = []
+        if self.stack_views and same:  # extract_features
+            b = images[0].size(0)
+            x = torch.cat(images, dim=0)
+            if self._s_ref_channels_last:
+                ref_image = images[0].contiguous(memory_format=torch.channels_last)
+            stacked = self.feature(x)
+            for i in range(len(images)):
+                feats.append({3: stacked[3][i * b:(i + 1) * b], 2: stacked[2][i * b:(i + 1) * b], 1: stacked[1][i * b:(i + 1) * b]})
+        else:
+            for im in images:
+                feats.append(self.feature(im))
+        depth_min = depth_min.float()
+        depth_max = depth_max.float()
+
+        dev = intrinsics.device
+        depth = torch.empty(0, device=dev)
+        score = torch.empty(0, device=dev)
+        view_weights = torch.empty(0, device=dev)
+        per_stage: Dict[int, List[Tensor]] = {}
+        all_proj: Optional[Tensor] = None
+        if self._s_fast:
+            K3 = intrinsics.unsqueeze(0).repeat(3, 1, 1, 1, 1)
+            K3[:, :, :, :2] *= torch.ops.pmb200.device_copy(self._s_stage_scales, K3)
+            all_proj = extrinsics.unsqueeze(0).repeat(3, 1, 1, 1, 1)
+            all_proj[:, :, :, :3, :4] = torch.matmul(K3, extrinsics[:, :, :3, :4])
+        scale = 0.125
+        for stage in [3, 2, 1]:
+            if all_proj is not None:
+                proj = all_proj[3 - stage]
+            else:
+                K = intrinsics.clone()
+                K[:, :, :2] *= scale
+                proj = extrinsics.clone()
+                proj[:, :, :3, :4] = torch.matmul(K, extrinsics[:, :, :3, :4])
+            projs = torch.unbind(proj, 1)
+            scale *= 2.0
+            src = [f[stage] for f in feats[1:]]
+            if stage == 3:
+                depths, score, view_weights = self.patchmatch_3(feats[0][3], src, projs[0], projs[1:], depth_min, depth_max, depth,
+                                                                view_weights)
+            elif stage == 2:
+                depths, score, view_weights = self.patchmatch_2(feats[0][2], src, projs[0], projs[1:], depth_min, depth_max, depth,
+                                                                view_weights)
+            else:
+                depths, score, view_weights = self.patchmatch_1(feats[0][1], src, projs[0], projs[1:], depth_min, depth_max, depth,
+                                                                view_weights)
+            per_stage[stage] = depths
+            depth = depths[-1].detach()
+            if stage > 1:
+                depth = F.interpolate(depth, scale_factor=2.0, mode="nearest")
+                view_weights = F.interpolate(view_weights, scale_factor=2.0, mode="nearest")
+
+        depth = self.upsample_net(ref_image, depth, depth_min, depth_max)
+        if Hr != H0 or Wr != W0:
+            depth = F.interpolate(depth, size=[H0, W0], mode="bilinear", align_corners=False)
+        per_stage[0] = [depth]
+        D = self.patchmatch_num_sample[0]
+        if self._s_fast and score.size(1) == D:
+            return depth, torch.ops.pmb200.photometric_confidence(score, H0, W0), per_stage
+        mass4 = 4 * F.avg_pool3d(F.pad(score.unsqueeze(1), pad=[0, 0, 0, 0, 1, 2]), (4, 1, 1), stride=1, padding=0).squeeze(1)
+        idx = torch.sum(score * torch.arange(D, device=score.device, dtype=torch.float).view(1, D, 1, 1), dim=1)
+        idx = idx.unsqueeze(1).long().clamp(0, D - 1)
+        conf = torch.gather(mass4, 1, idx)
+        conf = F.interpolate(conf, size=[H0, W0], mode="nearest").squeeze(1)
+        return depth, conf, per_stage
+
+    @torch.jit.unused
+    def _forward_eager(
         self,
         images: List[Tensor],
         intrinsics: Tensor,

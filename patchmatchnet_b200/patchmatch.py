@@ -215,6 +215,8 @@ class PatchMatch(nn.Module):
         # Tests inject a shared U[0,1) draw here when comparing against an oracle on another device;
         # by default the draw is torch.rand on the compute device, exactly as reference patchmatch.py:61-63.
         self.rand_source = None  # Optional[Callable]
+        # its counterpart in a scripted module (TorchScript cannot hold a callable): a fixed U[0,1) draw [B,48,H,W], empty = torch.rand
+        self.rand_draw = torch.empty(0)
         # eval mode: apply the 1x1x1 heads in the kernels' epilogues (BatchNorm folded); set False to
         # run them as cuDNN ops on materialised similarity tensors (the training path always does)
         self.fuse_heads = True
@@ -247,6 +249,10 @@ class PatchMatch(nn.Module):
         self._conv_precision = 3
         self._native_propa = False  # ops.conv_prefers_native(...) for the two offset convs, frozen likewise
         self._native_eval = False
+        # which native form runs each offset conv, as ops.conv_tc5_mode picks it for the eager path: 0 = the mma.sync kernel
+        # (conv2d_nhwc, filter in fragment order), 1 = the wgmma tap form, 2 = the wgmma halo-tile form (conv2d_tc5)
+        self._off_propa_form = 0
+        self._off_eval_form = 0
         self.register_load_state_dict_post_hook(_refresh_after_load)
 
     # ------------------------------------------------------------------
@@ -262,11 +268,18 @@ class PatchMatch(nn.Module):
         fits = lambda conv: max(conv.in_channels, conv.out_channels) <= 64
         self._native_propa = fits(self.propa_conv) and ops.conv_prefers_native(self.propa_conv.in_channels, self.propa_conv.out_channels, 3)
         self._native_eval = fits(self.eval_conv) and ops.conv_prefers_native(self.eval_conv.in_channels, self.eval_conv.out_channels, 3)
+        self._off_propa_form, self._off_propa_frag = self._freeze_offset_conv(self.propa_conv, self._native_propa)
+        self._off_eval_form, self._off_eval_frag = self._freeze_offset_conv(self.eval_conv, self._native_eval)
+
+    def _freeze_offset_conv(self, conv: nn.Conv2d, native: bool) -> Tuple[int, Tensor]:
+        """(form, host filter image) of one offset conv for the scripted forward: the form `_offset_conv` takes in eager mode."""
+        if not native:
+            return 0, torch.zeros(1)
+        tc5 = ops.conv_tc5_mode(conv.in_channels, conv.out_channels, conv.kernel_size[0], 1)
         with torch.no_grad():
-            if self._native_propa:
-                self._off_propa_frag = ops.pack_conv_filter(self.propa_conv.weight, self._conv_precision).cpu()
-            if self._native_eval:
-                self._off_eval_frag = ops.pack_conv_filter(self.eval_conv.weight, self._conv_precision).cpu()
+            if tc5:
+                return (2 if tc5 == "halo" else 1), ops.pack_conv_filter_tc5_for(conv.weight, tc5).cpu()
+            return 0, ops.pack_conv_filter(conv.weight, self._conv_precision).cpu()
 
     def train(self, mode: bool = True):
         super().train(mode)
@@ -335,29 +348,34 @@ class PatchMatch(nn.Module):
         propa_off: Optional[Tensor] = None
         if Kp > 0 and not (self.stage == 1 and iters == 1):
             if self._native_propa:
-                propa_off = torch.ops.pmb200.conv2d_nhwc(
-                    ref_feature, self._off_propa_frag, self.propa_conv.bias, 2 * Kp, 3, 1, self.dilation, self.dilation, False,
-                    self._conv_precision)
+                propa_off = self._script_offset_conv(ref_feature, self._off_propa_form, self._off_propa_frag, self.propa_conv.bias, 2 * Kp)
             else:
                 propa_off = self.propa_conv(ref_feature)
         if self._native_eval:
-            eval_off = torch.ops.pmb200.conv2d_nhwc(
-                ref_feature, self._off_eval_frag, self.eval_conv.bias, 2 * Ke, 3, 1, self.dilation, self.dilation, False,
-                self._conv_precision)
+            eval_off = self._script_offset_conv(ref_feature, self._off_eval_form, self._off_eval_frag, self.eval_conv.bias, 2 * Ke)
         else:
             eval_off = self.eval_conv(ref_feature)
 
+        # the three layouts of _forward_eager: one pack; reference and uniform sources of another size apart; a ragged pack of
+        # sources that differ from each other (CPU extents beside the flat data)
         same_size = True
+        uniform = True
         for f in src_features:
-            if f.size(2) != H or f.size(3) != W:
+            if f.size(0) != B or f.size(1) != ref_feature.size(1) or f.size(2) != H or f.size(3) != W:
                 same_size = False
+            if f.size() != src_features[0].size():
+                uniform = False
+        extents: Optional[Tensor] = None
         if same_size:
             pack = torch.ops.pmb200.pack_nhwc([ref_feature] + src_features)
             ref_nhwc = pack[0]
             src_nhwc = pack[1:]
-        else:
+        elif uniform:
             ref_nhwc = torch.ops.pmb200.pack_nhwc([ref_feature])[0]
             src_nhwc = torch.ops.pmb200.pack_nhwc(src_features)
+        else:
+            ref_nhwc = torch.ops.pmb200.pack_nhwc([ref_feature])[0]
+            src_nhwc, extents = torch.ops.pmb200.pack_nhwc_views(src_features)
         rt = torch.ops.pmb200.relative_projection(ref_proj, src_projs)
         feature_weight = torch.ops.pmb200.offset_corr_weight(ref_nhwc, eval_off, self._head_fw, self.G, Ke, self.dilation)
 
@@ -371,7 +389,10 @@ class PatchMatch(nn.Module):
             if Kp > 0 and not last_of_stage1:
                 kp_now = Kp
             if sample.numel() == 0:
-                seed = torch.rand([B, 48, H, W], device=ref_feature.device)
+                if self.rand_draw.numel() != 0:
+                    seed = self.rand_draw.to(ref_feature.device)
+                else:
+                    seed = torch.rand([B, 48, H, W], device=ref_feature.device)
                 mode, ns = 0, 48
             elif self.patchmatch_num_sample == 1:
                 seed, mode, ns = sample, 2, 1
@@ -384,16 +405,27 @@ class PatchMatch(nn.Module):
                 seed, off_now, dmin, dmax, mode, ns, kp_now, self.dilation, self.patchmatch_interval_scale
             )
             if vw.numel() == 0:
-                vw, sims = torch.ops.pmb200.warp_corr_view_weights(ref_nhwc, src_nhwc, rt, hyp, self._head_pw, self.G)
+                if extents is None:
+                    vw, sims = torch.ops.pmb200.warp_corr_view_weights(ref_nhwc, src_nhwc, rt, hyp, self._head_pw, self.G)
+                else:
+                    vw, sims = torch.ops.pmb200.warp_corr_view_weights_views(ref_nhwc, src_nhwc, extents, rt, hyp, self._head_pw, self.G)
                 torch.ops.pmb200.aggregate_views_score_(sims, vw, self._head_sim, xs)
-            else:
+            elif extents is None:
                 torch.ops.pmb200.warp_corr_score_(ref_nhwc, src_nhwc, rt, hyp, vw, self._head_sim, self.G, xs)
+            else:
+                torch.ops.pmb200.warp_corr_score_views_(ref_nhwc, src_nhwc, extents, rt, hyp, vw, self._head_sim, self.G, xs)
             new_depth, prob = torch.ops.pmb200.adaptive_eval(
                 xs, hyp, eval_off, feature_weight, dmin, dmax, self.dilation, self.patchmatch_interval_scale, last_of_stage1
             )
             sample = new_depth.unsqueeze(1)
             outs.append(sample)
         return outs, prob, vw.detach()
+
+    def _script_offset_conv(self, x: Tensor, form: int, frag: Tensor, bias: Optional[Tensor], cout: int) -> Tensor:
+        """One offset conv in the form `refresh_script_heads` froze (what `_offset_conv` runs in eager mode)."""
+        if form == 0:
+            return torch.ops.pmb200.conv2d_nhwc(x, frag, bias, cout, 3, 1, self.dilation, self.dilation, False, self._conv_precision)
+        return torch.ops.pmb200.conv2d_tc5(x, frag, bias, cout, 3, 1, self.dilation, self.dilation, False, form == 2)
 
     @torch.jit.unused
     def _forward_eager(

@@ -6,7 +6,7 @@
 
 Input per scan (datasets/mvs.py): pair.txt, images/[light/]%08d.jpg (--image-extension), cams/%08d_cam.txt, depth_gt/%08d.pfm.  Output in the
 output folder: params_%06d.ckpt ({"epoch", "model", "optimizer"}; model keys carry the reference's DataParallel "module."
-prefix, in its named_parameters order), module_%06d.pt (a TorchScript archive of the eval-mode network's state dict) and
+prefix, in its named_parameters order), module_%06d.pt (the eval-mode network scripted with TorchScript) and
 train_log.jsonl (one line per scalar: {"tag", "step", "value"}, the reference's TensorBoard tags).
 
 One step: the network forward, autograd.DepthLoss (the K-L loss kernels: no boolean indexing, no host round trip), the
@@ -360,27 +360,14 @@ def checkpoint_state(net: torch.nn.Module, optimizer: torch.optim.Optimizer, epo
     return {"epoch": epoch, "model": model, "optimizer": optimizer.state_dict()}
 
 
-class _StateHolder(torch.nn.Module):
-    def forward(self, x: Tensor) -> Tensor:
-        return x
-
-
 def export_module(net: torch.nn.Module, path: str) -> None:
-    """module_%06d.pt: a TorchScript archive whose state dict is the eval-mode network's, under the reference's keys (no
-    prefix, train.py:51-54 scripts the child module).  The native network calls its kernels through ctypes, which TorchScript
-    cannot compile, so the archive carries the weights only: `reconstruct --input-type module` loads it."""
+    """module_%06d.pt (train.py:50-55): `torch.jit.script(net.eval())`, a runnable TorchScript network over the
+    `torch.ops.pmb200.*` operators whose state dict is the eval-mode network's under the reference's keys (no prefix: the
+    reference scripts the child module).  `torch.jit.load` runs it after `import patchmatchnet_b200` (C++: after loading
+    libpmb200_torch.so); `reconstruct --input-type module` loads its state dict."""
     was_training = net.training
-    net.eval()
-    root = _StateHolder()
-    for key, value in net.state_dict().items():
-        *path_, leaf = key.split(".")
-        mod = root
-        for name in path_:
-            if name not in mod._modules:
-                mod.add_module(name, _StateHolder())
-            mod = mod._modules[name]
-        mod.register_buffer(leaf, value.detach().cpu().clone())
-    torch.jit.script(root).save(path)
+    net.eval()  # freezes the eval-mode decisions and folded weights the scripted forward runs on
+    torch.jit.script(net).save(path)
     net.train(was_training)
 
 
