@@ -225,6 +225,28 @@ int pmb200_geometric_filter_views(const float *ref_depth, const float *confidenc
  * All pointers are device memory.  Three launches on `stream` (count, scan, write); no host synchronisation. */
 int pmb200_fuse_points(const unsigned char *final_mask, const double *depth_avg, const float *ref_img_hwc, const double *cam25,
                        int H, int W, unsigned char *ply_body_out, int *count_out, int *block_scratch, void *stream);
+/* pmb200_fuse_points with oriented records: the same launches and the same surviving pixels in the same order, each written
+ * as a 27-byte vertex in the property order of COLMAP's fused.ply: float32 x, y, z, nx, ny, nz, uint8 red, green, blue.
+ *   normals_hwc [H*W*3] float32 (device): the reference view's camera-frame normal map (pmb200_depth_normals).  The world
+ *               normal is the rotation block of inverse(ref_extrinsics) (cam25[9..]) times it; a zero normal stays zero.
+ *   ply_body_out  capacity H*W*27 bytes. */
+int pmb200_fuse_points_oriented(const unsigned char *final_mask, const double *depth_avg, const float *ref_img_hwc,
+                                const float *normals_hwc, const double *cam25, int H, int W, unsigned char *ply_body_out,
+                                int *count_out, int *block_scratch, void *stream);
+
+/* Per-pixel surface normals of one depth map (beyond the reference, which has none), one launch, no host synchronisation,
+ * bit-identical from run to run.  Pixel p = (x, y) back-projects to P(p) = D(p) K^-1 (x, y, 1) (float64).  Its inliers are
+ * the pixels q of the (2 radius + 1)^2 window around p, clipped at the image border, with a finite depth > 0 and
+ * |D(q) - D(p)| <= depth_thres * D(p) (p included).  The normal is the unit eigenvector of the smallest eigenvalue of the
+ * inliers' covariance about their centroid (float64, closed-form 3x3 solve), facing the camera (n . P(p) < 0), in the camera
+ * frame.  It is (0, 0, 0) when D(p) is not finite and > 0, when there are fewer than min_inliers inliers, or when the middle
+ * eigenvalue is <= 1e-6 times the largest (collinear or coincident points).
+ *   depth [H*W] float32 (device); kinv_host: HOST, 9 doubles, K^-1 row-major at the map's size (the float32 inverse, widened)
+ *   normals_out [H*W*3] float32 (device), the layout of COLMAP's normal maps
+ * PMB200_EINVAL, nothing launched, for a null pointer, a bad size, radius outside 1..7, depth_thres < 0 or NaN, or
+ * min_inliers < 1. */
+int pmb200_depth_normals(const float *depth, const double *kinv_host, int H, int W, int radius, double depth_thres,
+                         int min_inliers, float *normals_out, void *stream);
 
 /* ------------------------------------------------------------------------------------
  * DTU point-cloud evaluation (reference evaluations/dtu/*.m; INTEGRATION.md "DTU evaluation"), float64 throughout.

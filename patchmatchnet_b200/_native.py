@@ -131,6 +131,8 @@ _SIGNATURES = {
     "pmb200_refine_full": (c_int, [c_void_p] * 13 + [c_int] * 3 + [c_void_p]),
     "pmb200_geometric_filter": (c_int, [c_void_p] * 4 + [c_int] * 5 + [c_double, c_float, c_float, c_int] + [c_void_p] * 5),
     "pmb200_fuse_points": (c_int, [c_void_p] * 4 + [c_int] * 2 + [c_void_p] * 4),
+    "pmb200_fuse_points_oriented": (c_int, [c_void_p] * 5 + [c_int] * 2 + [c_void_p] * 4),
+    "pmb200_depth_normals": (c_int, [c_void_p, POINTER(c_double), c_int, c_int, c_int, c_double, c_int, c_void_p, c_void_p]),
     "pmb200_thin_points_workspace_bytes": (c_int64, [c_int64]),
     "pmb200_thin_points": (c_int, [c_void_p, c_void_p, c_int64, c_double, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
     "pmb200_nearest_distance_workspace_bytes": (c_int64, [c_int64]),

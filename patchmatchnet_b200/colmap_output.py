@@ -1,13 +1,21 @@
-"""Scene folder + reconstruct results -> COLMAP dense workspace: the counterpart of the reference's colmap_output.py (host only).
+"""Scene folder + reconstruct results -> COLMAP dense workspace: the counterpart of the reference's colmap_output.py.
 
-    python -m patchmatchnet_b200.colmap_output --input-folder scene --results-folder outputs --output-folder workspace
-    colmap stereo_fusion --workspace_path workspace --input_type geometric --output_path fused_colmap.ply
+    python -m patchmatchnet_b200.reconstruct --input-folder scene --output-folder outputs --checkpoint-path model.pt
+    python -m patchmatchnet_b200.colmap_output --input-folder scene --results-folder outputs --output-folder workspace --normals
+    colmap stereo_fusion --workspace_path workspace --input_type geometric --output_path workspace/fused.ply
+    colmap poisson_mesher --input_path workspace/fused.ply --output_path workspace/meshed-poisson.ply
 
 Writes, under the output folder: images/ (a copy of the scene's images), stereo/depth_maps/<image>.geometric.bin and
 stereo/confidence_maps/<image>.geometric.bin (.bin results are copied, .pfm results converted through data_io.read_map /
 save_map), stereo/patch-match.cfg and stereo/fusion.cfg from pair.txt, and sparse/{cameras,images,points3D}.txt with one
 PINHOLE camera per view and the quaternion of each rotation from the reference's eigen-decomposition.  The empty
-consistency_graphs/ and normal_maps/ folders COLMAP expects are created too.
+consistency_graphs/ folder COLMAP expects is created too, and normal_maps/, which stays empty without --normals.
+
+COLMAP's stereo_fusion skips every image whose stereo/normal_maps/<image>.geometric.bin is missing, and its
+max_normal_error test reads those maps.  With --normals (off by default; it needs a CUDA device and changes no other
+file) each image's normal map is estimated on the GPU from its depth map (ops.estimate_normals: camera-frame unit normals,
+(0, 0, 0) where there is no estimate) with the cam file's intrinsics scaled to the depth map's size, and written there as
+a 3-channel COLMAP .bin at the depth map's size.  Without the flag the command runs on the host only, as before.
 
 Difference from the reference: cameras and images are listed in ascending view ID (the reference lists them in os.listdir
 order, which depends on the file system), and the map extension is taken from the first depth map in sorted order.
@@ -64,6 +72,25 @@ def copy_maps(input_path: str, results_path: str, output_path: str) -> None:
                 shutil.copy(src, dst)
             else:
                 data_io.save_map(dst, data_io.read_map(src))
+
+
+def write_normal_maps(input_path: str, results_path: str, output_path: str, device: str = "cuda:0") -> None:
+    """stereo/normal_maps/<image file>.geometric.bin per image of the scene: ops.estimate_normals on its depth map, with the
+    intrinsics of cams/<name>_cam.txt scaled from the image's size to the depth map's (reconstruct --image-max-dim writes
+    smaller maps)."""
+    from PIL import Image as PilImage
+
+    from . import ops
+
+    ext = os.path.splitext(sorted(os.listdir(os.path.join(results_path, "depth_est")))[0])[1]
+    for image_file in sorted(os.listdir(os.path.join(input_path, "images"))):
+        name = os.path.splitext(image_file)[0]
+        depth = data_io.read_map_to_device(os.path.join(results_path, "depth_est", name + ext), device)[..., 0]
+        with PilImage.open(os.path.join(input_path, "images", image_file), "r") as img:
+            width, height = img.width, img.height
+        k, _, _ = data_io.read_cam_file(os.path.join(input_path, "cams", name + "_cam.txt"))
+        normals = ops.estimate_normals(depth, data_io.scale_intrinsics(k, tuple(depth.shape), height, width))
+        data_io.save_map_from_device(os.path.join(output_path, "stereo", "normal_maps", image_file + ".geometric.bin"), normals)
 
 
 def read_reconstruction(path: str) -> Tuple[List[Camera], List[Image], List[Tuple[int, List[int]]]]:
@@ -123,6 +150,9 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--input-folder", type=str, help="Input PatchMatchNet reconstruction dir")
     ap.add_argument("--results-folder", type=str, default="", help="Input PatchMatchNet results dir")
     ap.add_argument("--output-folder", type=str, default="", help="Output ColMap MVS workspace")
+    ap.add_argument("--normals", action="store_true",
+                    help="estimate a normal map per image on the GPU and write it to stereo/normal_maps (COLMAP's "
+                         "stereo_fusion needs them)")
     return ap
 
 
@@ -145,10 +175,17 @@ def check_args(args: argparse.Namespace) -> None:
 
 
 def export(args: argparse.Namespace) -> None:
-    """The command's library call."""
+    """The command's library call.  With --normals it raises before it writes anything when there is no CUDA device."""
     check_args(args)
+    if args.normals:
+        import torch
+
+        if not torch.cuda.is_available():
+            raise RuntimeError("colmap_output --normals needs a CUDA device (H100); there is no CPU fallback")
     create_output_dirs(args.output_folder)
     copy_maps(args.input_folder, args.results_folder, args.output_folder)
+    if args.normals:
+        write_normal_maps(args.input_folder, args.results_folder, args.output_folder)
     cameras, images, pairs = read_reconstruction(args.input_folder)
     write_patch_match_config(os.path.join(args.output_folder, "stereo", "patch-match.cfg"), images, pairs)
     write_fusion_config(os.path.join(args.output_folder, "stereo", "fusion.cfg"), images, pairs)

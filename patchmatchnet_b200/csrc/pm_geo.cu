@@ -122,9 +122,12 @@ __global__ void __launch_bounds__(1024) fuse_scan_kernel(int *counts, int nblock
     if (threadIdx.x == 0) *total = s_carry;
 }
 
+// kOriented: the 27-byte records of pmb200_fuse_points_oriented, with the pixel's normal from `normals` ([n,3], read only
+// then).  The normal map is the last parameter, so the plain instantiation keeps its parameter block and its code.
+template <bool kOriented>
 __global__ void __launch_bounds__(kFuseBlock) fuse_write_kernel(const unsigned char *mask, const double *depth_avg, const float *rgb,
                                                                 const double *cam, int W, int n, const int *offsets,
-                                                                unsigned char *body) {
+                                                                unsigned char *body, const float *normals) {
     __shared__ int s_warp[kFuseBlock / 32];
     __shared__ double s_cam[pmgeo::kFuseCamDoubles];
     if (threadIdx.x < pmgeo::kFuseCamDoubles) s_cam[threadIdx.x] = cam[threadIdx.x];
@@ -138,7 +141,59 @@ __global__ void __launch_bounds__(kFuseBlock) fuse_write_kernel(const unsigned c
     for (int w = 0; w < warp; ++w) before += s_warp[w];
     if (!keep) return;
     const int rank = offsets[blockIdx.x] + before + __popc(m & ((1u << lane) - 1u));
-    pmgeo::fuse_point(s_cam, i % W, i / W, depth_avg[i], rgb + (size_t)i * 3, body + (size_t)rank * pmgeo::kPlyVertexBytes);
+    if constexpr (kOriented)
+        pmgeo::fuse_point_oriented(s_cam, i % W, i / W, depth_avg[i], rgb + (size_t)i * 3, normals + (size_t)i * 3,
+                                   body + (size_t)rank * pmgeo::kPlyOrientedVertexBytes);
+    else
+        pmgeo::fuse_point(s_cam, i % W, i / W, depth_avg[i], rgb + (size_t)i * 3, body + (size_t)rank * pmgeo::kPlyVertexBytes);
+}
+
+template <bool kOriented>
+int fuse_points(const unsigned char *final_mask, const double *depth_avg, const float *ref_img_hwc, const float *normals_hwc,
+                const double *cam25, int H, int W, unsigned char *ply_body_out, int *count_out, int *block_scratch, void *stream,
+                const char *what) {
+    const int n = H * W, nblocks = (n + kFuseBlock - 1) / kFuseBlock;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    fuse_count_kernel<<<nblocks, kFuseBlock, 0, st>>>(final_mask, n, block_scratch);
+    fuse_scan_kernel<<<1, 1024, 0, st>>>(block_scratch, nblocks, count_out);
+    fuse_write_kernel<kOriented><<<nblocks, kFuseBlock, 0, st>>>(final_mask, depth_avg, ref_img_hwc, cam25, W, n, block_scratch,
+                                                                 ply_body_out, normals_hwc);
+    return pmb200_internal_launch_status(what);
+}
+
+// ---- surface normals (pmb200_depth_normals): one thread per pixel over a 32 x 8 tile of the depth map staged in shared
+// memory with a halo of r, the per-pixel arithmetic of pmgeo::normal_pixel.  No atomics: run-to-run bit-identical. ----------
+constexpr int kNormTileX = 32, kNormTileY = 8;
+constexpr int kNormPitchMax = kNormTileX + 2 * pmgeo::kNormalMaxRadius;
+
+struct NormalParams {
+    const float *depth;
+    float *normals;
+    int H, W, radius, min_inliers;
+    double depth_thres;
+    double kinv[9];
+};
+
+__global__ void __launch_bounds__(kNormTileX * kNormTileY, 3) depth_normals_kernel(const NormalParams p) {
+    __shared__ float s_tile[kNormPitchMax * (kNormTileY + 2 * pmgeo::kNormalMaxRadius)];
+    const int r = p.radius, pitch = kNormTileX + 2 * r, rows = kNormTileY + 2 * r;
+    const int tx0 = blockIdx.x * kNormTileX - r, ty0 = blockIdx.y * kNormTileY - r;
+    for (int i = threadIdx.x; i < pitch * rows; i += kNormTileX * kNormTileY) {
+        const int gy = ty0 + i / pitch, gx = tx0 + i % pitch;
+        s_tile[i] = (gx >= 0 && gx < p.W && gy >= 0 && gy < p.H) ? __ldg(p.depth + (size_t)gy * p.W + gx) : 0.0f;
+    }
+    __syncthreads();
+    const int lx = threadIdx.x % kNormTileX, ly = threadIdx.x / kNormTileX;
+    const int x = blockIdx.x * kNormTileX + lx, y = blockIdx.y * kNormTileY + ly;
+    if (x >= p.W || y >= p.H) return;
+    const int dx0 = -min(r, x), dx1 = min(r, p.W - 1 - x), dy0 = -min(r, y), dy1 = min(r, p.H - 1 - y);
+    float nrm[3];
+    pmgeo::normal_pixel(s_tile + (ly + r) * pitch + lx + r, pitch, x, y, dx0, dx1, dy0, dy1, p.kinv, p.depth_thres, p.min_inliers,
+                        nrm);
+    float *o = p.normals + ((size_t)y * p.W + x) * 3;
+    o[0] = nrm[0];
+    o[1] = nrm[1];
+    o[2] = nrm[2];
 }
 
 }  // namespace
@@ -149,12 +204,37 @@ extern "C" int pmb200_fuse_points(const unsigned char *final_mask, const double 
     if (!final_mask || !depth_avg || !ref_img_hwc || !cam25 || !ply_body_out || !count_out || !block_scratch)
         return pmb200_internal_fail(PMB200_EINVAL, "fuse_points: null pointer");
     if (H < 1 || W < 1 || (long long)H * W >= (1ll << 31)) return pmb200_internal_fail(PMB200_EINVAL, "fuse_points: bad size");
-    const int n = H * W, nblocks = (n + kFuseBlock - 1) / kFuseBlock;
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    fuse_count_kernel<<<nblocks, kFuseBlock, 0, st>>>(final_mask, n, block_scratch);
-    fuse_scan_kernel<<<1, 1024, 0, st>>>(block_scratch, nblocks, count_out);
-    fuse_write_kernel<<<nblocks, kFuseBlock, 0, st>>>(final_mask, depth_avg, ref_img_hwc, cam25, W, n, block_scratch, ply_body_out);
-    return pmb200_internal_launch_status("fuse_points");
+    return fuse_points<false>(final_mask, depth_avg, ref_img_hwc, nullptr, cam25, H, W, ply_body_out, count_out, block_scratch,
+                              stream, "fuse_points");
+}
+
+extern "C" int pmb200_fuse_points_oriented(const unsigned char *final_mask, const double *depth_avg, const float *ref_img_hwc,
+                                           const float *normals_hwc, const double *cam25, int H, int W, unsigned char *ply_body_out,
+                                           int *count_out, int *block_scratch, void *stream) {
+    if (!final_mask || !depth_avg || !ref_img_hwc || !normals_hwc || !cam25 || !ply_body_out || !count_out || !block_scratch)
+        return pmb200_internal_fail(PMB200_EINVAL, "fuse_points_oriented: null pointer");
+    if (H < 1 || W < 1 || (long long)H * W >= (1ll << 31))
+        return pmb200_internal_fail(PMB200_EINVAL, "fuse_points_oriented: bad size");
+    return fuse_points<true>(final_mask, depth_avg, ref_img_hwc, normals_hwc, cam25, H, W, ply_body_out, count_out, block_scratch,
+                             stream, "fuse_points_oriented");
+}
+
+extern "C" int pmb200_depth_normals(const float *depth, const double *kinv_host, int H, int W, int radius, double depth_thres,
+                                    int min_inliers, float *normals_out, void *stream) {
+    if (!depth || !kinv_host || !normals_out) return pmb200_internal_fail(PMB200_EINVAL, "depth_normals: null pointer");
+    if (H < 1 || W < 1 || (long long)H * W >= (1ll << 31) || (H + kNormTileY - 1) / kNormTileY > 65535)
+        return pmb200_internal_fail(PMB200_EINVAL, "depth_normals: bad size");
+    if (radius < 1 || radius > pmgeo::kNormalMaxRadius)
+        return pmb200_internal_fail(PMB200_EINVAL, "depth_normals: radius must be in 1..7");
+    if (!(depth_thres >= 0.0) || min_inliers < 1)
+        return pmb200_internal_fail(PMB200_EINVAL, "depth_normals: depth_thres must be >= 0 and min_inliers >= 1");
+    NormalParams p;
+    p.depth = depth; p.normals = normals_out;
+    p.H = H; p.W = W; p.radius = radius; p.min_inliers = min_inliers; p.depth_thres = depth_thres;
+    for (int i = 0; i < 9; ++i) p.kinv[i] = kinv_host[i];
+    const dim3 grid((W + kNormTileX - 1) / kNormTileX, (H + kNormTileY - 1) / kNormTileY);
+    depth_normals_kernel<<<grid, kNormTileX * kNormTileY, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+    return pmb200_internal_launch_status("depth_normals");
 }
 
 extern "C" int pmb200_geometric_filter(const float *ref_depth, const float *confidence, const float *src_depths,

@@ -164,8 +164,9 @@ PMG_HD PixelResult filter_pixel(const double *cams, const float *src_flat, const
 // truncated to uint8.
 constexpr int kFuseCamDoubles = 25;
 constexpr int kPlyVertexBytes = 15;
+constexpr int kPlyOrientedVertexBytes = 27;  // float32 x, y, z, nx, ny, nz, uint8 r, g, b: the order of COLMAP's fused.ply
 
-PMG_HD void fuse_point(const double *cam, int x, int y, double depth, const float *rgb, unsigned char *rec) {
+PMG_HD void fuse_position(const double *cam, int x, int y, double depth, unsigned char *rec) {
     const double px = (double)x * depth, py = (double)y * depth, pz = depth;
     const double *K = cam, *E = cam + 9;
     const double rx = fma(K[2], pz, fma(K[1], py, K[0] * px));
@@ -177,7 +178,150 @@ PMG_HD void fuse_point(const double *cam, int x, int y, double depth, const floa
     out[2] = (float)fma(E[11], 1.0, fma(E[10], rz, fma(E[9], ry, E[8] * rx)));
     const unsigned char *b = reinterpret_cast<const unsigned char *>(out);
     for (int i = 0; i < 12; ++i) rec[i] = b[i];
-    for (int c = 0; c < 3; ++c) rec[12 + c] = (unsigned char)mul32(load32(rgb + c), 255.0f);
+}
+
+PMG_HD void fuse_colour(const float *rgb, unsigned char *rec) {
+    for (int c = 0; c < 3; ++c) rec[c] = (unsigned char)mul32(load32(rgb + c), 255.0f);
+}
+
+PMG_HD void fuse_point(const double *cam, int x, int y, double depth, const float *rgb, unsigned char *rec) {
+    fuse_position(cam, x, y, depth, rec);
+    fuse_colour(rgb, rec + 12);
+}
+
+// fuse_point with the pixel's camera-frame normal (a pmb200_depth_normals output) rotated into the world frame by the rotation
+// block of inverse(extrinsics) (cam + 9, rows of 4); a zero normal (no estimate) stays exactly zero.
+PMG_HD void fuse_point_oriented(const double *cam, int x, int y, double depth, const float *rgb, const float *normal,
+                                unsigned char *rec) {
+    fuse_position(cam, x, y, depth, rec);
+    const double nx = (double)load32(normal), ny = (double)load32(normal + 1), nz = (double)load32(normal + 2);
+    const double *E = cam + 9;
+    float out[3] = {0.0f, 0.0f, 0.0f};
+    if (nx != 0.0 || ny != 0.0 || nz != 0.0) {
+        out[0] = (float)fma(E[2], nz, fma(E[1], ny, E[0] * nx));
+        out[1] = (float)fma(E[6], nz, fma(E[5], ny, E[4] * nx));
+        out[2] = (float)fma(E[10], nz, fma(E[9], ny, E[8] * nx));
+    }
+    const unsigned char *b = reinterpret_cast<const unsigned char *>(out);
+    for (int i = 0; i < 12; ++i) rec[12 + i] = b[i];
+    fuse_colour(rgb, rec + 24);
+}
+
+// ---- surface normals from one depth map (pmb200_depth_normals; this project's own definition, the reference has none) ----
+// The normal of pixel p = (x, y) is the direction of least spread of the back-projected points P(q) = D(q) K^-1 (x_q, y_q, 1)
+// of its inliers: the valid pixels q (finite depth > 0) of the (2r+1)^2 window around p, clipped at the image border, whose
+// depth is within depth_thres * D(p) of D(p) (p included).  Everything runs in float64.  The points are shifted by P(p) before
+// the covariance about their centroid is formed (two passes: centroid, then covariance), so ~10^3 mm coordinates do not
+// cancel.  Zero normal: p invalid, fewer than min_inliers inliers, or lambda_mid <= 1e-6 lambda_max (collinear or coincident
+// points).  Otherwise the unit eigenvector of lambda_min, turned to face the camera (n . P(p) < 0), in the camera frame.
+constexpr int kNormalMaxRadius = 7;
+constexpr double kNormalDegenerate = 1e-6;
+
+#if defined(__CUDA_ARCH__)
+PMG_HD double cos_pi(double v) { return cospi(v); }  // no Payne-Hanek slow path: cos(pi * v) without a stack frame
+PMG_HD double rsqrt64(double v) { return rsqrt(v); }
+#else
+PMG_HD double cos_pi(double v) { return cos(3.14159265358979323846 * v); }
+PMG_HD double rsqrt64(double v) { return 1.0 / sqrt(v); }
+#endif
+
+PMG_HD bool valid_depth(float d) { return isfinite(d) && d > 0.0f; }
+
+// Eigenvalues l0 <= l1 <= l2 of the symmetric matrix [a0 a1 a2; a1 a3 a4; a2 a4 a5] (trigonometric closed form).
+PMG_HD void sym3_eigenvalues(const double *a, double &l0, double &l1, double &l2) {
+    const double off = a[1] * a[1] + a[2] * a[2] + a[4] * a[4];
+    const double q = (a[0] + a[3] + a[5]) * (1.0 / 3.0);
+    const double b0 = a[0] - q, b3 = a[3] - q, b5 = a[5] - q;
+    const double p2 = (b0 * b0 + b3 * b3 + b5 * b5 + 2.0 * off) * (1.0 / 6.0);
+    if (p2 == 0.0) {  // a multiple of the identity
+        l0 = l1 = l2 = q;
+        return;
+    }
+    const double ip = rsqrt64(p2), p = p2 * ip;
+    const double c0 = b0 * ip, c1 = a[1] * ip, c2 = a[2] * ip, c3 = b3 * ip, c4 = a[4] * ip, c5 = b5 * ip;
+    double hdet = 0.5 * (c0 * (c3 * c5 - c4 * c4) - c1 * (c1 * c5 - c4 * c2) + c2 * (c1 * c4 - c3 * c2));
+    hdet = hdet < -1.0 ? -1.0 : (hdet > 1.0 ? 1.0 : hdet);
+    const double t = acos(hdet) * (1.0 / (3.0 * 3.14159265358979323846));  // phi / pi, phi in [0, pi/3]
+    l2 = q + 2.0 * p * cos_pi(t);
+    l0 = q + 2.0 * p * cos_pi(t + 2.0 / 3.0);
+    l1 = 3.0 * q - l0 - l2;
+}
+
+// Unit eigenvector of the symmetric matrix `a` (as above) for its eigenvalue `lam`: the largest cross product of two rows of
+// a - lam I.  False when every cross product vanishes.
+PMG_HD void cross_keep_largest(double u0, double u1, double u2, double w0, double w1, double w2, double &best, double *v) {
+    const double c0 = u1 * w2 - u2 * w1, c1 = u2 * w0 - u0 * w2, c2 = u0 * w1 - u1 * w0;
+    const double n2 = c0 * c0 + c1 * c1 + c2 * c2;
+    if (n2 > best) {
+        best = n2;
+        v[0] = c0; v[1] = c1; v[2] = c2;
+    }
+}
+
+PMG_HD bool sym3_eigenvector(const double *a, double lam, double *v) {
+    const double m0 = a[0] - lam, m3 = a[3] - lam, m5 = a[5] - lam;
+    double best = 0.0;
+    cross_keep_largest(m0, a[1], a[2], a[1], m3, a[4], best, v);  // row 0 x row 1
+    cross_keep_largest(m0, a[1], a[2], a[2], a[4], m5, best, v);  // row 0 x row 2
+    cross_keep_largest(a[1], m3, a[4], a[2], a[4], m5, best, v);  // row 1 x row 2
+    if (!(best > 0.0)) return false;
+    const double s = rsqrt64(best);
+    v[0] *= s; v[1] *= s; v[2] *= s;
+    return true;
+}
+
+// The normal of pixel (x, y).  dp points at the pixel's depth in a row-major map (or a tile of it) of row pitch `pitch`; the
+// window is dx in [dx0, dx1], dy in [dy0, dy1], already clipped at the image border.  kinv: K^-1 row-major.  -> out[3].
+PMG_HD void normal_pixel(const float *dp, int pitch, int x, int y, int dx0, int dx1, int dy0, int dy1, const double *kinv,
+                         double depth_thres, int min_inliers, float *out) {
+    out[0] = out[1] = out[2] = 0.0f;
+    const float dpf = dp[0];
+    if (!valid_depth(dpf)) return;
+    const double d0 = (double)dpf, tol = depth_thres * d0;
+    const double px = d0 * (kinv[0] * x + kinv[1] * y + kinv[2]);
+    const double py = d0 * (kinv[3] * x + kinv[4] * y + kinv[5]);
+    const double pz = d0 * (kinv[6] * x + kinv[7] * y + kinv[8]);
+    int n = 0;
+    double sx = 0.0, sy = 0.0, sz = 0.0;
+    for (int dy = dy0; dy <= dy1; ++dy)
+        for (int dx = dx0; dx <= dx1; ++dx) {
+            const float df = dp[dy * pitch + dx];
+            if (!valid_depth(df) || !(fabs((double)df - d0) <= tol)) continue;
+            const double d = (double)df, u = (double)(x + dx), w = (double)(y + dy);
+            sx += d * (kinv[0] * u + kinv[1] * w + kinv[2]) - px;
+            sy += d * (kinv[3] * u + kinv[4] * w + kinv[5]) - py;
+            sz += d * (kinv[6] * u + kinv[7] * w + kinv[8]) - pz;
+            ++n;
+        }
+    if (n < min_inliers) return;
+    const double inv_n = 1.0 / (double)n, cx = sx * inv_n, cy = sy * inv_n, cz = sz * inv_n;
+    double a[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int dy = dy0; dy <= dy1; ++dy)
+        for (int dx = dx0; dx <= dx1; ++dx) {
+            const float df = dp[dy * pitch + dx];
+            if (!valid_depth(df) || !(fabs((double)df - d0) <= tol)) continue;
+            const double d = (double)df, u = (double)(x + dx), w = (double)(y + dy);
+            const double ex = d * (kinv[0] * u + kinv[1] * w + kinv[2]) - px - cx;
+            const double ey = d * (kinv[3] * u + kinv[4] * w + kinv[5]) - py - cy;
+            const double ez = d * (kinv[6] * u + kinv[7] * w + kinv[8]) - pz - cz;
+            a[0] += ex * ex; a[1] += ex * ey; a[2] += ex * ez;
+            a[3] += ey * ey; a[4] += ey * ez; a[5] += ez * ez;
+        }
+    double scale = 0.0;  // the solve runs on the matrix scaled to a largest entry in [1, 2)
+    for (int i = 0; i < 6; ++i) scale = fabs(a[i]) > scale ? fabs(a[i]) : scale;
+    if (!(scale > 0.0)) return;
+    const int e = ilogb(scale);  // a power-of-two scale: exact
+    for (int i = 0; i < 6; ++i) a[i] = ldexp(a[i], -e);
+    double l0, l1, l2, v[3];
+    sym3_eigenvalues(a, l0, l1, l2);
+    if (!(l1 > kNormalDegenerate * l2)) return;
+    if (!sym3_eigenvector(a, l0, v)) return;
+    if (v[0] * px + v[1] * py + v[2] * pz > 0.0) {
+        v[0] = -v[0]; v[1] = -v[1]; v[2] = -v[2];
+    }
+    out[0] = (float)v[0];
+    out[1] = (float)v[1];
+    out[2] = (float)v[2];
 }
 
 }  // namespace pmgeo

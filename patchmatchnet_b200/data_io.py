@@ -244,17 +244,21 @@ def save_map_from_device(path: str, tensor: torch.Tensor, scale: float = 1) -> N
 def save_ply(path: str, body) -> None:
     """Write the reference's fused.ply (eval.py:283-296: PlyData([PlyElement.describe(vertex_all, "vertex")]).write -- binary
     little endian, one `vertex` element with float x, y, z and uchar red, green, blue) from vertex records produced by
-    ops.fuse_points: uint8 [n,15] tensor(s) (a list concatenates the per-reference-view clouds, eval.py:283-284)."""
+    ops.fuse_points: uint8 [n,15] tensor(s) (a list concatenates the per-reference-view clouds, eval.py:283-284).
+    Oriented records, uint8 [n,27] (ops.fuse_points with normals), write float nx, ny, nz between z and red, the property
+    order of COLMAP's fused.ply; every part of one file has the same record size."""
     import torch
 
     parts = list(body) if isinstance(body, (list, tuple)) else [body]
     parts = [b.detach().cpu().contiguous() for b in parts]
+    width = int(parts[0].shape[1]) if parts and parts[0].dim() == 2 else 15
     for b in parts:
-        if b.dtype != torch.uint8 or b.dim() != 2 or b.shape[1] != 15:
-            raise ValueError("save_ply: vertex records must be uint8 [n,15] tensors (ops.fuse_points)")
+        if b.dtype != torch.uint8 or b.dim() != 2 or b.shape[1] not in (15, 27) or b.shape[1] != width:
+            raise ValueError("save_ply: vertex records must be uint8 [n,15] or [n,27] tensors of one size (ops.fuse_points)")
     n = sum(int(b.shape[0]) for b in parts)
+    normals = "property float nx\nproperty float ny\nproperty float nz\n" if width == 27 else ""
     header = ("ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\nproperty float z\n"
-              "property uchar red\nproperty uchar green\nproperty uchar blue\nend_header\n" % n)
+              "%sproperty uchar red\nproperty uchar green\nproperty uchar blue\nend_header\n" % (n, normals))
     with open(path, "wb") as f:
         f.write(header.encode("ascii"))
         for b in parts:

@@ -977,11 +977,15 @@ def compose_fusion_camera(ref_K, ref_E) -> Tensor:
     return torch.from_numpy(np.concatenate([np.linalg.inv(f32(ref_K)).ravel(), np.linalg.inv(f32(ref_E)).ravel()]).astype(np.float64))
 
 
-def fuse_points(final_mask: Tensor, depth_averaged: Tensor, ref_img: Tensor, cam25: Tensor) -> Tensor:
+def fuse_points(final_mask: Tensor, depth_averaged: Tensor, ref_img: Tensor, cam25: Tensor, normals: Optional[Tensor] = None) -> Tensor:
     """Point-cloud half of the fusion for one reference view (reference eval.py:273-296): -> uint8 [n,15] CUDA tensor, the
     binary little-endian PLY vertex records (float32 x, y, z, uint8 r, g, b) of the surviving pixels in row-major order.
     final_mask bool / uint8 [H,W], depth_averaged float64 [H,W] (as geometric_filter returns them), ref_img float32
-    [H,W,3] in [0,1].  One host synchronisation at the end (the vertex count sizes the result)."""
+    [H,W,3] in [0,1].  One host synchronisation at the end (the vertex count sizes the result).
+
+    With `normals`, the reference view's camera-frame normal map (float32 [H,W,3], estimate_normals), the records are the
+    27-byte oriented ones, uint8 [n,27] (pmb200_fuse_points_oriented): float32 x, y, z, nx, ny, nz, uint8 r, g, b, the
+    normal rotated into the world frame; the same pixels in the same order."""
     if not _on_device(final_mask) or not _on_device(depth_averaged) or not _on_device(ref_img):
         raise RuntimeError("fuse_points: the H100 path needs CUDA tensors; there is no CPU fallback")
     H, W = depth_averaged.shape
@@ -989,18 +993,57 @@ def fuse_points(final_mask: Tensor, depth_averaged: Tensor, ref_img: Tensor, cam
         raise RuntimeError("fuse_points: final_mask [H,W], depth_averaged float64 [H,W], ref_img float32 [H,W,3]")
     if cam25.shape != (25,) or cam25.dtype != torch.float64:
         raise RuntimeError("fuse_points: cam25 must be a [25] float64 tensor (compose_fusion_camera)")
+    if normals is not None:
+        normals = _require(normals, "fuse_points: normals", 3)
+        if tuple(normals.shape) != (H, W, 3):
+            raise RuntimeError(f"fuse_points: normals must be [H,W,3] = [{H},{W},3], got {tuple(normals.shape)}")
     mask = final_mask.to(torch.uint8).contiguous()
     depth = depth_averaged.contiguous()
     img = ref_img.contiguous()
     cam = cam25.to(depth.device).contiguous()
-    body = torch.empty((H * W, 15), dtype=torch.uint8, device=depth.device)
+    body = torch.empty((H * W, 15 if normals is None else 27), dtype=torch.uint8, device=depth.device)
     count = torch.zeros(1, dtype=torch.int32, device=depth.device)
     scratch = torch.empty(((H * W + 255) // 256,), dtype=torch.int32, device=depth.device)
     with _device_guard(depth):
-        rc = _native.lib().pmb200_fuse_points(mask.data_ptr(), depth.data_ptr(), img.data_ptr(), cam.data_ptr(), H, W, body.data_ptr(),
-                                              count.data_ptr(), scratch.data_ptr(), _stream(depth))
-    _native.check(rc, "fuse_points")
+        if normals is None:
+            rc = _native.lib().pmb200_fuse_points(mask.data_ptr(), depth.data_ptr(), img.data_ptr(), cam.data_ptr(), H, W, body.data_ptr(),
+                                                  count.data_ptr(), scratch.data_ptr(), _stream(depth))
+        else:
+            rc = _native.lib().pmb200_fuse_points_oriented(mask.data_ptr(), depth.data_ptr(), img.data_ptr(), normals.data_ptr(),
+                                                           cam.data_ptr(), H, W, body.data_ptr(), count.data_ptr(), scratch.data_ptr(),
+                                                           _stream(depth))
+    _native.check(rc, "fuse_points" if normals is None else "fuse_points_oriented")
     return body[: int(count.item())]
+
+
+def _kinv_host(K):
+    """K^-1 as pmb200_depth_normals takes it: the float32 inverse numpy computes (as compose_fusion_camera inverts), widened
+    to 9 float64 values in a host array."""
+    import ctypes
+
+    import numpy as np
+
+    k = np.asarray(K.detach().cpu().numpy() if isinstance(K, torch.Tensor) else K, dtype=np.float32)
+    if k.shape != (3, 3):
+        raise RuntimeError(f"estimate_normals: K must be [3,3], got {k.shape}")
+    return (ctypes.c_double * 9)(*np.linalg.inv(k).astype(np.float64).ravel().tolist())
+
+
+def estimate_normals(depth: Tensor, K, radius: int = 3, depth_thres: float = 0.01, min_inliers: int = 6) -> Tensor:
+    """Per-pixel unit normals of a depth map in the camera frame (pmb200_depth_normals; this project's own definition, see
+    include/patchmatch_b200.h): the least-spread direction of the back-projected points of the pixels within `radius` whose
+    depth is within depth_thres * D(p) of the pixel's, facing the camera; (0, 0, 0) where there is no estimate.
+    depth CUDA float32 [H,W]; K float32 [3,3] (array or tensor) at the map's size.  -> CUDA float32 [H,W,3], the layout of
+    COLMAP's normal maps.  radius 1..7 (PMB200_EINVAL otherwise, before any launch)."""
+    d = _require(depth, "estimate_normals: depth", 2)
+    H, W = d.shape
+    kinv = _kinv_host(K)
+    out = torch.empty((H, W, 3), dtype=torch.float32, device=d.device)
+    with _device_guard(d):
+        rc = _native.lib().pmb200_depth_normals(d.data_ptr(), kinv, H, W, int(radius), float(depth_thres), int(min_inliers),
+                                                out.data_ptr(), _stream(d))
+    _native.check(rc, "depth_normals")
+    return out
 
 
 def split_ply_body(body: Tensor):

@@ -29,6 +29,17 @@ ops.compose_fusion_camera -> ops.fuse_points (pmb200_fuse_points).  The vertex r
 data_io.save_ply writes the scan's fused.ply once.  With --output-type both the maps come from the map bank; with
 --output-type fusion each map file is read once per scan (data_io.read_map_to_device).
 
+With --normals (off by default; it changes no other output) each reference view's normal map is estimated from its raw
+depth map with that view's intrinsics (ops.estimate_normals, pmb200_depth_normals) and fused.ply is written oriented:
+float x, y, z, nx, ny, nz, uchar red, green, blue per point (pmb200_fuse_points_oriented), which Poisson surface
+reconstruction takes as is.  For COLMAP's own fusion and meshers, export the results instead:
+
+    python -m patchmatchnet_b200.reconstruct --input-folder scene --output-folder outputs --checkpoint-path model.pt --normals
+    PoissonRecon --in outputs/fused.ply --out mesh.ply            # or Open3D, or colmap poisson_mesher on this file
+    python -m patchmatchnet_b200.colmap_output --input-folder scene --results-folder outputs --output-folder ws --normals
+    colmap stereo_fusion --workspace_path ws --input_type geometric --output_path ws/fused.ply
+    colmap poisson_mesher --input_path ws/fused.ply --output_path ws/meshed-poisson.ply
+
 Device memory held besides the engines, for a scan of n_img images of H x W and n_ref reference views:
     image bank   n_img * 3 * H * W * 4 bytes
     map bank     n_ref * 2 * H * W * 4 bytes
@@ -87,6 +98,9 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--photo-thres", type=float, default=0.5, help="threshold for photometric consistency filtering")
     ap.add_argument("--seed", type=int, default=0, help="seed of the stage-3 random initialisation (per request slot: seed + slot)")
     ap.add_argument("--tf32", action="store_true", help="TF32 operands in the convolutions (default: fp32-accurate)")
+    ap.add_argument("--normals", action="store_true",
+                    help="write an oriented fused.ply (float nx, ny, nz per point, for Poisson meshers) with normals estimated "
+                         "from each reference view's depth map")
     return ap
 
 
@@ -320,7 +334,7 @@ class _DiskMaps:
 def fuse_scan(args: argparse.Namespace, scan: str, bank: SceneBank, pairs: Sequence[Tuple[int, List[int]]], maps,
               log: Callable[..., None] = print) -> int:
     """filter_depth (eval.py:193-297) for one scan; `maps[view]` -> (depth [H,W], confidence [H,W]) on the device.
-    Writes the mask PNGs and fused.ply; -> the number of points."""
+    Writes the mask PNGs and fused.ply (oriented with --normals); -> the number of points."""
     out_dir = os.path.join(args.output_folder, scan)
     os.makedirs(os.path.join(out_dir, "mask"), exist_ok=True)
     bodies = []
@@ -339,9 +353,11 @@ def fuse_scan(args: argparse.Namespace, scan: str, bank: SceneBank, pairs: Seque
         data_io.save_image(os.path.join(out_dir, "mask", "{:0>8}_final.png".format(ref)), final_h)
         log("processing {}, ref-view{:0>3}, geo_mask:{:3f}, photo_mask:{:3f}, final_mask: {:3f}".format(
             os.path.join(args.input_folder, scan), ref, geo_h.mean(), photo_h.mean(), final_h.mean()))
+        # --normals: from the raw depth map (depth_est), with the view's own intrinsics at that map's size
+        normals = ops.estimate_normals(ref_depth, bank.intrinsics[ref]) if args.normals else None
         body = ops.fuse_points(final, avg, bank.images[ref].permute(1, 2, 0).contiguous(),
-                               ops.compose_fusion_camera(bank.intrinsics[ref], bank.extrinsics[ref]))
-        bodies.append(body.clone())  # drop the [H*W,15] allocation behind the returned slice
+                               ops.compose_fusion_camera(bank.intrinsics[ref], bank.extrinsics[ref]), normals)
+        bodies.append(body.clone())  # drop the [H*W,15] (or [H*W,27]) allocation behind the returned slice
     ply = os.path.join(out_dir, "fused.ply")
     data_io.save_ply(ply, bodies)
     log("saving the final model to", ply)
