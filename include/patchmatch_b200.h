@@ -249,6 +249,80 @@ int pmb200_depth_normals(const float *depth, const double *kinv_host, int H, int
                          int min_inliers, float *normals_out, void *stream);
 
 /* ------------------------------------------------------------------------------------
+ * Meshes: TSDF integration of depth maps and marching cubes (beyond the reference, which has no mesher; INTEGRATION.md
+ * "Meshes (beyond the reference)").  Definition:
+ *
+ * Grid.  The grid is anchored at the world origin.  Voxel (i, j, k) (int32) has its centre at ((i, j, k) + 0.5) * s, where s
+ * is the voxel size.  Voxels come in blocks of 8^3.  Block key = the block's (bi, bj, bk) packed into 64 bits, 21 bits per
+ * axis with an offset so that the keys sort in z, y, x order: (bk + 2^20) << 42 | (bj + 2^20) << 21 | (bi + 2^20).  Reject
+ * (PMB200_EINVAL) any point whose voxel index does not fit: floor((p -+ tau) / s) must lie in [-2^23, 2^23) on every axis.
+ *
+ * Allocation.  The allocated blocks are the sorted unique keys of every block that meets the cube [p - tau, p + tau] of some
+ * seed point p.  The truncation is tau = trunc * s, with trunc in [1, 4] voxels, so a point meets at most 8 blocks.  Memory
+ * and work are proportional to the number of allocated blocks, whatever the cloud's extent: a far outlier adds its own few
+ * blocks, never a dense box.
+ *
+ * Integration.  Each allocated voxel, with centre X in float64, runs through views v = 0..V-1 in order:
+ *   Xc = R_v X + t_v, then u = K_v Xc / Xc.z; everything float64, the float32 camera values widened;
+ *   skip the view if Xc.z <= 0;
+ *   pixel (px, py) = floor(u + 0.5); skip the view if the pixel is outside that view's own W_v x H_v;
+ *   d = depth_v[py, px] (float32); skip the view unless d is finite and > 0 (0 marks a pixel that is not an observation);
+ *   sdf = d - Xc.z; skip the view if sdf < -tau;
+ *   otherwise n += 1, F += min(1, sdf / tau), C += rgb_v[:, py, px].
+ * After the last view: weight = n, tsdf = F / n (1 when n = 0), colour = clamp(round(255 * C / n)) as uint8 (round half to
+ * even; 0 when n = 0).  There are no atomics: each voxel's sums are formed in one thread in view order, so reruns are
+ * bit-identical.
+ *
+ * Extraction (marching cubes).  A voxel is valid when it is allocated and weight >= min_weight.  The cube whose minimum corner
+ * is voxel a is meshed when all 8 of its corners are valid and its cube index (bit c set when corner c has tsdf < 0, corners
+ * numbered 0 (0,0,0), 1 (1,0,0), 2 (1,1,0), 3 (0,1,0), 4..7 the same one voxel up in z) is not 0 or 255.  Vertices lie on cube
+ * edges, and each edge belongs to its lower voxel, so a vertex shared by neighbouring cubes, including cubes in different
+ * blocks, is written once.  Vertex position: X_a + t (X_b - X_a) with t = tsdf_a / (tsdf_a - tsdf_b); its colour is
+ * interpolated the same way and rounded.  Triangles come from the 256-case table of csrc/pm_mesh_math.cuh, wound so that the
+ * right-hand normal points from negative to positive tsdf, which is towards the cameras.  The output has no unreferenced
+ * vertices: an edge gets a vertex only when one of its four cubes is meshed.  Output order:
+ *   vertices by (block key, voxel index in the block with x fastest, edge axis x / y / z);
+ *   faces by cube in the same order, then in table order.
+ *
+ * Calls (device pointers unless marked HOST; `stream` a cudaStream_t; *_workspace_bytes return bytes or a negative PMB200_E*):
+ *   pmb200_tsdf_alloc: seed points [n,3] float32 -> the sorted unique block keys, uint64 [n_blocks], written at the START of
+ *       the workspace, and n_blocks to *n_blocks_out (HOST).  Key generation, CUB radix sort and unique, then ONE host
+ *       synchronisation of `stream` (the block count sizes the volume).  PMB200_EINVAL for a null pointer, n < 0 or
+ *       n >= 2^28, s not finite and > 0, trunc outside 1..4, or a point whose voxel index does not fit.
+ *   pmb200_tsdf_integrate: one launch, one CTA per block, every view.  views_host: HOST table of n_views >= 1 views; view v
+ *       reads depth float32 [H_v,W_v] at depth_flat + depth_offset_v and image float32 [3,H_v,W_v] in [0,1] at
+ *       image_flat + image_offset_v (signed element offsets, so the views may live in separate allocations of one device).
+ *       The call copies the table into the workspace.  Outputs per voxel, index block * 512 + x + 8 y + 64 z: tsdf_out and
+ *       weight_out float32, colour_out uint8 x4 (red, green, blue, 0): 12 bytes per voxel.  1 <= n_blocks < 2^22.
+ *   pmb200_tsdf_mesh_count: per voxel its owned vertices and its cube's triangles, per block their totals, scanned;
+ *       totals_out: TWO int64 (device), the vertex and face counts.  min_weight >= 1.
+ *   pmb200_tsdf_mesh_write: with the same workspace, after the count call: vertices_out [nv,15] bytes, the records of the
+ *       plain fused.ply (float32 x, y, z, uint8 red, green, blue); faces_out int32 [nf,3].  nv < 2^31.
+ * Enqueue only, except the one synchronisation of pmb200_tsdf_alloc. */
+typedef struct pmb200_tsdf_view {
+    double K[9];            /* intrinsics, row-major */
+    double Rt[12];          /* world -> camera [R | t], row-major 3x4 */
+    int64_t depth_offset;   /* float32 elements from depth_flat */
+    int64_t image_offset;   /* float32 elements from image_flat */
+    int32_t height, width;
+} pmb200_tsdf_view;
+
+int64_t pmb200_tsdf_alloc_workspace_bytes(int64_t n_points);
+int pmb200_tsdf_alloc(const float *points, int64_t n_points, double voxel_size, int trunc, int64_t *n_blocks_out,
+                      void *workspace, int64_t workspace_bytes, void *stream);
+int64_t pmb200_tsdf_integrate_workspace_bytes(int n_views);
+int pmb200_tsdf_integrate(const uint64_t *block_keys, int64_t n_blocks, double voxel_size, int trunc,
+                          const pmb200_tsdf_view *views_host, int n_views, const float *depth_flat, const float *image_flat,
+                          float *tsdf_out, float *weight_out, unsigned char *colour_out, void *workspace,
+                          int64_t workspace_bytes, void *stream);
+int64_t pmb200_tsdf_mesh_workspace_bytes(int64_t n_blocks);
+int pmb200_tsdf_mesh_count(const uint64_t *block_keys, int64_t n_blocks, const float *tsdf, const float *weight, int min_weight,
+                           int64_t *totals_out, void *workspace, int64_t workspace_bytes, void *stream);
+int pmb200_tsdf_mesh_write(const uint64_t *block_keys, int64_t n_blocks, double voxel_size, const float *tsdf,
+                           const float *weight, const unsigned char *colour, int min_weight, unsigned char *vertices_out,
+                           int *faces_out, void *workspace, int64_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------
  * DTU point-cloud evaluation (reference evaluations/dtu/*.m; INTEGRATION.md "DTU evaluation"), float64 throughout.
  * Both calls sort the cloud into a fine / coarse cell hash held in a caller-owned device workspace of
  * *_workspace_bytes(n) bytes (O(n), whatever the extent of the cloud; the size query returns bytes or a negative PMB200_E*).

@@ -17,11 +17,12 @@ from typing import Optional
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 _REPO_DIR = os.path.dirname(_PKG_DIR)
 LIB_PATH = os.path.join(_PKG_DIR, "libpmb200.so")
-SOURCES = [os.path.join(_PKG_DIR, "csrc", f) for f in ("pm_kernels.cu", "pm_backward.cu", "pm_conv.cu", "pm_conv5.cu", "pm_stem.cu", "pm_refine.cu", "pm_geo.cu", "pm_cloud.cu", "pm_colmap.cu", "pm_train.cu", "pm_mapio.cpp")]
+SOURCES = [os.path.join(_PKG_DIR, "csrc", f) for f in ("pm_kernels.cu", "pm_backward.cu", "pm_conv.cu", "pm_conv5.cu", "pm_stem.cu", "pm_refine.cu", "pm_geo.cu", "pm_cloud.cu", "pm_colmap.cu", "pm_mesh.cu", "pm_train.cu", "pm_mapio.cpp")]
 HEADERS = [
     os.path.join(_PKG_DIR, "csrc", "pm_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_warpcorr4.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_geo_math.cuh"),
+    os.path.join(_PKG_DIR, "csrc", "pm_mesh_math.cuh"),
     os.path.join(_REPO_DIR, "include", "patchmatch_b200.h"),
 ]
 NVCC_FLAGS = [
@@ -111,6 +112,13 @@ class ViewExtent(ctypes.Structure):
 
 _PVIEW = POINTER(ViewExtent)
 
+
+class TsdfView(ctypes.Structure):
+    """pmb200_tsdf_view (include/patchmatch_b200.h): one view of the TSDF integration."""
+
+    _fields_ = [("K", c_double * 9), ("Rt", c_double * 12), ("depth_offset", c_int64), ("image_offset", c_int64),
+                ("height", c_int), ("width", c_int)]
+
 _SIGNATURES = {
     "pmb200_abi_version": (c_int, []),
     "pmb200_last_error": (c_char_p, []),
@@ -133,6 +141,13 @@ _SIGNATURES = {
     "pmb200_fuse_points": (c_int, [c_void_p] * 4 + [c_int] * 2 + [c_void_p] * 4),
     "pmb200_fuse_points_oriented": (c_int, [c_void_p] * 5 + [c_int] * 2 + [c_void_p] * 4),
     "pmb200_depth_normals": (c_int, [c_void_p, POINTER(c_double), c_int, c_int, c_int, c_double, c_int, c_void_p, c_void_p]),
+    "pmb200_tsdf_alloc_workspace_bytes": (c_int64, [c_int64]),
+    "pmb200_tsdf_alloc": (c_int, [c_void_p, c_int64, c_double, c_int, POINTER(c_int64), c_void_p, c_int64, c_void_p]),
+    "pmb200_tsdf_integrate_workspace_bytes": (c_int64, [c_int]),
+    "pmb200_tsdf_integrate": (c_int, [c_void_p, c_int64, c_double, c_int, c_void_p, c_int] + [c_void_p] * 6 + [c_int64, c_void_p]),
+    "pmb200_tsdf_mesh_workspace_bytes": (c_int64, [c_int64]),
+    "pmb200_tsdf_mesh_count": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pmb200_tsdf_mesh_write": (c_int, [c_void_p, c_int64, c_double] + [c_void_p] * 3 + [c_int] + [c_void_p] * 3 + [c_int64, c_void_p]),
     "pmb200_thin_points_workspace_bytes": (c_int64, [c_int64]),
     "pmb200_thin_points": (c_int, [c_void_p, c_void_p, c_int64, c_double, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
     "pmb200_nearest_distance_workspace_bytes": (c_int64, [c_int64]),

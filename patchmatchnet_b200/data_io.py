@@ -241,12 +241,14 @@ def save_map_from_device(path: str, tensor: torch.Tensor, scale: float = 1) -> N
         _raise(rc)
 
 
-def save_ply(path: str, body) -> None:
+def save_ply(path: str, body, faces=None) -> None:
     """Write the reference's fused.ply (eval.py:283-296: PlyData([PlyElement.describe(vertex_all, "vertex")]).write -- binary
     little endian, one `vertex` element with float x, y, z and uchar red, green, blue) from vertex records produced by
     ops.fuse_points: uint8 [n,15] tensor(s) (a list concatenates the per-reference-view clouds, eval.py:283-284).
     Oriented records, uint8 [n,27] (ops.fuse_points with normals), write float nx, ny, nz between z and red, the property
-    order of COLMAP's fused.ply; every part of one file has the same record size."""
+    order of COLMAP's fused.ply; every part of one file has the same record size.
+    With `faces`, int32 [nf,3] vertex indices (ops.tsdf_mesh), a `face` element (property list uchar int vertex_indices)
+    follows the vertices; without it the file is the vertex element alone."""
     import torch
 
     parts = list(body) if isinstance(body, (list, tuple)) else [body]
@@ -257,12 +259,25 @@ def save_ply(path: str, body) -> None:
             raise ValueError("save_ply: vertex records must be uint8 [n,15] or [n,27] tensors of one size (ops.fuse_points)")
     n = sum(int(b.shape[0]) for b in parts)
     normals = "property float nx\nproperty float ny\nproperty float nz\n" if width == 27 else ""
+    face_rows = None
+    if faces is not None:
+        fc = faces.detach().cpu().contiguous()
+        if fc.dtype != torch.int32 or fc.dim() != 2 or fc.shape[1] != 3:
+            raise ValueError("save_ply: faces must be an int32 [nf,3] tensor (ops.tsdf_mesh)")
+        if fc.numel() and (int(fc.min()) < 0 or int(fc.max()) >= n):
+            raise ValueError(f"save_ply: a face refers to a vertex outside 0..{n - 1}")
+        face_rows = np.empty(fc.shape[0], dtype=[("n", "u1"), ("v", "<i4", (3,))])
+        face_rows["n"] = 3
+        face_rows["v"] = fc.numpy()
+    face_header = "element face %d\nproperty list uchar int vertex_indices\n" % face_rows.shape[0] if face_rows is not None else ""
     header = ("ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\nproperty float z\n"
-              "%sproperty uchar red\nproperty uchar green\nproperty uchar blue\nend_header\n" % (n, normals))
+              "%sproperty uchar red\nproperty uchar green\nproperty uchar blue\n%send_header\n" % (n, normals, face_header))
     with open(path, "wb") as f:
         f.write(header.encode("ascii"))
         for b in parts:
             f.write(b.numpy().tobytes())
+        if face_rows is not None:
+            f.write(face_rows.tobytes())
 
 
 _PLY_TYPES = {

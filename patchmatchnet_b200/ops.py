@@ -1046,6 +1046,179 @@ def estimate_normals(depth: Tensor, K, radius: int = 3, depth_thres: float = 0.0
     return out
 
 
+MESH_VOXEL_BYTES = 12  # tsdf float32, weight float32, colour uchar4 per voxel (pmb200_tsdf_integrate)
+
+
+def _mesh_grid_args(voxel_size, trunc, what: str) -> Tuple[float, int]:
+    import math
+
+    if isinstance(voxel_size, bool) or not isinstance(voxel_size, (int, float)) or not math.isfinite(voxel_size) or voxel_size <= 0:
+        raise ValueError(f"{what}: voxel_size must be a positive finite number, got {voxel_size!r}")
+    if isinstance(trunc, bool) or not isinstance(trunc, int) or not 1 <= trunc <= 4:
+        raise ValueError(f"{what}: trunc must be an int in 1..4 (voxels), got {trunc!r}")
+    return float(voxel_size), int(trunc)
+
+
+def tsdf_allocate(points: Tensor, voxel_size: float, trunc: int = 3) -> Tensor:
+    """The sorted unique keys (int64 [n_blocks], the uint64 keys' bits) of every 8^3-voxel block that the cube
+    [p - trunc * voxel_size, p + trunc * voxel_size] of some seed point p meets (pmb200_tsdf_alloc).  points CUDA float32
+    [n,3].  One host synchronisation (the block count).  ValueError for bad arguments and for a point whose voxel index does
+    not fit in [-2^23, 2^23)."""
+    import ctypes
+
+    s, trunc = _mesh_grid_args(voxel_size, trunc, "tsdf_allocate")
+    if not isinstance(points, Tensor) or not _on_device(points) or points.dtype != torch.float32 or points.dim() != 2 or points.shape[1] != 3:
+        raise ValueError("tsdf_allocate: points must be a CUDA float32 [n,3] tensor")
+    pts = points.contiguous()
+    n = pts.shape[0]
+    lib = _native.lib()
+    ws_bytes = lib.pmb200_tsdf_alloc_workspace_bytes(n)
+    if ws_bytes < 0:
+        raise ValueError("tsdf_allocate: " + lib.pmb200_last_error().decode("utf-8", "replace"))
+    ws = torch.empty(max(int(ws_bytes), 1), dtype=torch.uint8, device=pts.device)
+    nb = ctypes.c_int64(0)
+    with _device_guard(pts):
+        rc = lib.pmb200_tsdf_alloc(pts.data_ptr(), n, s, trunc, ctypes.byref(nb), ws.data_ptr(), int(ws_bytes), _stream(pts))
+    if rc == -1:
+        raise ValueError(lib.pmb200_last_error().decode("utf-8", "replace"))
+    _native.check(rc, "tsdf_alloc")
+    return ws[: 8 * nb.value].view(torch.int64).clone()
+
+
+def tsdf_view_table(depths: Sequence[Tensor], images: Sequence[Tensor], Ks, Es):
+    """(ctypes array of pmb200_tsdf_view, depth base pointer, image base pointer, tensors to keep alive) for the integration.
+    The maps are read in place: each view's offsets are counted in float32 elements from the lowest-addressed map, so
+    views in separate allocations (an image bank) need no copy.  depths CUDA float32 [H_v,W_v] (0 where a pixel is not an
+    observation), images CUDA float32 [3,H_v,W_v] in [0,1], Ks [3,3] and Es [4,4] (world -> camera) float32 arrays or
+    tensors."""
+    import numpy as np
+
+    V = len(depths)
+    if V == 0 or len(images) != V or len(Ks) != V or len(Es) != V:
+        raise ValueError(f"tsdf_mesh: need one depth, image, K and E per view and at least one view (got {len(depths)}, "
+                         f"{len(images)}, {len(Ks)}, {len(Es)})")
+    f32 = lambda m: np.asarray(m.detach().cpu().numpy() if isinstance(m, Tensor) else m, dtype=np.float32)
+    keep, dev = [], None
+    table = (_native.TsdfView * V)()
+    for v in range(V):
+        d, img = depths[v], images[v]
+        for t, what in ((d, "depth"), (img, "image")):
+            if not isinstance(t, Tensor) or not _on_device(t) or t.dtype != torch.float32:
+                raise ValueError(f"tsdf_mesh: view {v}: the {what} must be a CUDA float32 tensor")
+        if d.dim() != 2 or tuple(img.shape) != (3,) + tuple(d.shape) or d.shape[0] < 1 or d.shape[1] < 1:
+            raise ValueError(f"tsdf_mesh: view {v}: depth [H,W] and image [3,H,W], got {tuple(d.shape)} and {tuple(img.shape)}")
+        if dev is None:
+            dev = d.device
+        if d.device != dev or img.device != dev:
+            raise ValueError("tsdf_mesh: every map must be on one device")
+        k, e = f32(Ks[v]), f32(Es[v])
+        if k.shape != (3, 3) or e.shape != (4, 4):
+            raise ValueError(f"tsdf_mesh: view {v}: K must be [3,3] and E [4,4], got {k.shape} and {e.shape}")
+        table[v].K[:] = k.astype(np.float64).ravel().tolist()
+        table[v].Rt[:] = e[:3, :4].astype(np.float64).ravel().tolist()
+        table[v].height, table[v].width = int(d.shape[0]), int(d.shape[1])
+        keep += [d.contiguous(), img.contiguous()]
+    dbase = min(t.data_ptr() for t in keep[0::2])
+    ibase = min(t.data_ptr() for t in keep[1::2])
+    for v in range(V):
+        table[v].depth_offset = (keep[2 * v].data_ptr() - dbase) // 4
+        table[v].image_offset = (keep[2 * v + 1].data_ptr() - ibase) // 4
+    return table, dbase, ibase, keep
+
+
+def tsdf_integrate(keys: Tensor, depths: Sequence[Tensor], images: Sequence[Tensor], Ks, Es, voxel_size: float,
+                   trunc: int = 3) -> Tuple[Tensor, Tensor, Tensor]:
+    """TSDF integration of every view into the blocks `keys` (tsdf_allocate), one launch (pmb200_tsdf_integrate; definition
+    in include/patchmatch_b200.h).  -> (tsdf float32, weight float32, colour uint8 [.,4]) per voxel, [n_blocks * 512],
+    voxel index block * 512 + x + 8 y + 64 z."""
+    import ctypes
+
+    s, trunc = _mesh_grid_args(voxel_size, trunc, "tsdf_integrate")
+    if not isinstance(keys, Tensor) or not _on_device(keys) or keys.dtype != torch.int64 or keys.dim() != 1 or keys.shape[0] < 1:
+        raise ValueError("tsdf_integrate: keys must be a non-empty CUDA int64 [n_blocks] tensor (tsdf_allocate)")
+    table, dbase, ibase, keep = tsdf_view_table(depths, images, Ks, Es)
+    if keep[0].device != keys.device:
+        raise ValueError("tsdf_integrate: the maps must be on the keys' device")
+    nb, V = keys.shape[0], len(depths)
+    lib = _native.lib()
+    ws = _workspace(lib.pmb200_tsdf_integrate_workspace_bytes(V), "tsdf_integrate_workspace_bytes", keys.device)
+    tsdf = torch.empty(nb * 512, dtype=torch.float32, device=keys.device)
+    weight = torch.empty_like(tsdf)
+    colour = torch.empty((nb * 512, 4), dtype=torch.uint8, device=keys.device)
+    with _device_guard(keys):
+        rc = lib.pmb200_tsdf_integrate(keys.data_ptr(), nb, s, trunc, ctypes.addressof(table), V, dbase, ibase, tsdf.data_ptr(),
+                                       weight.data_ptr(), colour.data_ptr(), ws.data_ptr(), ws.numel(), _stream(keys))
+    _native.check(rc, "tsdf_integrate")
+    return tsdf, weight, colour
+
+
+def tsdf_extract(keys: Tensor, tsdf: Tensor, weight: Tensor, colour: Tensor, voxel_size: float, min_weight: int = 1
+                 ) -> Tuple[Tensor, Tensor]:
+    """Marching cubes over the integrated blocks (pmb200_tsdf_mesh_count / _write): -> (vertex records uint8 [nv,15], the
+    layout of the plain fused.ply, faces int32 [nf,3]) on the device, in the documented order.  One host synchronisation
+    (the counts size the outputs)."""
+    s, _ = _mesh_grid_args(voxel_size, 1, "tsdf_extract")
+    if isinstance(min_weight, bool) or not isinstance(min_weight, int) or min_weight < 1:
+        raise ValueError(f"tsdf_extract: min_weight must be an int >= 1, got {min_weight!r}")
+    nb = keys.shape[0]
+    if tsdf.shape != (nb * 512,) or weight.shape != (nb * 512,) or colour.shape != (nb * 512, 4):
+        raise ValueError("tsdf_extract: tsdf, weight [n_blocks*512] and colour [n_blocks*512,4] as tsdf_integrate returns them")
+    lib = _native.lib()
+    ws_bytes = lib.pmb200_tsdf_mesh_workspace_bytes(nb)
+    ws = _workspace(ws_bytes, "tsdf_mesh_workspace_bytes", keys.device)
+    totals = torch.zeros(2, dtype=torch.int64, device=keys.device)
+    with _device_guard(keys):
+        rc = lib.pmb200_tsdf_mesh_count(keys.data_ptr(), nb, tsdf.data_ptr(), weight.data_ptr(), min_weight, totals.data_ptr(),
+                                        ws.data_ptr(), int(ws_bytes), _stream(keys))
+    _native.check(rc, "tsdf_mesh_count")
+    nv, nf = (int(v) for v in totals.tolist())
+    if nv >= 2 ** 31:
+        raise ValueError(f"tsdf_extract: {nv} vertices do not fit int32 face indices; use a larger voxel size")
+    verts = torch.empty((nv, 15), dtype=torch.uint8, device=keys.device)
+    faces = torch.empty((nf, 3), dtype=torch.int32, device=keys.device)
+    if nv == 0 and nf == 0:
+        return verts, faces
+    with _device_guard(keys):
+        rc = lib.pmb200_tsdf_mesh_write(keys.data_ptr(), nb, s, tsdf.data_ptr(), weight.data_ptr(), colour.data_ptr(), min_weight,
+                                        verts.data_ptr(), faces.data_ptr(), ws.data_ptr(), int(ws_bytes), _stream(keys))
+    _native.check(rc, "tsdf_mesh_write")
+    return verts, faces
+
+
+def tsdf_mesh_bytes(n_blocks: int) -> int:
+    """Device memory the volume and the extraction need for n_blocks allocated blocks (the views' maps not included):
+    n_blocks * 512 * 12 bytes of volume, plus 3 bytes per voxel and a few per block of extraction workspace."""
+    return n_blocks * 512 * (MESH_VOXEL_BYTES + 3) + n_blocks * 40
+
+
+def tsdf_mesh(points: Tensor, depths: Sequence[Tensor], images: Sequence[Tensor], Ks, Es, voxel_size: float, trunc: int = 3,
+              min_weight: int = 1) -> Tuple[Tensor, Tensor]:
+    """A coloured triangle mesh of the views' depth maps: TSDF integration over the blocks the seed points allocate, then
+    marching cubes (this project's own definition, include/patchmatch_b200.h).  points CUDA float32 [n,3] (e.g. the xyz of
+    the fused points); per view the depth float32 [H,W] (0 where there is no observation), the image float32 [3,H,W] in
+    [0,1], K [3,3] and E [4,4] (world -> camera); voxel_size in world units, trunc in voxels (1..4), min_weight the views a
+    voxel needs.  -> (vertex records uint8 [nv,15], faces int32 [nf,3]) on the device.
+
+    ValueError before any launch on bad arguments, and before the volume is allocated when its memory would exceed the
+    device's free memory (the message gives the block count: use a larger voxel size)."""
+    _mesh_grid_args(voxel_size, trunc, "tsdf_mesh")
+    if isinstance(min_weight, bool) or not isinstance(min_weight, int) or min_weight < 1:
+        raise ValueError(f"tsdf_mesh: min_weight must be an int >= 1, got {min_weight!r}")
+    tsdf_view_table(depths, images, Ks, Es)  # the views' checks, before any launch
+    keys = tsdf_allocate(points, voxel_size, trunc)
+    nb = keys.shape[0]
+    if nb == 0:
+        return torch.empty((0, 15), dtype=torch.uint8, device=points.device), torch.empty((0, 3), dtype=torch.int32, device=points.device)
+    need = tsdf_mesh_bytes(nb)
+    with _device_guard(keys):
+        free = torch.cuda.mem_get_info(keys.device)[0] + torch.cuda.memory_reserved(keys.device) - torch.cuda.memory_allocated(keys.device)
+    if nb >= 2 ** 22 or need > free:
+        raise ValueError(f"tsdf_mesh: the volume has {nb} blocks of 8^3 voxels and needs {need / 2 ** 30:.2f} GiB "
+                         f"({free / 2 ** 30:.2f} GiB free, at most 4194303 blocks); use a larger voxel size")
+    tsdf, weight, colour = tsdf_integrate(keys, depths, images, Ks, Es, voxel_size, trunc)
+    return tsdf_extract(keys, tsdf, weight, colour, voxel_size, min_weight)
+
+
 def split_ply_body(body: Tensor):
     """uint8 [n,15] vertex records -> (vertices float32 [n,3], colours uint8 [n,3]) on the CPU."""
     b = body.detach().cpu().contiguous()

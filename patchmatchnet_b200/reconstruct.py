@@ -40,6 +40,15 @@ reconstruction takes as is.  For COLMAP's own fusion and meshers, export the res
     colmap stereo_fusion --workspace_path ws --input_type geometric --output_path ws/fused.ply
     colmap poisson_mesher --input_path ws/fused.ply --output_path ws/meshed-poisson.ply
 
+With --mesh (off by default; it changes no other output) the scan is also meshed on the GPU and written to <scan>/mesh.ply,
+a coloured triangle mesh (vertex x, y, z, red, green, blue and a face element): every reference view's geometrically
+filtered depth (its final-masked averaged depth, 0 elsewhere) is integrated into a truncated signed distance volume over
+the blocks the fused points allocate, with the colours of the image bank read in place, and marching cubes extracts the
+surface (ops.tsdf_mesh; definition in include/patchmatch_b200.h).  --mesh-voxel-size defaults to twice the median over
+reference views of (median valid depth / fx), a heuristic; --mesh-trunc (voxels, 1..4) and --mesh-min-weight (views) set
+the truncation and the observations a voxel needs.  The volume needs blocks * 512 * 12 bytes besides the kept maps
+(n_ref * H * W * 4 bytes).  dtu_eval scores the mesh's vertices with --ply-template "{outputs}/scan{scan}/mesh.ply".
+
 Device memory held besides the engines, for a scan of n_img images of H x W and n_ref reference views:
     image bank   n_img * 3 * H * W * 4 bytes
     map bank     n_ref * 2 * H * W * 4 bytes
@@ -101,7 +110,25 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--normals", action="store_true",
                     help="write an oriented fused.ply (float nx, ny, nz per point, for Poisson meshers) with normals estimated "
                          "from each reference view's depth map")
+    # the mesh options stay out of the namespace unless given (defaults in MESH_DEFAULTS, read through mesh_options), so the
+    # arguments of a run without them are exactly what they were before the mesher existed
+    ap.add_argument("--mesh", action="store_true", default=argparse.SUPPRESS,
+                    help="also write mesh.ply: TSDF integration of the filtered depth maps and marching cubes, on the GPU")
+    ap.add_argument("--mesh-voxel-size", type=float, default=argparse.SUPPRESS,
+                    help="voxel edge in world units (default: twice the median over reference views of median valid depth / fx, "
+                         "a heuristic)")
+    ap.add_argument("--mesh-trunc", type=int, default=argparse.SUPPRESS, help="TSDF truncation in voxels, 1..4 (default 3)")
+    ap.add_argument("--mesh-min-weight", type=int, default=argparse.SUPPRESS,
+                    help="views that must observe a voxel for it to be meshed (default 1)")
     return ap
+
+
+MESH_DEFAULTS = {"mesh": False, "mesh_voxel_size": None, "mesh_trunc": 3, "mesh_min_weight": 1}
+
+
+def mesh_options(args: argparse.Namespace) -> argparse.Namespace:
+    """--mesh, --mesh-voxel-size, --mesh-trunc and --mesh-min-weight of `args`, with their defaults where not given."""
+    return argparse.Namespace(**{k: getattr(args, k, v) for k, v in MESH_DEFAULTS.items()})
 
 
 def parse_args(argv: Optional[Sequence[str]] = None) -> argparse.Namespace:
@@ -124,6 +151,16 @@ def check_args(args: argparse.Namespace) -> List[str]:
         raise Exception("Invalid input folder: {}".format(args.input_folder))
     if args.checkpoint_path is None or not os.path.isfile(args.checkpoint_path):
         raise Exception("Invalid checkpoint file: {}".format(args.checkpoint_path))
+    m = mesh_options(args)
+    if m.mesh:
+        if m.mesh_voxel_size is not None and not (0 < m.mesh_voxel_size < float("inf")):
+            raise ValueError(f"--mesh-voxel-size must be positive and finite, got {m.mesh_voxel_size}")
+        if not 1 <= m.mesh_trunc <= 4:
+            raise ValueError(f"--mesh-trunc must be 1..4 voxels, got {m.mesh_trunc}")
+        if m.mesh_min_weight < 1:
+            raise ValueError(f"--mesh-min-weight must be >= 1, got {m.mesh_min_weight}")
+        if args.output_type == "depth":
+            raise ValueError("--mesh needs the fusion stage (--output-type fusion or both)")
     scans = list_scans(args.scan_list)
     if not args.output_folder:
         args.output_folder = args.input_folder
@@ -331,13 +368,38 @@ class _DiskMaps:
         return self._get("depth_est", view), self._get("confidence", view)
 
 
+def default_mesh_voxel_size(depths: Sequence[Tensor], Ks: Sequence[np.ndarray]) -> float:
+    """Twice the median over reference views of (median valid depth / fx), the maps' size: about two pixel footprints at
+    a typical depth.  A heuristic."""
+    per_view = [float(d[d > 0].median()) / float(K[0, 0]) for d, K in zip(depths, Ks) if bool((d > 0).any())]
+    if not per_view:
+        raise ValueError("--mesh: no reference view has a valid depth after filtering, so there is no default voxel size")
+    return 2.0 * float(np.median(per_view))
+
+
+def mesh_scan(args: argparse.Namespace, bank: SceneBank, refs: Sequence[int], depths: Sequence[Tensor], bodies: Sequence[Tensor],
+              path: str) -> Dict[str, float]:
+    """mesh.ply of one scan from the kept final-masked depths, the fused points as seeds and the image bank."""
+    t0 = time.perf_counter()
+    m = mesh_options(args)
+    Ks = [bank.intrinsics[r] for r in refs]
+    s = m.mesh_voxel_size if m.mesh_voxel_size is not None else default_mesh_voxel_size(depths, Ks)
+    seeds = torch.cat([b[:, :12] for b in bodies]).contiguous().view(torch.float32).view(-1, 3)
+    verts, faces = ops.tsdf_mesh(seeds, depths, [bank.images[r] for r in refs], Ks, [bank.extrinsics[r] for r in refs], s,
+                                 trunc=m.mesh_trunc, min_weight=m.mesh_min_weight)
+    data_io.save_ply(path, verts, faces)
+    return {"mesh_vertices": int(verts.shape[0]), "mesh_faces": int(faces.shape[0]), "mesh_seconds": time.perf_counter() - t0}
+
+
 def fuse_scan(args: argparse.Namespace, scan: str, bank: SceneBank, pairs: Sequence[Tuple[int, List[int]]], maps,
-              log: Callable[..., None] = print) -> int:
+              log: Callable[..., None] = print) -> Tuple[int, Dict[str, float]]:
     """filter_depth (eval.py:193-297) for one scan; `maps[view]` -> (depth [H,W], confidence [H,W]) on the device.
-    Writes the mask PNGs and fused.ply (oriented with --normals); -> the number of points."""
+    Writes the mask PNGs and fused.ply (oriented with --normals), and mesh.ply with --mesh; -> (the number of points, the
+    mesh counts and seconds, empty without --mesh)."""
     out_dir = os.path.join(args.output_folder, scan)
     os.makedirs(os.path.join(out_dir, "mask"), exist_ok=True)
     bodies = []
+    mesh_depths: List[Tensor] = []  # --mesh: each reference view's final-masked averaged depth, float32, 0 elsewhere
     for ref, srcs in pairs:
         ref_depth, conf = maps[ref]
         src_list = [maps[s][0] for s in srcs]
@@ -358,17 +420,25 @@ def fuse_scan(args: argparse.Namespace, scan: str, bank: SceneBank, pairs: Seque
         body = ops.fuse_points(final, avg, bank.images[ref].permute(1, 2, 0).contiguous(),
                                ops.compose_fusion_camera(bank.intrinsics[ref], bank.extrinsics[ref]), normals)
         bodies.append(body.clone())  # drop the [H*W,15] (or [H*W,27]) allocation behind the returned slice
+        if mesh_options(args).mesh:
+            mesh_depths.append(torch.where(final.bool(), avg.float(), torch.zeros((), dtype=torch.float32, device=avg.device)))
     ply = os.path.join(out_dir, "fused.ply")
     data_io.save_ply(ply, bodies)
     log("saving the final model to", ply)
-    return sum(int(b.shape[0]) for b in bodies)
+    mesh = {}
+    if mesh_options(args).mesh:
+        path = os.path.join(out_dir, "mesh.ply")
+        mesh = mesh_scan(args, bank, [ref for ref, _ in pairs], mesh_depths, bodies, path)
+        log("saving the mesh to", path, "({} vertices, {} faces)".format(mesh["mesh_vertices"], mesh["mesh_faces"]))
+    return sum(int(b.shape[0]) for b in bodies), mesh
 
 
 def reconstruct(args: argparse.Namespace, *, device: str = "cuda:0", n_slots: int = 3,
                 log: Callable[..., None] = print) -> Dict[str, float]:
     """The command's library call.  `args` as parse_args returns it.  -> seconds of the depth stage (image decoding and
     upload, engine set-up, network, map files), of the fusion stage (filter, masks, fusion, fused.ply) and end to end, plus
-    counts (scans, depth maps, points, engines built and their set-up seconds).  Raises before it creates any output when the arguments are invalid or there is no CUDA device."""
+    counts (scans, depth maps, points, engines built and their set-up seconds); with --mesh also the mesh vertices, faces
+    and the seconds of meshing (inside the fusion stage's).  Raises before it creates any output when the arguments are invalid or there is no CUDA device."""
     scans = check_args(args)
     if not torch.cuda.is_available():
         raise RuntimeError("reconstruct needs a CUDA device (H100); there is no CPU fallback")
@@ -378,6 +448,8 @@ def reconstruct(args: argparse.Namespace, *, device: str = "cuda:0", n_slots: in
     os.makedirs(args.output_folder, exist_ok=True)
     stats = {"depth_seconds": 0.0, "fusion_seconds": 0.0, "engine_setup_seconds": 0.0, "engines_built": 0, "scans": len(scans),
              "depth_maps": 0, "points": 0}
+    if mesh_options(args).mesh:
+        stats.update({"mesh_vertices": 0, "mesh_faces": 0, "mesh_seconds": 0.0})
     t_start = time.perf_counter()
     with precision(args.tf32), torch.cuda.device(dev), torch.no_grad():
         stage = DepthStage(load_network(args).to(dev), dev, n_slots=n_slots, seed=args.seed) if do_depth else None
@@ -398,8 +470,11 @@ def reconstruct(args: argparse.Namespace, *, device: str = "cuda:0", n_slots: in
                 log(f"depth {scene_dir}: {len(maps)} maps in {t1 - t0:.3f} s")
                 t0 = t1
             if do_fusion:
-                stats["points"] += fuse_scan(args, scan, bank, pairs,
-                                             maps if maps is not None else _DiskMaps(out_dir, args.file_format, dev), log)
+                points, mesh = fuse_scan(args, scan, bank, pairs,
+                                         maps if maps is not None else _DiskMaps(out_dir, args.file_format, dev), log)
+                stats["points"] += points
+                for k, v in mesh.items():
+                    stats[k] += v
                 torch.cuda.synchronize(dev)
                 stats["fusion_seconds"] += time.perf_counter() - t0
             del bank, maps
