@@ -72,14 +72,19 @@ int pmb200_conv2d_tc5_filter_floats(int Cin, int Cout, int KS);
 int pmb200_conv2d_tc5(const float *x_nhwc, const float *filter_tc5, const float *bias, float *y_nhwc, int N, int H, int W, int Cin,
                       int Cout, int KS, int stride, int pad, int dil, int relu, int y_channel_stride, int y_channel_offset,
                       void *stream);
-/* Stride-1 form of the same convolution (K-D5h): the input halo of an 8 x 16 output tile is fetched ONCE (one dense TMA box),
+/* Stride-1 form of the same convolution (K-D5h): the input halo of an 8 x 8 output unit is fetched ONCE (one dense TMA box),
  * split once into channel-chunk planes [Cin/4][rows][cols][4 floats]; every filter tap is a shifted view of them (no-swizzle
  * K-major wgmma operand: 8 consecutive pixels of a plane are one core matrix).  Same arguments minus the stride.
  *   filter_tc5h  same float count as filter_tc5, layout [tap][Cin/4 chunks][w_hi rows Npad | w_lo rows Npad][4 floats] */
 int pmb200_conv2d_tc5h(const float *x_nhwc, const float *filter_tc5h, const float *bias, float *y_nhwc, int N, int H, int W, int Cin,
                        int Cout, int KS, int pad, int dil, int relu, int y_channel_stride, int y_channel_offset, void *stream);
+/* The shared-memory plan pmb200_conv2d_tc5h launches a layer of `units` 8 x 8 output units with, on a device of `sms` SMs whose
+ * per-block opt-in limit is smem_optin bytes: plan[0] staging buffers (1 or 2), plan[1] filter stages, plan[2] 1 when the whole
+ * filter stays resident, plan[3] dynamic shared-memory bytes, plan[4] CTAs per SM its shared memory allows (1 to 4), plan[5] plane sets
+ * (2, or 1 when units <= sms).  Non-zero when the layer does not fit. */
+int pmb200_conv2d_tc5h_plan(int Cin, int Cout, int KS, int dil, int units, int sms, int smem_optin, int *plan);
 /* Debugging aid (not a reference interface): a device buffer of 256 int64 that following K-D5h launches stamp with clock64
- * for the four roles of CTA 0 ([role][tile 0..15][event 0..3]); NULL switches it off. */
+ * for warpgroup 0 of CTA 0 ([role][unit 0..15][event 0..3]: producer, wgmmas done, split, epilogue done); NULL switches it off. */
 int pmb200_debug_conv5h_trace(long long *device_buffer_256);
 
 /* ------------------------------------------------------------------------------------

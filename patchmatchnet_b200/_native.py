@@ -133,6 +133,7 @@ _SIGNATURES = {
     "pmb200_conv2d_tc5_filter_floats": (c_int, [c_int] * 3),
     "pmb200_conv2d_tc5": (c_int, [c_void_p] * 4 + [c_int] * 12 + [c_void_p]),
     "pmb200_conv2d_tc5h": (c_int, [c_void_p] * 4 + [c_int] * 11 + [c_void_p]),
+    "pmb200_conv2d_tc5h_plan": (c_int, [c_int] * 7 + [POINTER(c_int)]),
     "pmb200_debug_conv5h_trace": (c_int, [c_void_p]),
     "pmb200_conv_stem": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_void_p]),
     "pmb200_refine_low": (c_int, [c_void_p] * 8 + [c_int] * 3 + [c_void_p]),

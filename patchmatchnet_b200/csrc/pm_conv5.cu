@@ -326,32 +326,39 @@ __global__ void __launch_bounds__(kThreads) conv5_kernel(const Conv5Params p, co
 //   * the next 8-row group of the operand = the next output row = + (halo cols * 16) bytes      (descriptor SBO),
 //   * the second half of an 8-channel K slice = the next plane = + (halo rows * cols * 16) bytes (descriptor LBO),
 //   * filter tap (ky, kx) = start address + ((ky*dil) * cols + kx*dil) * 16 bytes -- always 16-byte aligned, no swizzle phase,
-//   * the second consumer warpgroup's M = 64 half = output rows 8..15 = + 8 * cols * 16 bytes.
 // The halo tile arrives as ONE dense TMA box {Cin, cols, rows, 1} (rows of Cin*4 bytes, zero fill for the padding) in a staging
-// buffer; the two consumer warpgroups, which touch every element anyway, write A_hi / A_lo TRANSPOSED into the planes (chunk
-// order rotated by pixel: conflict-free reads and writes).  Output tile: 8 wide x 16 tall.  Load and split happen ONCE per
-// tile; the filter taps stay resident in shared memory when they fit, else stream through a small ring.
+// buffer; the consumer warpgroup that owns it, which touches every element anyway, writes A_hi / A_lo TRANSPOSED into its
+// planes (chunk order rotated by pixel: conflict-free reads and writes).
+// Work unit: the 8 x 8 output block one warpgroup's M = 64 covers.  Each consumer warpgroup walks its OWN units (worker
+// blockIdx.x + wg * gridDim.x of 2 * gridDim.x) with its own plane set: it splits, issues its wgmmas and runs its epilogue
+// without meeting the other warpgroup, so one warpgroup's split and epilogue run under the other's wgmmas.  Load and split
+// happen ONCE per unit; the filter taps stay resident in shared memory when they fit, else stream through a small ring that
+// both warpgroups read in step (a warpgroup out of units passes over the ring's taps until the other one is done).
 // The filter tap is stored as ONE operand [chunk][w_hi rows | w_lo rows][4 floats] (ops.pack_conv_filter_tc5h): a_hi x
 // [w_hi | w_lo] is one wgmma of N = 2 Npad, a_lo x w_hi one of N = Npad -- 2 wgmmas per K slice instead of 3.
 // ----------------------------------------------------------------------------------------------------------------------
-constexpr int kHTW = 8, kHTH = 16;
+constexpr int kHT = 8;  // output unit: 8 x 8 pixels = one warpgroup's M = 64
 
 struct Conv5hParams {
     const float *wpack;  // [tap][Cin/4 chunks][hi rows Npad | lo rows Npad][4]
     const float *bias;
     float *y;
     int N, H, W, Ho, Wo, Cin, Cout, Npad, KS, pad, dil, relu, ycs, yco;
-    int tiles_x, tiles_y, total_tiles;
-    int hcols, hrows;     // halo tile: 8 + dil*(KS-1) columns, 16 + dil*(KS-1) rows
+    int tiles_x, tiles_y, total_tiles;  // 8 x 8 units
+    int hcols, hrows;     // halo tile: 8 + dil*(KS-1) columns and rows
     int plane_bytes;      // hrows * hcols * 16
     int a_bytes;          // plane_bytes * Cin/4 (one of hi / lo) = what one TMA box delivers into a staging buffer
     int a_stride;         // a_bytes rounded up to 128: distance between staging buffers, hi -> lo, plane sets (2 * a_stride)
-    int hbufs;            // plane sets (hi, lo): 2 when they fit (split of tile i+1 while the other warpgroup finishes tile i), else 1
-    int sbufs;            // staging buffers: 2 when they fit (TMA of tile i+1 under the split of tile i), else 1
+    int sbufs;            // staging buffers shared by both warpgroups in request order: 2 when they fit (one per warpgroup), else 1
+    int psets;            // plane sets: 2 (one per consumer warpgroup), or 1 when there are no more units than CTAs (warpgroup 1
+                          // then never owns a unit and the space goes to the filter ring)
     int w_bytes;          // Npad * Cin * 4 (one of hi / lo)
     int wstages;
-    int w_resident;       // 1: wstages == KS*KS, every tap loaded once per CTA; 0: taps stream through the ring per tile
-    long long *trace;     // debugging aid (pmb200_debug_conv5h_trace): clock64 stamps of CTA 0's roles, [role][tile 0..15][event 0..3]
+    int w_resident;       // 1: wstages == KS*KS, every tap loaded once per CTA; 0: taps stream through the ring per unit
+    // Debugging aid (pmb200_debug_conv5h_trace): clock64 stamps of CTA 0, [role][unit 0..15 of warpgroup 0][event 0..3]:
+    // role 0 producer (ev 0: halo requested), 1 wgmmas (ev 0: all completed), 2 split (ev 0: halo landed, ev 1: planes
+    // written), 3 epilogue (ev 0: stored).  Only warpgroup 0's units are stamped.
+    long long *trace;
 };
 
 __device__ __forceinline__ void stamp(const Conv5hParams &p, int role, int it, int ev) {
@@ -374,13 +381,13 @@ template <int NPAD>
 __global__ void __launch_bounds__(kThreads) conv5h_kernel(const Conv5hParams p, const __grid_constant__ CUtensorMap xmap) {
     extern __shared__ unsigned char smem_raw[];
     unsigned char *smem = smem_raw + ((128u - (smem_u32(smem_raw) & 127u)) & 127u);
-    uint64_t *h_full = reinterpret_cast<uint64_t *>(smem);  // [2] halo tile landed in a staging buffer
-    uint64_t *s_free = h_full + 2;                           // [2] the split has read the staging buffer
+    uint64_t *h_full = reinterpret_cast<uint64_t *>(smem);  // [warpgroup] this warpgroup's next halo tile has landed
+    uint64_t *s_free = h_full + 2;                           // [sbufs] the split has read the staging buffer
     uint64_t *w_full = s_free + 2;                           // [25] filter tap landed
     uint64_t *w_empty = w_full + 25;                         // [25] its wgmmas have completed (8 consumer warps)
     unsigned char *stage0 = smem + 640;                                     // [sbufs][a_stride]  dense [rows][cols][Cin]
-    unsigned char *halo0 = stage0 + (size_t)p.sbufs * p.a_stride;           // [hbufs][hi, lo][a_stride]  planes
-    unsigned char *wring = halo0 + (size_t)p.hbufs * 2 * p.a_stride;        // [wstages][hi, lo][w_bytes]
+    unsigned char *halo0 = stage0 + (size_t)p.sbufs * p.a_stride;           // [psets][hi, lo][a_stride]  planes of warpgroup 0, 1
+    unsigned char *wring = halo0 + (size_t)p.psets * 2 * p.a_stride;        // [wstages][hi, lo][w_bytes]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
@@ -398,46 +405,60 @@ __global__ void __launch_bounds__(kThreads) conv5h_kernel(const Conv5hParams p, 
 
     const int T = p.KS * p.KS;
     const int per_img = p.tiles_x * p.tiles_y;
+    // unit k of warpgroup g is blockIdx.x + (2k + g) * gridDim.x; warpgroup 0 has n0 units, warpgroup 1 n0 or n0 - 1
+    const int G = gridDim.x, U = p.total_tiles;
+    const int n0 = ((int)blockIdx.x < U) ? (U - (int)blockIdx.x + 2 * G - 1) / (2 * G) : 0;
+    auto unit_of = [&](int g, int k) { return (int)blockIdx.x + (2 * k + g) * G; };
 
     if (warp == kProducerWarp) {
         // ------------------------------------------------ TMA producer ------------------------------------------------
+        // Halo requests are numbered r = 2k + g and take staging buffer r % sbufs: request r waits for the split of r - sbufs
+        // (only this thread waits on s_free, in request order).  Each warpgroup has its own h_full, so it waits on every phase
+        // of it in turn even when the two share one staging buffer.
         if (lane == 0) {
-            auto load_halo = [&](int tile, int use) {  // `use` = how many halo tiles this CTA has requested before
-                const int sb = use % p.sbufs;
-                const int n = tile / per_img, tt = tile - n * per_img;
+            auto load_halo = [&](int g, int k) {
+                const int u = unit_of(g, k);
+                if (k >= n0 || u >= U) return;
+                const int r = 2 * k + g, sb = r % p.sbufs;
+                const int n = u / per_img, tt = u - n * per_img;
                 const int ty = tt / p.tiles_x, tx = tt - ty * p.tiles_x;
-                mbar_wait(&s_free[sb], ((uint32_t)(use / p.sbufs) & 1u) ^ 1u);
-                stamp(p, 0, use, 0);
-                mbar_arrive_expect_tx(&h_full[sb], (uint32_t)p.a_bytes);
-                tma_box_4d(stage0 + (size_t)sb * p.a_stride, &xmap, 0, tx * kHTW - p.pad, ty * kHTH - p.pad, n, &h_full[sb]);
+                mbar_wait(&s_free[sb], ((uint32_t)(r / p.sbufs) & 1u) ^ 1u);
+                if (g == 0) stamp(p, 0, k, 0);
+                mbar_arrive_expect_tx(&h_full[g], (uint32_t)p.a_bytes);
+                tma_box_4d(stage0 + (size_t)sb * p.a_stride, &xmap, 0, tx * kHT - p.pad, ty * kHT - p.pad, n, &h_full[g]);
             };
             auto load_tap = [&](int t, int s) {
                 mbar_arrive_expect_tx(&w_full[s], (uint32_t)(2 * p.w_bytes));
                 bulk_g2s(wring + (size_t)s * 2 * p.w_bytes, reinterpret_cast<const unsigned char *>(p.wpack) + (size_t)t * 2 * p.w_bytes,
                          (uint32_t)(2 * p.w_bytes), &w_full[s]);
             };
-            if ((int)blockIdx.x < p.total_tiles) load_halo(blockIdx.x, 0);
+            load_halo(0, 0);
+            load_halo(1, 0);
             if (p.w_resident)
                 for (int t = 0; t < T; ++t) load_tap(t, t);  // the whole filter stays in shared memory: loaded once per CTA
-            int it = 0, s = 0;
+            int s = 0;
             uint32_t wpar = 0;
-            for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-                // the NEXT tile's halo first: its latency (and its split) hide under this tile's wgmmas
-                if (tile + (int)gridDim.x < p.total_tiles) load_halo(tile + gridDim.x, it + 1);
+            for (int k = 0; k < n0; ++k) {
+                // the NEXT units' halos first: their latency (and their splits) hide under this unit's wgmmas.  With one
+                // staging buffer, warpgroup 1's request waits for warpgroup 0's split of unit k + 1, which needs the taps of
+                // unit k: issue those first.
+                load_halo(0, k + 1);
+                if (p.w_resident || p.sbufs > 1) load_halo(1, k + 1);
                 if (p.w_resident) continue;
                 for (int t = 0; t < T; ++t) {
                     mbar_wait(&w_empty[s], wpar ^ 1u);
                     load_tap(t, s);
                     if (++s == p.wstages) { s = 0; wpar ^= 1u; }
                 }
+                if (p.sbufs == 1) load_halo(1, k + 1);
             }
         }
         return;
     }
     // ------------------------------------------------- consumers -------------------------------------------------
-    const int wg = warp >> 2, ct = threadIdx.x;  // ct: 0..255 over both consumer warpgroups
+    const int wg = warp >> 2, wt = threadIdx.x & 127;  // wt: 0..127 within this warpgroup
     float acc[NPAD];
-    int it = 0, s = 0;
+    int s = 0;
     uint32_t wpar = 0;
     const int kslices = p.Cin / 8;
     const int P = p.hcols * p.hrows, NC = p.Cin / 4;  // pixels of the halo tile, 16-byte channel chunks per pixel
@@ -445,21 +466,35 @@ __global__ void __launch_bounds__(kThreads) conv5h_kernel(const Conv5hParams p, 
     const uint32_t w_hiword = 128u >> 4;                  // SBO = 128 bytes
     const uint32_t a_lbo16 = (uint32_t)p.plane_bytes >> 4, w_lbo16 = 2u * (uint32_t)NPAD;  // next chunk: plane / 2 Npad rows
     const uint32_t a_kstep = 2u * a_lbo16, w_kstep = 2u * w_lbo16;                        // one K slice = two chunks
-    const uint32_t halo_u32 = smem_u32(halo0), ring_u32 = smem_u32(wring);
-    const uint32_t half16 = (uint32_t)wg * 8u * (uint32_t)p.hcols;  // output rows 8..15 for the second warpgroup
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-        const int sb = it % p.sbufs, hb = it % p.hbufs;
-        // ---- split: dense staging tile -> A_hi / A_lo planes.  With two plane sets the set of tile it-2 is free: both
-        // warpgroups passed the barrier below for tile it-1 only after their wgmmas of tile it-2 completed.  With one set,
-        // wait here until the other warpgroup's wgmmas of tile it-1 have completed.
-        mbar_wait(&h_full[sb], (uint32_t)(it / p.sbufs) & 1u);
-        if (ct == 0) stamp(p, 2, it, 0);
-        if (p.hbufs == 1) bar_sync(1, 256);
+    const uint32_t ring_u32 = smem_u32(wring);
+    unsigned char *planes = halo0 + (size_t)wg * 2 * p.a_stride;  // this warpgroup's A_hi, A_lo
+    const uint32_t ahi_lo = (smem_u32(planes) >> 4) | (a_lbo16 << 16);
+    const uint32_t alo_lo = ahi_lo + ((uint32_t)p.a_stride >> 4);
+    const bool stamps = wg == 0 && wt == 0;
+    // With a streamed filter both warpgroups read every tap of the ring, so both walk n0 units; a warpgroup whose unit lies
+    // past the end only passes over the taps.  A resident filter needs no such pass.
+    const int iters = wg == 0 || !p.w_resident ? n0 : (n0 > 0 && unit_of(1, n0 - 1) < U ? n0 : n0 - 1);
+    for (int k = 0; k < iters; ++k) {
+        const int unit = unit_of(wg, k);
+        if (unit >= U) {
+            for (int t = 0; t < T; ++t) {
+                mbar_wait(&w_full[s], wpar);
+                if (lane == 0) mbar_arrive(&w_empty[s]);
+                if (++s == p.wstages) { s = 0; wpar ^= 1u; }
+            }
+            continue;
+        }
+        // ---- split: dense staging tile -> this warpgroup's A_hi / A_lo planes.  The barrier first: every warp of the
+        // warpgroup has waited for its wgmmas of unit k - 1, which read the planes.
+        const int r = 2 * k + wg, sb = r % p.sbufs;
+        mbar_wait(&h_full[wg], (uint32_t)k & 1u);
+        if (stamps) stamp(p, 2, k, 0);
+        bar_sync(1 + wg, 128);
         {
             const float4 *src = reinterpret_cast<const float4 *>(stage0 + (size_t)sb * p.a_stride);
-            float4 *ahi = reinterpret_cast<float4 *>(halo0 + (size_t)hb * 2 * p.a_stride);
-            float4 *alo = reinterpret_cast<float4 *>(halo0 + (size_t)hb * 2 * p.a_stride + p.a_stride);
-            for (int px = ct; px < P; px += 256) {
+            float4 *ahi = reinterpret_cast<float4 *>(planes);
+            float4 *alo = reinterpret_cast<float4 *>(planes + p.a_stride);
+            for (int px = wt; px < P; px += 128) {
                 for (int j = 0; j < NC; ++j) {
                     const int c = (j + px) & (NC - 1);  // rotated by pixel: the 8 lanes of a quarter-warp read 8 bank groups
                     const float4 v = src[px * NC + c], h = tf32_hi(v);
@@ -469,23 +504,19 @@ __global__ void __launch_bounds__(kThreads) conv5h_kernel(const Conv5hParams p, 
             }
         }
         proxy_fence_async();
-        bar_sync(1, 256);
-        if (ct == 0) {
-            mbar_arrive(&s_free[sb]);
-            stamp(p, 2, it, 1);
-        }
-        // ---- wgmmas of this warpgroup's 64 rows
-        const uint32_t ahi_lo = (((halo_u32 + (uint32_t)(hb * 2 * p.a_stride)) >> 4) + half16) | (a_lbo16 << 16);
-        const uint32_t alo_lo = ahi_lo + ((uint32_t)p.a_stride >> 4);
+        bar_sync(1 + wg, 128);
+        if (wt == 0) mbar_arrive(&s_free[sb]);
+        if (stamps) stamp(p, 2, k, 1);
+        // ---- wgmmas of this unit's 64 pixels
         int pend = -1;  // ring slot whose wgmmas may still be in flight
         acc_fence(acc);
         for (int ky = 0; ky < p.KS; ++ky) {
             for (int kx = 0; kx < p.KS; ++kx) {
-                if (!p.w_resident || it == 0) mbar_wait(&w_full[s], wpar);  // a resident filter is waited for once
+                if (!p.w_resident || k == 0) mbar_wait(&w_full[s], wpar);  // a resident filter is waited for once
                 const uint32_t shift = (uint32_t)((ky * p.dil) * p.hcols + kx * p.dil);
                 const uint32_t ah = ahi_lo + shift, al = alo_lo + shift;
                 const uint32_t w = ((ring_u32 + (uint32_t)(s * 2 * p.w_bytes)) >> 4) | (w_lbo16 << 16);
-                const uint32_t first = (ky | kx) ? 1u : 0u;  // 0 for the very first wgmma of the tile (overwrites the accumulators)
+                const uint32_t first = (ky | kx) ? 1u : 0u;  // 0 for the very first wgmma of the unit (overwrites the accumulators)
                 wg_fence();
                 switch (kslices) {  // unrolled: the per-slice descriptor steps become immediates
                 case 1: issue_tap<NPAD, 1>(acc, ah, al, w, a_kstep, w_kstep, a_hiword, w_hiword, first); break;
@@ -508,12 +539,12 @@ __global__ void __launch_bounds__(kThreads) conv5h_kernel(const Conv5hParams p, 
         wg_wait<0>();
         acc_fence(acc);
         if (pend >= 0 && lane == 0) mbar_arrive(&w_empty[pend]);
-        if (ct == 0) stamp(p, 1, it, 0);
-        const int n = tile / per_img, tt = tile - n * per_img;
+        if (stamps) stamp(p, 1, k, 0);
+        const int n = unit / per_img, tt = unit - n * per_img;
         const int ty = tt / p.tiles_x, tx = tt - ty * p.tiles_x;
-        store_tile<NPAD>(acc, p.bias, p.y, n, p.Ho, p.Wo, p.Cout, p.relu, p.ycs, p.yco, 64 * wg,
-                         [&](int m, int &oy, int &ox) { oy = ty * kHTH + m / kHTW; ox = tx * kHTW + m % kHTW; });
-        if (ct == 0) stamp(p, 3, it, 0);
+        store_tile<NPAD>(acc, p.bias, p.y, n, p.Ho, p.Wo, p.Cout, p.relu, p.ycs, p.yco, 0,
+                         [&](int m, int &oy, int &ox) { oy = ty * kHT + m / kHT; ox = tx * kHT + m % kHT; });
+        if (stamps) stamp(p, 3, k, 0);
     }
 }
 
@@ -668,14 +699,66 @@ int pmb200_conv2d_tc5(const float *x_nhwc, const float *filter_tc5, const float 
     return by_npad<LaunchConv5>(p.Npad, p, xmap, dev, sms, smem_optin, reinterpret_cast<cudaStream_t>(stream));
 }
 
-// Debugging aid: device buffer of 4 roles x 16 tiles x 4 events (256 int64) that the next K-D5h launches stamp with clock64
-// for CTA 0 (producer / wgmmas done / split / epilogue done); nullptr switches it off.  Not part of the reference-facing surface.
+// Debugging aid: device buffer of 4 roles x 16 units x 4 events (256 int64) that the next K-D5h launches stamp with clock64
+// for warpgroup 0 of CTA 0 (Conv5hParams::trace: producer / wgmmas done / split / epilogue done); nullptr switches it off.  Not part of the reference-facing surface.
 int pmb200_debug_conv5h_trace(long long *device_buffer_256) {
     g_conv5h_trace = device_buffer_256;
     return 0;
 }
 
-// Stride-1 form (K-D5h): one halo tile per 8 x 16 output tile, filter taps as shifted views.  Filter image:
+// K-D5h shared-memory plan (see include/patchmatch_b200.h).  Barriers (640 B), staging buffers, one plane set (hi, lo) per
+// consumer warpgroup, filter stages, 128 B alignment slack.  Preference order: whole filter resident with a staging buffer per
+// warpgroup; resident with one shared staging buffer; else a ring as deep as fits (>= 2 stages; the staging buffer per
+// warpgroup is kept when 4 stages fit with it).  As many CTAs per SM (up to 4) as the SM's shared memory holds; the launch
+// lowers that to what the registers allow.  With no more units than SMs
+// every CTA gets one unit, run by warpgroup 0: one plane set and one staging buffer, the rest for the ring (the stage-3
+// offset convs, whose two-slot ring otherwise leaves every tap's filter load exposed).
+int pmb200_conv2d_tc5h_plan(int Cin, int Cout, int KS, int dil, int units, int sms, int smem_optin, int *plan) {
+    if (!plan || !pmb200_conv2d_tc5_supported(Cin, Cout, KS, 1) || dil < 1 || units < 1 || sms < 1)
+        return pmb200_internal_fail(PMB200_EINVAL, "conv2d_tc5h_plan: unsupported layer");
+    const int side = kHT + dil * (KS - 1);
+    if (side > 256) return pmb200_internal_fail(PMB200_EUNSUPPORTED, "conv2d_tc5h: dilation too large for one TMA box");
+    const long long a_stride = ((long long)side * side * 16 * (Cin / 4) + 127) / 128 * 128;
+    const long long w2 = 2LL * npad_of(Cout) * Cin * 4;  // one filter stage: hi + lo
+    const int T = KS * KS;
+    const int psets = units <= sms ? 1 : 2;
+    auto fixed_of = [&](int sb) { return 640 + sb * a_stride + psets * 2 * a_stride + 128; };
+    int sbufs = psets, wst = 0, resident = 0;
+    if (fixed_of(sbufs) + T * w2 <= smem_optin) { resident = 1; wst = T; }
+    else if (fixed_of(1) + T * w2 <= smem_optin) { sbufs = 1; resident = 1; wst = T; }
+    else {
+        const int want_w = T < 4 ? T : 4;
+        if (fixed_of(sbufs) + want_w * w2 > smem_optin) sbufs = 1;
+        const long long fit = (smem_optin - fixed_of(sbufs)) / w2;
+        wst = fit > 8 ? 8 : (int)(fit < 0 ? 0 : fit);
+        if (wst > T) wst = T;
+        // a ring slot is released one tap after its wgmmas were issued, so a streamed filter needs two slots
+        if (wst < 2) return pmb200_internal_fail(PMB200_EUNSUPPORTED, "conv2d_tc5h: halo tiles + filter ring do not fit in shared memory");
+    }
+    const long long per_sm = smem_optin + 1024;  // an SM's shared memory: the per-block limit + the 1 KB the driver reserves per block
+    // A resident filter that leaves room for one CTA only (conv6/7): a ring of >= 4 stages that lets two CTAs share the SM
+    // measured faster, alone and beside the other requests' kernels.
+    if (resident && psets == 2 && 2 * (fixed_of(sbufs) + wst * w2 + 1024) > per_sm) {
+        const long long budget = per_sm / 2 - 1024;
+        for (int sb = 2; sb >= 1; --sb) {
+            long long fit = (budget - fixed_of(sb)) / w2;
+            if (fit > 8) fit = 8;
+            if (fit > T) fit = T;
+            if (fit >= 4) { sbufs = sb; wst = (int)fit; resident = wst == T; break; }
+        }
+    }
+    const long long smem = fixed_of(sbufs) + wst * w2;
+    long long ctas = per_sm / (smem + 1024);
+    plan[0] = sbufs;
+    plan[1] = wst;
+    plan[2] = resident;
+    plan[3] = (int)smem;
+    plan[4] = (int)(ctas > 4 ? 4 : (ctas < 1 ? 1 : ctas));
+    plan[5] = psets;
+    return 0;
+}
+
+// Stride-1 form (K-D5h): one halo tile per 8 x 8 output unit, filter taps as shifted views.  Filter image:
 // [tap][Cin/4 chunks][hi rows Npad | lo rows Npad][4 floats] (ops.pack_conv_filter_tc5h), same float count as the per-tap form.
 int pmb200_conv2d_tc5h(const float *x_nhwc, const float *filter_tc5h, const float *bias, float *y_nhwc, int N, int H, int W, int Cin,
                        int Cout, int KS, int pad, int dil, int relu, int y_channel_stride, int y_channel_offset, void *stream) {
@@ -696,11 +779,11 @@ int pmb200_conv2d_tc5h(const float *x_nhwc, const float *filter_tc5h, const floa
     p.N = N; p.H = H; p.W = W; p.Ho = Ho; p.Wo = Wo; p.Cin = Cin; p.Cout = Cout; p.Npad = npad_of(Cout);
     p.KS = KS; p.pad = pad; p.dil = dil; p.relu = relu; p.ycs = y_channel_stride; p.yco = y_channel_offset;
     p.trace = g_conv5h_trace;
-    p.tiles_x = (Wo + kHTW - 1) / kHTW; p.tiles_y = (Ho + kHTH - 1) / kHTH;
+    p.tiles_x = (Wo + kHT - 1) / kHT; p.tiles_y = (Ho + kHT - 1) / kHT;
     const long long tiles = (long long)p.tiles_x * p.tiles_y * N;
     if (tiles > 0x7fffffffLL) return pmb200_internal_fail(PMB200_EINVAL, "conv2d_tc5h: too many tiles");
     p.total_tiles = (int)tiles;
-    p.hcols = kHTW + dil * (KS - 1); p.hrows = kHTH + dil * (KS - 1);
+    p.hcols = kHT + dil * (KS - 1); p.hrows = kHT + dil * (KS - 1);
     if (p.hcols > 256 || p.hrows > 256) return pmb200_internal_fail(PMB200_EUNSUPPORTED, "conv2d_tc5h: dilation too large for one TMA box");
     p.plane_bytes = p.hrows * p.hcols * 16;
     p.a_bytes = p.plane_bytes * (Cin / 4);
@@ -712,29 +795,11 @@ int pmb200_conv2d_tc5h(const float *x_nhwc, const float *filter_tc5h, const floa
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     p.a_stride = (p.a_bytes + 127) / 128 * 128;
-    // Shared memory: barriers (640 B), staging buffers, plane sets, filter stages, 128 B alignment slack.  Preference order:
-    // whole filter resident with both double buffers; resident with one plane set; else a ring as deep as fits (>= 2 stages
-    // wanted) with the buffers reduced in the order plane sets, staging.  Two CTAs per SM when everything fits twice.
-    const int T = KS * KS;
-    auto fixed_of = [&](int sb, int hb) { return 640 + sb * p.a_stride + hb * 2 * p.a_stride + 128; };
-    p.sbufs = 2; p.hbufs = 2; p.w_resident = 0;
-    int wst = 0;
-    if (fixed_of(2, 2) + T * 2 * p.w_bytes <= smem_optin) { p.w_resident = 1; wst = T; }
-    else if (fixed_of(2, 1) + T * 2 * p.w_bytes <= smem_optin) { p.hbufs = 1; p.w_resident = 1; wst = T; }
-    else {
-        const int want_w = T < 4 ? T : 4;
-        if (fixed_of(2, 2) + want_w * 2 * p.w_bytes > smem_optin) p.hbufs = 1;
-        if (fixed_of(2, p.hbufs) + want_w * 2 * p.w_bytes > smem_optin) p.sbufs = 1;
-        wst = (smem_optin - fixed_of(p.sbufs, p.hbufs)) / (2 * p.w_bytes);
-        if (wst > 8) wst = 8;
-        if (wst > T) wst = T;
-        if (wst < 1) return pmb200_internal_fail(PMB200_EUNSUPPORTED, "conv2d_tc5h: halo tile + filter ring do not fit in shared memory");
-    }
-    const int fixed = fixed_of(p.sbufs, p.hbufs);
-    int ctas = 1;
-    if (2 * (fixed + wst * 2 * p.w_bytes + 1024) <= smem_optin + 1024) ctas = 2;
-    p.wstages = wst;
-    const int smem = fixed + wst * 2 * p.w_bytes;
+    int plan[6];
+    const int rc = pmb200_conv2d_tc5h_plan(Cin, Cout, KS, dil, p.total_tiles, sms, smem_optin, plan);
+    if (rc != 0) return rc;
+    p.sbufs = plan[0]; p.wstages = plan[1]; p.w_resident = plan[2]; p.psets = plan[5];
+    const int smem = plan[3], ctas = plan[4];
     CUtensorMap xmap;
     const cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
     const cuuint64_t strides[3] = {(cuuint64_t)Cin * 4, (cuuint64_t)W * Cin * 4, (cuuint64_t)H * W * Cin * 4};

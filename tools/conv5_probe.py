@@ -37,8 +37,9 @@ if S == 1 and os.environ.get("C5_TRACE"):
     t = buf.cpu().view(4, 16, 4)
     t0 = int(t[t > 0].min())
     rel = torch.where(t > 0, t - t0, torch.full_like(t, -1))
-    names = {0: ("producer", ["halo requested"]), 1: ("mma", ["acc free", "planes split", "issued"]),
-             2: ("split", ["halo landed", "planes free", "done"]), 3: ("epilogue", ["acc full", "stored"])}
+    # pmb200_debug_conv5h_trace: warpgroup 0 of CTA 0, one row per 8 x 8 unit
+    names = {0: ("producer", ["halo requested"]), 1: ("mma", ["wgmmas done"]),
+             2: ("split", ["halo landed", "planes written"]), 3: ("epilogue", ["stored"])}
     out = {}
     for r, (name, evs) in names.items():
         out[name] = [{e: int(rel[r, it, k]) for k, e in enumerate(evs)} for it in range(16) if int(t[r, it, 0]) > 0]
