@@ -616,6 +616,11 @@ int pmb200_adaptive_eval(const float *score0, const float *depth_sample, const f
                          float *prob_out, float *depth_out,
                          int B, int D, int H, int W, int K, int dilation,
                          float interval_scale, int is_inverse, void *stream);
+/* The block shape pmb200_adaptive_eval launches a [B,D,H,W] evaluation with K neighbours on a device of `sms` SMs:
+ * plan[0] pixels per block (TP: 32, 16 when the map is too small to cover every SM twice, 8 when the shared-memory tile of
+ * 32 or 16 pixels exceeds 48 KB), plan[1] hypothesis lanes (DY), plan[2] shared-memory bytes.  The kb_tp / kb_dy tuning
+ * knobs, when both are set, replace (TP, DY) if TP * DY <= 256 and the tile fits 48 KB.  PMB200_EINVAL on a bad size. */
+int pmb200_adaptive_eval_plan(int B, int D, int H, int W, int K, int sms, int *plan);
 
 /* ====================================================================================
  * Backward entry points (training configuration).  Which gradients exist follows the

@@ -5,8 +5,9 @@ package; only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s
 ``cpu_baseline`` / ``--impl reference`` legs may.  The product path has no CPU
 fallback and never routes through here.
 
-What it is: a functional restatement (plain torch fp32 ops, runs on CPU or any
-torch device) of the algorithm in the reference's ``models/patchmatch.py`` and
+What it is: a functional restatement (plain torch ops in the dtype of its inputs:
+fp32 for parity with the reference, float64 as a high-precision yardstick; runs on
+CPU or any torch device) of the algorithm in the reference's ``models/patchmatch.py`` and
 ``models/module.py:130-181``.  The floating-point arithmetic of the path lives
 in PyTorch ATen (``grid_sampler_2d``, ``linalg_inv``, ``sort``, conv/BN) which
 is a third-party dependency of the reference (``requirements.txt:1`` pins no
@@ -59,8 +60,8 @@ def homography_warp(src_fea: Tensor, src_proj: Tensor, ref_proj: Tensor, depth: 
     with torch.no_grad():
         rot, trans = relative_projection(src_proj, ref_proj)
         ys, xs = torch.meshgrid(
-            torch.arange(0, H, dtype=torch.float32, device=dev),
-            torch.arange(0, W, dtype=torch.float32, device=dev),
+            torch.arange(0, H, dtype=rot.dtype, device=dev),
+            torch.arange(0, W, dtype=rot.dtype, device=dev),
             indexing="ij",
         )
         ys, xs = ys.reshape(H * W), xs.reshape(H * W)
@@ -138,8 +139,8 @@ def sampling_grid(table: Sequence[Tuple[int, int]], learned: Tensor, H: int, W: 
     dev = learned.device
     with torch.no_grad():
         ys, xs = torch.meshgrid(
-            torch.arange(0, H, dtype=torch.float32, device=dev),
-            torch.arange(0, W, dtype=torch.float32, device=dev),
+            torch.arange(0, H, dtype=learned.dtype, device=dev),
+            torch.arange(0, W, dtype=learned.dtype, device=dev),
             indexing="ij",
         )
         base = torch.stack((xs.reshape(H * W), ys.reshape(H * W))).unsqueeze(0).repeat(B, 1, 1)  # [B,2,HW]
@@ -337,8 +338,8 @@ class _Evaluation(nn.Module):
         have_w = view_weights.numel() != 0
         if have_w:
             assert len(src_feas) == view_weights.size(1), "Patchmatch Evaluation: Different number of images and view weights"
-        wsum = 1e-5 * torch.ones((B, 1, 1, H, W), dtype=torch.float32, device=dev)
-        ssum = torch.zeros((B, self.G, D, H, W), dtype=torch.float32, device=dev)
+        wsum = 1e-5 * torch.ones((B, 1, 1, H, W), dtype=ref_fea.dtype, device=dev)
+        ssum = torch.zeros((B, self.G, D, H, W), dtype=ref_fea.dtype, device=dev)
         fresh = []
         for v, (sf, sp) in enumerate(zip(src_feas, src_projs)):
             sim = groupwise_correlation(homography_warp(sf, sp, ref_proj, depth_sample), ref_fea, self.G)

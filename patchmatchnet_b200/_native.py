@@ -183,6 +183,7 @@ _SIGNATURES = {
     "pmb200_offset_corr_weight": (c_int, [c_void_p] * 2 + [c_int, _PMLP, c_void_p] + [c_int] * 7 + [c_void_p]),
     "pmb200_init_propagate": (c_int, [c_void_p] * 2 + [c_int] + [c_void_p] * 4 + [c_int] * 8 + [c_float, c_void_p]),
     "pmb200_adaptive_eval": (c_int, [c_void_p] * 5 + [c_int] + [c_void_p] * 5 + [c_int] * 6 + [c_float, c_int, c_void_p]),
+    "pmb200_adaptive_eval_plan": (c_int, [c_int] * 6 + [POINTER(c_int)]),
     "pmb200_warp_corr_backward": (c_int, [c_void_p] * 8 + [c_int] * 9 + [c_void_p]),
     "pmb200_warp_corr_views_backward": (c_int, [c_void_p, c_void_p, _PVIEW] + [c_void_p] * 6 + [c_int] * 7 + [c_void_p]),
     "pmb200_aggregate_views_backward": (c_int, [c_void_p] * 5 + [c_int] * 6 + [c_void_p]),

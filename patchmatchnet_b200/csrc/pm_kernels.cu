@@ -1754,6 +1754,35 @@ int pmb200_init_propagate(const float *seed_map, const float *offsets, int offse
     return launch_status("init_propagate");
 }
 
+int pmb200_adaptive_eval_plan(int B, int D, int H, int W, int K, int sms, int *plan) {
+    if (!plan || B < 1 || D < 1 || D > PMB200_MAX_HYPOTHESES || H < 2 || W < 2 || (K != 9 && K != 17) || sms < 1)
+        return fail(PMB200_EINVAL, "adaptive_eval_plan: bad size");
+    const long long HW = (long long)H * W;
+    // Block shape: large maps want 32 pixels x few hypothesis lanes (each thread then walks D/DY hypotheses with the
+    // footprints it already decoded), small maps 16 pixels x 16 lanes so that the grid still covers every SM twice.
+    int TP = 32, DY = D <= 16 ? (D < 4 ? D : 4) : 8;
+    if ((HW + 31) / 32 * B < 2LL * sms) {
+        TP = 16;
+        DY = D < 16 ? D : 16;
+    }
+    auto smem_for = [&](int tp) { return (size_t)K * tp * (sizeof(float4) + sizeof(int) + sizeof(float)) + 2 * (size_t)D * tp * sizeof(float); };
+    if (smem_for(TP) > 48 * 1024) {  // many hypotheses: fewer pixels per block keeps the tile under the default 48 KB
+        TP = 8;
+        DY = D < 32 ? D : 32;
+    }
+    {   // measurement aid (tools/kbench.py): kb_tp / kb_dy override the block shape
+        const int etp = tune(kTuneKbTp), edy = tune(kTuneKbDy);
+        if (etp > 0 && edy > 0 && etp * edy <= 256 && smem_for(etp) <= 48 * 1024) {
+            TP = etp;
+            DY = edy < D ? edy : D;
+        }
+    }
+    plan[0] = TP;
+    plan[1] = DY;
+    plan[2] = (int)smem_for(TP);
+    return 0;
+}
+
 int pmb200_adaptive_eval(const float *score0, const float *depth_sample, const float *xnorm, const float *xnorm_score,
                          const float *offsets, int offsets_channels_last, const float *feature_weight, const float *depth_min,
                          const float *depth_max, float *prob_out, float *depth_out, int B, int D, int H, int W, int K,
@@ -1773,26 +1802,11 @@ int pmb200_adaptive_eval(const float *score0, const float *depth_sample, const f
     p.B = B; p.D = D; p.H = H; p.W = W; p.K = K; p.dilation = dilation; p.is_inverse = is_inverse;
     p.interval_scale = interval_scale;
     const int HW = H * W;
-    // Block shape: large maps want 32 pixels x few hypothesis lanes (each thread then walks D/DY hypotheses with the
-    // footprints it already decoded), small maps 16 pixels x 16 lanes so that the grid still covers every SM twice.
-    int TP = 32, DY = D <= 16 ? (D < 4 ? D : 4) : 8;
-    if ((long long)((HW + 31) / 32) * B < 2LL * device_facts().sms) {
-        TP = 16;
-        DY = D < 16 ? D : 16;
-    }
-    auto smem_for = [&](int tp) { return (size_t)K * tp * (sizeof(float4) + sizeof(int) + sizeof(float)) + 2 * (size_t)D * tp * sizeof(float); };
-    if (smem_for(TP) > 48 * 1024) {  // many hypotheses: fewer pixels per block keeps the tile under the default 48 KB
-        TP = 8;
-        DY = D < 32 ? D : 32;
-    }
-    {   // measurement aid (tools/kbench.py): kb_tp / kb_dy override the block shape
-        const int etp = tune(kTuneKbTp), edy = tune(kTuneKbDy);
-        if (etp > 0 && edy > 0 && etp * edy <= 256 && smem_for(etp) <= 48 * 1024) {
-            TP = etp;
-            DY = edy < D ? edy : D;
-        }
-    }
-    const size_t smem = smem_for(TP);
+    int plan[3];
+    const int rc = pmb200_adaptive_eval_plan(B, D, H, W, K, device_facts().sms, plan);
+    if (rc != 0) return rc;
+    const int TP = plan[0], DY = plan[1];
+    const size_t smem = (size_t)plan[2];
     dim3 grid((HW + TP - 1) / TP, B);
     if (K == 9) adaptive_eval_kernel<9><<<grid, dim3(TP, DY), smem, as_stream(stream)>>>(p);
     else adaptive_eval_kernel<17><<<grid, dim3(TP, DY), smem, as_stream(stream)>>>(p);
