@@ -528,6 +528,11 @@ int pmb200_warp_corr_backward(const float *ref_nhwc, const float *src_nhwc, cons
         return pmb200_internal_fail(PMB200_EINVAL, "warp_corr_backward: null pointer");
     if (V < 1 || V > PMB200_MAX_VIEWS || B < 1 || B > 65535 || H < 1 || W < 1 || Hs < 1 || Ws < 1 || D < 1)
         return pmb200_internal_fail(PMB200_EINVAL, "warp_corr_backward: bad size");
+    // every check runs before anything is written: the tap keys hold a 29-bit texel index (pm::Cell)
+    if ((long long)Hs * Ws >= (1LL << pm::kKeyDxShift))
+        return pmb200_internal_fail(PMB200_EINVAL, "warp_corr_backward: source map too large");
+    if (!((C == 64 && G == 8) || (C == 32 && G == 8) || (C == 16 && G == 4)))
+        return pmb200_internal_fail(PMB200_EUNSUPPORTED, "warp_corr_backward: (C,G) must be (64,8), (32,8) or (16,4)");
     WarpCorrBwdParams p;
     p.ref = ref_nhwc; p.src = src_nhwc; p.rt = rt; p.depth = depth; p.vw = view_weights; p.gout = grad_out;
     p.dref = d_ref_nhwc; p.dsrc = d_src_nhwc;
@@ -546,8 +551,7 @@ int pmb200_warp_corr_backward(const float *ref_nhwc, const float *src_nhwc, cons
     } while (0)
     if (C == 64 && G == 8) PMB200_LAUNCH_WB(64, 8);
     else if (C == 32 && G == 8) PMB200_LAUNCH_WB(32, 8);
-    else if (C == 16 && G == 4) PMB200_LAUNCH_WB(16, 4);
-    else return pmb200_internal_fail(PMB200_EUNSUPPORTED, "warp_corr_backward: (C,G) must be (64,8), (32,8) or (16,4)");
+    else PMB200_LAUNCH_WB(16, 4);
 #undef PMB200_LAUNCH_WB
     return pmb200_internal_launch_status("warp_corr_backward");
 }
@@ -653,6 +657,13 @@ int pmb200_init_propagate_backward(const float *seed_map, const float *offsets, 
         return pmb200_internal_fail(PMB200_EINVAL, "init_propagate_backward: bad size");
     if (Kp != 4 && Kp != 8 && Kp != 16)
         return pmb200_internal_fail(PMB200_EUNSUPPORTED, "init_propagate_backward: propagate_neighbors must be 4, 8 or 16");
+    // what pmb200_init_propagate rejects: the kernel reads seed[(b*48 + k)*HW] for every k < Ns in random mode, one
+    // seed plane otherwise, and packs 29-bit texel indices (pm::border_cell)
+    if (mode == 0 && Ns != 48)
+        return pmb200_internal_fail(PMB200_EINVAL, "init_propagate_backward: random init has 48 samples");
+    if (mode == 2 && Ns != 1) return pmb200_internal_fail(PMB200_EINVAL, "init_propagate_backward: passthrough needs Ns == 1");
+    if (Ns + Kp > PMB200_MAX_HYPOTHESES) return pmb200_internal_fail(PMB200_EINVAL, "init_propagate_backward: too many hypotheses");
+    if ((long long)H * W >= (1LL << pm::kKeyDxShift)) return pmb200_internal_fail(PMB200_EINVAL, "init_propagate_backward: map too large");
     PropBwdParams p;
     p.seed = seed_map; p.offsets = offsets; p.dmin = depth_min; p.dmax = depth_max; p.gout = grad_out; p.doff = d_offsets;
     p.mode = mode; p.B = B; p.H = H; p.W = W; p.Ns = Ns; p.Kp = Kp; p.dilation = dilation; p.interval_scale = interval_scale;
@@ -673,6 +684,10 @@ int pmb200_adaptive_eval_backward(const float *score0, const float *depth_sample
     if (B < 1 || B > 65535 || H < 2 || W < 2 || D < 1 || D > PMB200_MAX_HYPOTHESES)
         return pmb200_internal_fail(PMB200_EINVAL, "adaptive_eval_backward: bad size");
     if (K != 9 && K != 17) return pmb200_internal_fail(PMB200_EUNSUPPORTED, "adaptive_eval_backward: evaluate_neighbors must be 9 or 17");
+    // what pmb200_adaptive_eval rejects, before the zero fill: the inverse regression divides by D - 1, and the gathers
+    // pack 29-bit texel indices (pm::border_cell)
+    if (is_inverse && D < 2) return pmb200_internal_fail(PMB200_EINVAL, "adaptive_eval_backward: inverse regression needs D >= 2");
+    if ((long long)H * W >= (1LL << pm::kKeyDxShift)) return pmb200_internal_fail(PMB200_EINVAL, "adaptive_eval_backward: map too large");
     EvalBwdParams p;
     p.score0 = score0; p.depth = depth_sample; p.xnorm = xnorm; p.offsets = offsets; p.fw = feature_weight;
     p.dmin = depth_min; p.dmax = depth_max; p.prob = prob; p.gdepth = grad_depth; p.gprob = grad_prob;

@@ -1732,6 +1732,7 @@ int pmb200_init_propagate(const float *seed_map, const float *offsets, int offse
         return fail(PMB200_EUNSUPPORTED, "init_propagate: propagate_neighbors must be 0, 4, 8 or 16");
     if (Kp > 0 && !offsets) return fail(PMB200_EINVAL, "init_propagate: offsets missing");
     if (Ns + Kp > PMB200_MAX_HYPOTHESES) return fail(PMB200_EINVAL, "init_propagate: too many hypotheses");
+    if ((long long)H * W >= (1LL << pm::kKeyDxShift)) return fail(PMB200_EINVAL, "init_propagate: map too large");
     PropParams p;
     p.seed = seed_map; p.offsets = offsets; p.dmin = depth_min; p.dmax = depth_max; p.out = out; p.xnorm = xnorm_out;
     p.xstride = xnorm_stride < 1 ? 1 : xnorm_stride;
@@ -1794,6 +1795,7 @@ int pmb200_adaptive_eval(const float *score0, const float *depth_sample, const f
         return fail(PMB200_EINVAL, "adaptive_eval: bad size");
     if (K != 9 && K != 17) return fail(PMB200_EUNSUPPORTED, "adaptive_eval: evaluate_neighbors must be 9 or 17");
     if (is_inverse && D < 2) return fail(PMB200_EINVAL, "adaptive_eval: inverse regression needs D >= 2");
+    if ((long long)H * W >= (1LL << pm::kKeyDxShift)) return fail(PMB200_EINVAL, "adaptive_eval: map too large");
     EvalParams p;
     p.score0 = score0; p.depth = depth_sample; p.xnorm = xnorm; p.offsets = offsets; p.fw = feature_weight;
     p.xs = reinterpret_cast<const float2 *>(xnorm_score);
