@@ -354,6 +354,46 @@ int pmb200_nearest_distance(const double *to_points, int64_t n_to, const double 
                             double max_dist, double cell, double *dist_out, void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------
+ * Tanks and Temples evaluation (beyond the reference; INTEGRATION.md "Tanks and Temples evaluation"), float64 throughout,
+ * every product and sum rounded on its own (no fused multiply-add).  Points are [n,3] float64 device arrays, n < 2^31.
+ * A 4 x 4 transform is HOST, row-major, finite, with last row exactly 0 0 0 1; a point p maps to
+ * x' = ((m00 x + m01 y) + m02 z) + m03 per row.  No call synchronises the host.
+ *
+ * pmb200_crop_polygon (Open3D's SelectionPolygonVolume): writes points_out = T p and keep_out (uint8, 1 = kept).  With
+ * w = orthogonal_axis (0 x, 1 y, 2 z) and in-plane axes (u, v) = (1, 2), (0, 2), (0, 1) for w = 0, 1, 2, a point is kept
+ * when axis_min <= p_w <= axis_max and the number of crossings c < p_u is odd.  polygon_host: HOST [n_vertices,3] (only the
+ * u and v columns are read), n_vertices <= 128.  Edge (i, j = i + 1 mod n_vertices) crosses when v_i < p_v <= v_j or
+ * v_j < p_v <= v_i, at c = u_i + ((p_v - v_i) / (v_j - v_i)) * (u_j - u_i).
+ *
+ * pmb200_voxel_downsample (Open3D's VoxelDownSample): bounds_host HOST (min xyz, max xyz) over the cloud.  Origin
+ * o = min - s/2; a point's voxel is floor((p - o) / s) per axis; PMB200_EINVAL when s * (2^31 - 1) < (max + s/2) - o on
+ * some axis, or an index would exceed 2^31 - 1.  Output: one point per occupied voxel, the float64 sum of its points in
+ * original order divided by their count, voxels in ascending (x, y, z) index order; points_out has room for n points and
+ * count_out (ONE int64, device) receives the voxel count.  Reruns give the same bits.
+ *
+ * ICP correspondences: pmb200_icp_target sorts the target into the fine / coarse cell hash of the DTU calls (cell: speed
+ * only) in a target workspace of pmb200_icp_target_workspace_bytes(n_target); that workspace is then read by any number of
+ * pmb200_icp_query calls with the same n_target and cell.  pmb200_icp_query: for each source point p' = T p (the source is
+ * never rewritten) the nearest target point with distance <= max_dist, ties to the smallest target index, written to
+ * corr_out [n_source] (int32, -1 = none; corr_out may be NULL), and over the correspondences, with p = p' - origin and
+ * q = target - origin (origin_host HOST, 3 doubles), the 18 sums moments_out (device): [0] count, [1] sum d^2,
+ * [2..4] sum p, [5..7] sum q, [8..16] sum q_a p_b (row a, column b), [17] sum |p|^2.  The sums are per-CTA partials, then
+ * one ordered sum: no atomics, so reruns give the same bits.  max_dist / 256 <= cell. */
+int pmb200_crop_polygon(const double *points, int64_t n, const double *transform_host, int orthogonal_axis, double axis_min,
+                        double axis_max, const double *polygon_host, int n_vertices, double *points_out, unsigned char *keep_out,
+                        void *stream);
+int64_t pmb200_voxel_downsample_workspace_bytes(int64_t n);
+int pmb200_voxel_downsample(const double *points, int64_t n, const double *bounds_host, double voxel_size, double *points_out,
+                            int64_t *count_out, void *workspace, int64_t workspace_bytes, void *stream);
+int64_t pmb200_icp_target_workspace_bytes(int64_t n_target);
+int pmb200_icp_target(const double *target, int64_t n_target, double cell, void *target_workspace, int64_t workspace_bytes,
+                      void *stream);
+int64_t pmb200_icp_query_workspace_bytes(int64_t n_source);
+int pmb200_icp_query(const double *source, int64_t n_source, const double *transform_host, const double *origin_host,
+                     double max_dist, const void *target_workspace, int64_t n_target, double cell, int *corr_out,
+                     double *moments_out, void *workspace, int64_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------
  * COLMAP sparse model -> scene folder (reference colmap_input.py:318-373; INTEGRATION.md "COLMAP interop"), float64 throughout.
  * The model: points xyz [n_points,3]; observations in CSR form, obs_offsets [n_images+1] (int32, obs_offsets[0] = 0) and
  * obs_points [n_obs] (int32 dense point indices in each image's own 2D-point order, -1 entries removed); camera centres

@@ -1,7 +1,9 @@
 // pm_cloud.cu -- point-cloud thinning and exact nearest-neighbour distances for the DTU point-cloud evaluation
-// (reference evaluations/dtu: reducePts_haa.m, MaxDistCP.m; semantics restated in INTEGRATION.md "DTU evaluation").
+// (reference evaluations/dtu: reducePts_haa.m, MaxDistCP.m; semantics restated in INTEGRATION.md "DTU evaluation"), and the
+// polygon crop, voxel down-sampling and ICP correspondences of the Tanks and Temples evaluation (INTEGRATION.md "Tanks and
+// Temples evaluation"; definitions in include/patchmatch_b200.h).
 //
-// Both entry points sit on one spatial structure over a float64 cloud:
+// The searches sit on one spatial structure over a float64 cloud:
 //   - fine cells of edge `cell`; fine coordinate f = floor(x / cell), clamped to [-2^20, 2^20);
 //   - coarse cells of 16^3 fine cells (coarse coordinate f >> 4, 17 bits per axis);
 //   - a 63-bit key  coarse(x,y,z) << 12 | fine-within-coarse(x,y,z): sorting the points by it (CUB radix sort) makes every
@@ -15,6 +17,7 @@
 #include <stdint.h>
 
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 #include "../../include/patchmatch_b200.h"
 
@@ -365,6 +368,286 @@ long long nearest_layout(Carver &c, long long n_to, Grid &g) {
     return (long long)c.used;
 }
 
+// ---- Tanks and Temples evaluation: polygon crop, voxel down-sampling, ICP correspondences (include/patchmatch_b200.h) ----
+
+constexpr int kMaxPolygon = 128;  // crop polygon vertices held in the kernel parameters
+constexpr int kMoments = 18;      // ICP query: count, sum d^2, sum p, sum q, sum q p^T, sum |p|^2
+
+struct Affine {
+    double m[12];  // rows of the top 3 x 4 of a 4 x 4 whose last row is 0 0 0 1
+};
+
+// ((m0 x + m1 y) + m2 z) + m3 per row, every operation rounded on its own (no fused multiply-add)
+__device__ inline void apply_affine(const Affine &t, double x, double y, double z, double &ox, double &oy, double &oz) {
+    ox = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(t.m[0], x), __dmul_rn(t.m[1], y)), __dmul_rn(t.m[2], z)), t.m[3]);
+    oy = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(t.m[4], x), __dmul_rn(t.m[5], y)), __dmul_rn(t.m[6], z)), t.m[7]);
+    oz = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(t.m[8], x), __dmul_rn(t.m[9], y)), __dmul_rn(t.m[10], z)), t.m[11]);
+}
+
+__device__ inline double pick(int a, double x, double y, double z) { return a == 0 ? x : (a == 1 ? y : z); }
+
+struct CropParams {
+    Affine t;
+    int u, v, w, nv;
+    double axis_min, axis_max;
+    double pu[kMaxPolygon], pv[kMaxPolygon];
+};
+
+__global__ void __launch_bounds__(kBlock) crop_kernel(const double *p, int n, const CropParams c, double *out, unsigned char *keep) {
+    for (int i = blockIdx.x * kBlock + threadIdx.x; i < n; i += gridDim.x * kBlock) {
+        double x, y, z;
+        apply_affine(c.t, p[3 * (size_t)i], p[3 * (size_t)i + 1], p[3 * (size_t)i + 2], x, y, z);
+        out[3 * (size_t)i] = x; out[3 * (size_t)i + 1] = y; out[3 * (size_t)i + 2] = z;
+        const double pw = pick(c.w, x, y, z), pu = pick(c.u, x, y, z), pv = pick(c.v, x, y, z);
+        bool inside = false;
+        if (pw >= c.axis_min && pw <= c.axis_max) {
+            for (int a = 0; a < c.nv; ++a) {
+                const int b = a + 1 == c.nv ? 0 : a + 1;
+                const double va = c.pv[a], vb = c.pv[b];
+                if ((va < pv && vb >= pv) || (vb < pv && va >= pv)) {
+                    const double cross = __dadd_rn(c.pu[a], __dmul_rn(__ddiv_rn(__dsub_rn(pv, va), __dsub_rn(vb, va)), __dsub_rn(c.pu[b], c.pu[a])));
+                    if (cross < pu) inside = !inside;
+                }
+            }
+        }
+        keep[i] = inside ? 1 : 0;
+    }
+}
+
+struct VoxelParams {
+    double origin[3], size;
+    int bits[3];  // key bits per axis (bits of the largest index)
+    bool split;   // the x index does not fit beside y and z in 64 bits: sort by (y, z), then stably by x
+};
+
+__device__ inline int voxel_index(double x, double origin, double size) { return (int)floor(__ddiv_rn(__dsub_rn(x, origin), size)); }
+
+__device__ inline int3 voxel_of(const double *p, int i, const VoxelParams &v) {
+    return make_int3(voxel_index(p[3 * (size_t)i], v.origin[0], v.size), voxel_index(p[3 * (size_t)i + 1], v.origin[1], v.size),
+                     voxel_index(p[3 * (size_t)i + 2], v.origin[2], v.size));
+}
+
+__global__ void __launch_bounds__(kBlock) voxel_keys_kernel(const double *p, int n, const VoxelParams v, unsigned long long *keys, int *idx) {
+    for (int i = blockIdx.x * kBlock + threadIdx.x; i < n; i += gridDim.x * kBlock) {
+        const int3 c = voxel_of(p, i, v);
+        const unsigned long long yz = ((unsigned long long)c.y << v.bits[2]) | (unsigned long long)c.z;
+        keys[i] = v.split ? yz : (((unsigned long long)c.x << (v.bits[1] + v.bits[2])) | yz);
+        idx[i] = i;
+    }
+}
+
+__global__ void __launch_bounds__(kBlock) voxel_xkeys_kernel(const double *p, int n, const VoxelParams v, const int *idx, unsigned *xkeys) {
+    for (int i = blockIdx.x * kBlock + threadIdx.x; i < n; i += gridDim.x * kBlock)
+        xkeys[i] = (unsigned)voxel_index(p[3 * (size_t)idx[i]], v.origin[0], v.size);
+}
+
+__global__ void __launch_bounds__(kBlock) voxel_flags_kernel(const double *p, int n, const VoxelParams v, const int *idx, int *flags) {
+    for (int i = blockIdx.x * kBlock + threadIdx.x; i < n; i += gridDim.x * kBlock) {
+        bool first = i == 0;
+        if (!first) {
+            const int3 a = voxel_of(p, idx[i], v), b = voxel_of(p, idx[i - 1], v);
+            first = a.x != b.x || a.y != b.y || a.z != b.z;
+        }
+        flags[i] = first ? 1 : 0;
+    }
+}
+
+// runs[k] = sorted position where voxel k starts (k < count), runs[count] = n; *count_out = count
+__global__ void __launch_bounds__(kBlock) voxel_runs_kernel(const int *flags, const int *pos, int n, int *runs, long long *count_out) {
+    for (int i = blockIdx.x * kBlock + threadIdx.x; i < n; i += gridDim.x * kBlock) {
+        if (flags[i]) runs[pos[i] - 1] = i;
+        if (i == n - 1) { runs[pos[i]] = n; *count_out = pos[i]; }
+    }
+}
+
+// one thread per voxel: the float64 sum of its points in sorted order (voxel, then original index), divided by their count
+__global__ void __launch_bounds__(kBlock) voxel_mean_kernel(const double *p, const int *idx, const int *runs, const long long *count,
+                                                            double *out) {
+    const int nv = (int)*count;
+    for (int k = blockIdx.x * kBlock + threadIdx.x; k < nv; k += gridDim.x * kBlock) {
+        const int s = runs[k], e = runs[k + 1];
+        double sx = 0.0, sy = 0.0, sz = 0.0;
+        for (int j = s; j < e; ++j) {
+            const int q = idx[j];
+            sx = __dadd_rn(sx, p[3 * (size_t)q]); sy = __dadd_rn(sy, p[3 * (size_t)q + 1]); sz = __dadd_rn(sz, p[3 * (size_t)q + 2]);
+        }
+        const double c = (double)(e - s);
+        out[3 * (size_t)k] = __ddiv_rn(sx, c); out[3 * (size_t)k + 1] = __ddiv_rn(sy, c); out[3 * (size_t)k + 2] = __ddiv_rn(sz, c);
+    }
+}
+
+struct VoxelWork {
+    unsigned long long *keys_in, *keys_sorted;
+    unsigned *x_in, *x_sorted;
+    int *idx_in, *idx_sorted, *flags, *pos, *runs;
+    void *cub_temp;
+    size_t cub_bytes;
+};
+
+long long voxel_layout(Carver &c, long long n, VoxelWork &w) {
+    const int m = (int)(n < 1 ? 1 : n);
+    w.keys_in = c.take<unsigned long long>(n);
+    w.keys_sorted = c.take<unsigned long long>(n);
+    w.x_in = c.take<unsigned>(n);
+    w.x_sorted = c.take<unsigned>(n);
+    w.idx_in = c.take<int>(n);
+    w.idx_sorted = c.take<int>(n);
+    w.flags = c.take<int>(n);
+    w.pos = c.take<int>(n);
+    w.runs = c.take<int>(n + 1);
+    size_t a = 0, b = 0, s = 0;
+    if (cub::DeviceRadixSort::SortPairs(nullptr, a, (unsigned long long *)nullptr, (unsigned long long *)nullptr, (int *)nullptr, (int *)nullptr, m, 0, 64) != cudaSuccess ||
+        cub::DeviceRadixSort::SortPairs(nullptr, b, (unsigned *)nullptr, (unsigned *)nullptr, (int *)nullptr, (int *)nullptr, m, 0, 32) != cudaSuccess ||
+        cub::DeviceScan::InclusiveSum(nullptr, s, (int *)nullptr, (int *)nullptr, m) != cudaSuccess)
+        return -1;
+    w.cub_bytes = a > b ? a : b;
+    if (s > w.cub_bytes) w.cub_bytes = s;
+    w.cub_temp = c.take<char>(w.cub_bytes);
+    return (long long)c.used;
+}
+
+inline int bit_width(long long v) {
+    int b = 0;
+    while (b < 63 && (v >> b) != 0) ++b;
+    return b;
+}
+
+// ---- ICP correspondences: nearest target point within max_dist, ties to the smallest target index ----------------------
+
+struct IcpParams {
+    const double *src;
+    int n_src;
+    Affine t;
+    Table fine, coarse;
+    const double *pts;   // target, sorted
+    const int *idx;      // target, sorted -> original index
+    double inv_cell, cell, max_dist, origin[3];
+    int *corr;           // [n_src] or NULL
+    double *partials;    // [gridDim.x][kMoments]
+};
+
+__device__ inline void scan_run_index(const double *pts, const int *idx, int2 r, double x, double y, double z, double &best, int &bi, int &bj) {
+    for (int j = r.x; j < r.y; ++j) {
+        const double d2 = dist2(x, y, z, __ldg(pts + 3 * (size_t)j), __ldg(pts + 3 * (size_t)j + 1), __ldg(pts + 3 * (size_t)j + 2));
+        const int id = __ldg(idx + j);
+        if (d2 < best || (d2 == best && id < bi)) { best = d2; bi = id; bj = j; }
+    }
+}
+
+// The ring search of nearest_kernel, keeping the index: after fine ring k every unvisited point is more than
+// (k - kCellSlack) cells away, so a point at exactly the best distance is never left unvisited and the tie rule is exact.
+__device__ inline int nearest_index(const IcpParams &p, double x, double y, double z, double &best) {
+    best = INFINITY;
+    int bi = 0x7fffffff, bj = -1;
+    bool done = false;
+    const int fx = fine_coord(x, p.inv_cell), fy = fine_coord(y, p.inv_cell), fz = fine_coord(z, p.inv_cell);
+    for (int k = 0; k <= kFineRings && !done; ++k) {
+        for (int dx = -k; dx <= k; ++dx)
+            for (int dy = -k; dy <= k; ++dy) {
+                const bool face = dx == -k || dx == k || dy == -k || dy == k;
+                for (int dz = -k; dz <= k; dz += face ? 1 : (2 * k > 0 ? 2 * k : 1)) {
+                    const long long cx = (long long)fx + dx, cy = (long long)fy + dy, cz = (long long)fz + dz;
+                    if (!in_range(cx, -kFineClamp, kFineClamp) || !in_range(cy, -kFineClamp, kFineClamp) || !in_range(cz, -kFineClamp, kFineClamp))
+                        continue;
+                    scan_run_index(p.pts, p.idx, table_find(p.fine, fine_key((int)cx, (int)cy, (int)cz)), x, y, z, best, bi, bj);
+                }
+            }
+        const double reach = (k - kCellSlack) * p.cell;
+        if (k > 0 && (__dsqrt_rn(best) <= reach || reach >= p.max_dist)) done = true;
+    }
+    if (!done) {
+        const int cx0 = fx >> kFineBits, cy0 = fy >> kFineBits, cz0 = fz >> kFineBits;
+        const double coarse = p.cell * (1 << kFineBits);
+        const long long clo = -(kFineClamp >> kFineBits), chi = kFineClamp >> kFineBits;
+        for (int m = 0; !done; ++m) {
+            for (int dx = -m; dx <= m; ++dx)
+                for (int dy = -m; dy <= m; ++dy) {
+                    const bool face = dx == -m || dx == m || dy == -m || dy == m;
+                    for (int dz = -m; dz <= m; dz += face ? 1 : (2 * m > 0 ? 2 * m : 1)) {
+                        const long long cx = (long long)cx0 + dx, cy = (long long)cy0 + dy, cz = (long long)cz0 + dz;
+                        if (!in_range(cx, clo, chi) || !in_range(cy, clo, chi) || !in_range(cz, clo, chi)) continue;
+                        const double gx = fmax(abs(dx) - 1 - kCellSlack, 0.0) * coarse, gy = fmax(abs(dy) - 1 - kCellSlack, 0.0) * coarse,
+                                     gz = fmax(abs(dz) - 1 - kCellSlack, 0.0) * coarse;
+                        if (gx * gx + gy * gy + gz * gz > best) continue;
+                        scan_run_index(p.pts, p.idx, table_find(p.coarse, coarse_key((int)cx, (int)cy, (int)cz)), x, y, z, best, bi, bj);
+                    }
+                }
+            const double reach = (m - kCellSlack) * coarse;
+            if (m > 0 && (__dsqrt_rn(best) <= reach || reach >= p.max_dist)) done = true;
+        }
+    }
+    return bj;
+}
+
+// Each thread keeps its running sums in its own column of shared memory (no registers held across the search); the block
+// sum is a fixed tree over the 256 columns.  No atomics, so the partials (and the ordered final sum of icp_finish_kernel)
+// are the same bits on every run.
+__global__ void __launch_bounds__(kBlock) icp_query_kernel(const IcpParams p) {
+    __shared__ double acc[kMoments][kBlock];
+    const int t = threadIdx.x;
+    for (int k = 0; k < kMoments; ++k) acc[k][t] = 0.0;
+    for (int i = blockIdx.x * kBlock + t; i < p.n_src; i += gridDim.x * kBlock) {
+        double x, y, z, best;
+        apply_affine(p.t, p.src[3 * (size_t)i], p.src[3 * (size_t)i + 1], p.src[3 * (size_t)i + 2], x, y, z);
+        const int j = nearest_index(p, x, y, z, best);
+        const bool hit = j >= 0 && __dsqrt_rn(best) <= p.max_dist;
+        if (p.corr) p.corr[i] = hit ? __ldg(p.idx + j) : -1;
+        if (!hit) continue;
+        const double pp[3] = {__dsub_rn(x, p.origin[0]), __dsub_rn(y, p.origin[1]), __dsub_rn(z, p.origin[2])};
+        const double qq[3] = {__dsub_rn(__ldg(p.pts + 3 * (size_t)j), p.origin[0]), __dsub_rn(__ldg(p.pts + 3 * (size_t)j + 1), p.origin[1]),
+                              __dsub_rn(__ldg(p.pts + 3 * (size_t)j + 2), p.origin[2])};
+        acc[0][t] += 1.0;
+        acc[1][t] = __dadd_rn(acc[1][t], best);
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+            acc[2 + a][t] = __dadd_rn(acc[2 + a][t], pp[a]);
+            acc[5 + a][t] = __dadd_rn(acc[5 + a][t], qq[a]);
+#pragma unroll
+            for (int b = 0; b < 3; ++b) acc[8 + 3 * a + b][t] = __dadd_rn(acc[8 + 3 * a + b][t], __dmul_rn(qq[a], pp[b]));
+        }
+        acc[17][t] = __dadd_rn(acc[17][t], __dadd_rn(__dadd_rn(__dmul_rn(pp[0], pp[0]), __dmul_rn(pp[1], pp[1])), __dmul_rn(pp[2], pp[2])));
+    }
+    __syncthreads();
+    for (int o = kBlock / 2; o > 0; o >>= 1) {
+        if (t < o)
+            for (int k = 0; k < kMoments; ++k) acc[k][t] = __dadd_rn(acc[k][t], acc[k][t + o]);
+        __syncthreads();
+    }
+    if (t < kMoments) p.partials[(size_t)blockIdx.x * kMoments + t] = acc[t][0];
+}
+
+// one CTA: moment k = the sum over blocks b of partials[b][k], each thread summing a fixed stride of blocks in order, then
+// the 256 thread sums in a fixed tree
+__global__ void __launch_bounds__(kBlock) icp_finish_kernel(const double *partials, int blocks, double *out) {
+    __shared__ double s[kBlock];
+    for (int k = 0; k < kMoments; ++k) {
+        double v = 0.0;
+        for (int b = threadIdx.x; b < blocks; b += kBlock) v = __dadd_rn(v, partials[(size_t)b * kMoments + k]);
+        s[threadIdx.x] = v;
+        __syncthreads();
+        for (int o = kBlock / 2; o > 0; o >>= 1) {
+            if (threadIdx.x < o) s[threadIdx.x] = __dadd_rn(s[threadIdx.x], s[threadIdx.x + o]);
+            __syncthreads();
+        }
+        if (threadIdx.x == 0) out[k] = s[0];
+        __syncthreads();
+    }
+}
+
+long long icp_target_layout(Carver &c, long long n_tgt, Grid &g) {
+    if (!carve_grid(c, n_tgt, true, g)) return -1;
+    return (long long)c.used;
+}
+
+// host checks of a 4 x 4 row-major transform: finite, last row exactly 0 0 0 1
+bool affine_from_host(const double *m, Affine &t) {
+    for (int k = 0; k < 16; ++k)
+        if (!(m[k] == m[k]) || m[k] == INFINITY || m[k] == -INFINITY) return false;
+    if (m[12] != 0.0 || m[13] != 0.0 || m[14] != 0.0 || m[15] != 1.0) return false;
+    for (int k = 0; k < 12; ++k) t.m[k] = m[k];
+    return true;
+}
+
 }  // namespace
 
 extern "C" int64_t pmb200_thin_points_workspace_bytes(int64_t n) {
@@ -449,4 +732,156 @@ extern "C" int pmb200_nearest_distance(const double *to_points, int64_t n_to, co
     p.out = dist_out;
     nearest_kernel<<<blocks, kBlock, 0, st>>>(p);
     return pmb200_internal_launch_status("nearest_distance");
+}
+
+extern "C" int pmb200_crop_polygon(const double *points, int64_t n, const double *transform_host, int orthogonal_axis, double axis_min,
+                                   double axis_max, const double *polygon_host, int n_vertices, double *points_out,
+                                   unsigned char *keep_out, void *stream) {
+    if (((!points || !points_out || !keep_out) && n > 0) || !transform_host || !polygon_host)
+        return pmb200_internal_fail(PMB200_EINVAL, "crop_polygon: null pointer");
+    if (n < 0 || n >= (1ll << 31)) return pmb200_internal_fail(PMB200_EINVAL, "crop_polygon: 0 <= n < 2^31");
+    if (orthogonal_axis < 0 || orthogonal_axis > 2) return pmb200_internal_fail(PMB200_EINVAL, "crop_polygon: orthogonal_axis must be 0, 1 or 2");
+    if (n_vertices < 0 || n_vertices > kMaxPolygon) return pmb200_internal_fail(PMB200_EINVAL, "crop_polygon: 0 <= n_vertices <= 128");
+    CropParams c;
+    if (!affine_from_host(transform_host, c.t))
+        return pmb200_internal_fail(PMB200_EINVAL, "crop_polygon: the transform must be finite with last row 0 0 0 1");
+    c.w = orthogonal_axis;
+    c.u = orthogonal_axis == 0 ? 1 : 0;
+    c.v = orthogonal_axis == 2 ? 1 : 2;
+    c.nv = n_vertices;
+    c.axis_min = axis_min; c.axis_max = axis_max;
+    for (int k = 0; k < n_vertices; ++k) { c.pu[k] = polygon_host[3 * k + c.u]; c.pv[k] = polygon_host[3 * k + c.v]; }
+    if (n == 0) return 0;
+    crop_kernel<<<grid_blocks(n), kBlock, 0, reinterpret_cast<cudaStream_t>(stream)>>>(points, (int)n, c, points_out, keep_out);
+    return pmb200_internal_launch_status("crop_polygon");
+}
+
+extern "C" int64_t pmb200_voxel_downsample_workspace_bytes(int64_t n) {
+    if (n < 0 || n >= (1ll << 31)) return pmb200_internal_fail(PMB200_EINVAL, "voxel_downsample_workspace_bytes: 0 <= n < 2^31");
+    Carver c{nullptr};
+    VoxelWork w;
+    const long long b = voxel_layout(c, n, w);
+    return b < 0 ? pmb200_internal_fail(PMB200_EINVAL, "voxel_downsample_workspace_bytes: no CUDA device to size the CUB calls for") : b;
+}
+
+extern "C" int pmb200_voxel_downsample(const double *points, int64_t n, const double *bounds_host, double voxel_size, double *points_out,
+                                       int64_t *count_out, void *workspace, int64_t workspace_bytes, void *stream) {
+    if (((!points || !points_out) && n > 0) || !bounds_host || !count_out || !workspace)
+        return pmb200_internal_fail(PMB200_EINVAL, "voxel_downsample: null pointer");
+    if (n < 0 || n >= (1ll << 31)) return pmb200_internal_fail(PMB200_EINVAL, "voxel_downsample: 0 <= n < 2^31");
+    if (!(voxel_size > 0.0) || !(voxel_size < INFINITY)) return pmb200_internal_fail(PMB200_EINVAL, "voxel_downsample: voxel_size must be positive and finite");
+    VoxelParams v;
+    v.size = voxel_size;
+    v.split = false;
+    int total = 0;
+    for (int a = 0; a < 3; ++a) {
+        const double lo = bounds_host[a], hi = bounds_host[3 + a];
+        if (!(lo <= hi) || !(lo > -INFINITY) || !(hi < INFINITY))
+            return pmb200_internal_fail(PMB200_EINVAL, "voxel_downsample: bounds must be finite with min <= max");
+        v.origin[a] = lo - voxel_size * 0.5;
+        // Open3D's check: the voxel bounds' extent must stay within voxel_size * INT_MAX
+        if (voxel_size * 2147483647.0 < (hi + voxel_size * 0.5) - v.origin[a])
+            return pmb200_internal_fail(PMB200_EINVAL, "voxel_downsample: voxel_size too small for the extent (int32 voxel index overflow)");
+        const double top = floor((hi - v.origin[a]) / voxel_size);  // the largest index (the ops are monotone)
+        if (!(top >= 0.0) || top > 2147483647.0)
+            return pmb200_internal_fail(PMB200_EINVAL, "voxel_downsample: voxel_size too small for the extent (int32 voxel index overflow)");
+        v.bits[a] = bit_width((long long)top);
+        total += v.bits[a];
+    }
+    v.split = total > 64;
+    Carver c{static_cast<char *>(workspace)};
+    VoxelWork w;
+    const long long need = voxel_layout(c, n, w);
+    if (need < 0 || workspace_bytes < need)
+        return pmb200_internal_fail(PMB200_EINVAL, "voxel_downsample: workspace smaller than voxel_downsample_workspace_bytes(n)");
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    cudaMemsetAsync(count_out, 0, sizeof(int64_t), st);
+    if (n == 0) return pmb200_internal_launch_status("voxel_downsample");
+    const int blocks = grid_blocks(n);
+    voxel_keys_kernel<<<blocks, kBlock, 0, st>>>(points, (int)n, v, w.keys_in, w.idx_in);
+    size_t bytes = w.cub_bytes;
+    const int key_bits = v.split ? v.bits[1] + v.bits[2] : total;
+    if (cub::DeviceRadixSort::SortPairs(w.cub_temp, bytes, w.keys_in, w.keys_sorted, w.idx_in, w.idx_sorted, (int)n, 0,
+                                        key_bits > 0 ? key_bits : 1, st) != cudaSuccess)
+        return pmb200_internal_launch_status("voxel_downsample (sort)");
+    const int *order = w.idx_sorted;
+    if (v.split) {  // radix sorts are stable: sorting by x after (y, z) leaves (x, y, z, original index) order
+        voxel_xkeys_kernel<<<blocks, kBlock, 0, st>>>(points, (int)n, v, w.idx_sorted, w.x_in);
+        bytes = w.cub_bytes;
+        if (cub::DeviceRadixSort::SortPairs(w.cub_temp, bytes, w.x_in, w.x_sorted, w.idx_sorted, w.idx_in, (int)n, 0, v.bits[0], st) != cudaSuccess)
+            return pmb200_internal_launch_status("voxel_downsample (sort)");
+        order = w.idx_in;
+    }
+    voxel_flags_kernel<<<blocks, kBlock, 0, st>>>(points, (int)n, v, order, w.flags);
+    bytes = w.cub_bytes;
+    if (cub::DeviceScan::InclusiveSum(w.cub_temp, bytes, w.flags, w.pos, (int)n, st) != cudaSuccess)
+        return pmb200_internal_launch_status("voxel_downsample (scan)");
+    voxel_runs_kernel<<<blocks, kBlock, 0, st>>>(w.flags, w.pos, (int)n, w.runs, reinterpret_cast<long long *>(count_out));
+    voxel_mean_kernel<<<blocks, kBlock, 0, st>>>(points, order, w.runs, reinterpret_cast<const long long *>(count_out), points_out);
+    return pmb200_internal_launch_status("voxel_downsample");
+}
+
+extern "C" int64_t pmb200_icp_target_workspace_bytes(int64_t n_target) {
+    if (n_target < 0 || n_target >= (1ll << 31)) return pmb200_internal_fail(PMB200_EINVAL, "icp_target_workspace_bytes: 0 <= n_target < 2^31");
+    Carver c{nullptr};
+    Grid g;
+    const long long b = icp_target_layout(c, n_target, g);
+    return b < 0 ? pmb200_internal_fail(PMB200_EINVAL, "icp_target_workspace_bytes: no CUDA device to size the CUB sort for") : b;
+}
+
+extern "C" int pmb200_icp_target(const double *target, int64_t n_target, double cell, void *target_workspace, int64_t workspace_bytes,
+                                 void *stream) {
+    if ((!target && n_target > 0) || !target_workspace) return pmb200_internal_fail(PMB200_EINVAL, "icp_target: null pointer");
+    if (n_target < 0 || n_target >= (1ll << 31)) return pmb200_internal_fail(PMB200_EINVAL, "icp_target: 0 <= n_target < 2^31");
+    if (!(cell > 0.0) || !(cell < INFINITY)) return pmb200_internal_fail(PMB200_EINVAL, "icp_target: cell must be positive and finite");
+    Carver c{static_cast<char *>(target_workspace)};
+    Grid g;
+    const long long need = icp_target_layout(c, n_target, g);
+    if (need < 0 || workspace_bytes < need)
+        return pmb200_internal_fail(PMB200_EINVAL, "icp_target: workspace smaller than icp_target_workspace_bytes(n_target)");
+    if (n_target == 0) return 0;
+    if (build_grid(g, target, (int)n_target, cell, true, reinterpret_cast<cudaStream_t>(stream)) != cudaSuccess)
+        return pmb200_internal_launch_status("icp_target (sort)");
+    return pmb200_internal_launch_status("icp_target");
+}
+
+extern "C" int64_t pmb200_icp_query_workspace_bytes(int64_t n_source) {
+    if (n_source < 0 || n_source >= (1ll << 31)) return pmb200_internal_fail(PMB200_EINVAL, "icp_query_workspace_bytes: 0 <= n_source < 2^31");
+    return (int64_t)align256((size_t)grid_blocks(n_source) * kMoments * sizeof(double));
+}
+
+extern "C" int pmb200_icp_query(const double *source, int64_t n_source, const double *transform_host, const double *origin_host,
+                                double max_dist, const void *target_workspace, int64_t n_target, double cell, int *corr_out,
+                                double *moments_out, void *workspace, int64_t workspace_bytes, void *stream) {
+    if ((!source && n_source > 0) || !transform_host || !origin_host || !target_workspace || !moments_out || !workspace)
+        return pmb200_internal_fail(PMB200_EINVAL, "icp_query: null pointer");
+    if (n_source < 0 || n_source >= (1ll << 31) || n_target < 0 || n_target >= (1ll << 31))
+        return pmb200_internal_fail(PMB200_EINVAL, "icp_query: 0 <= n_source, n_target < 2^31");
+    if (!(max_dist > 0.0) || !(max_dist < INFINITY) || !(cell >= max_dist / kMaxCellsPerDist) || !(cell < INFINITY))
+        return pmb200_internal_fail(PMB200_EINVAL, "icp_query: max_dist finite and positive, max_dist / 256 <= cell < inf");
+    IcpParams p;
+    if (!affine_from_host(transform_host, p.t))
+        return pmb200_internal_fail(PMB200_EINVAL, "icp_query: the transform must be finite with last row 0 0 0 1");
+    for (int a = 0; a < 3; ++a) {
+        if (!(origin_host[a] > -INFINITY && origin_host[a] < INFINITY)) return pmb200_internal_fail(PMB200_EINVAL, "icp_query: origin must be finite");
+        p.origin[a] = origin_host[a];
+    }
+    if (workspace_bytes < pmb200_icp_query_workspace_bytes(n_source))
+        return pmb200_internal_fail(PMB200_EINVAL, "icp_query: workspace smaller than icp_query_workspace_bytes(n_source)");
+    Carver c{const_cast<char *>(static_cast<const char *>(target_workspace))};
+    Grid g;
+    if (icp_target_layout(c, n_target, g) < 0) return pmb200_internal_fail(PMB200_EINVAL, "icp_query: no CUDA device to size the CUB sort for");
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (n_source == 0 || n_target == 0) {  // no correspondences
+        cudaMemsetAsync(moments_out, 0, kMoments * sizeof(double), st);
+        if (n_source > 0 && corr_out) cudaMemsetAsync(corr_out, 0xff, (size_t)n_source * sizeof(int), st);
+        return pmb200_internal_launch_status("icp_query");
+    }
+    p.src = source; p.n_src = (int)n_source; p.fine = g.fine; p.coarse = g.coarse; p.pts = g.pts; p.idx = g.idx_sorted;
+    p.inv_cell = 1.0 / cell; p.cell = cell; p.max_dist = max_dist; p.corr = corr_out;
+    p.partials = static_cast<double *>(workspace);
+    const int blocks = grid_blocks(n_source);
+    icp_query_kernel<<<blocks, kBlock, 0, st>>>(p);
+    icp_finish_kernel<<<1, kBlock, 0, st>>>(p.partials, blocks, moments_out);
+    return pmb200_internal_launch_status("icp_query");
 }

@@ -1300,6 +1300,162 @@ def nearest_distance(to_points: Tensor, from_points: Tensor, bb, max_dist: float
     return out
 
 
+def _host_4x4(transform):
+    """A 4 x 4 (array-like, or None for the identity) -> HOST ctypes array of 16 doubles, row-major."""
+    import ctypes
+
+    import numpy as np
+
+    m = np.eye(4) if transform is None else np.asarray(transform, dtype=np.float64).reshape(4, 4)
+    return (ctypes.c_double * 16)(*m.reshape(16).tolist())
+
+
+def crop_points(points: Tensor, orthogonal_axis: int, axis_min: float, axis_max: float, polygon, transform=None):
+    """Open3D's SelectionPolygonVolume crop (include/patchmatch_b200.h, pmb200_crop_polygon) after the 4 x 4 `transform`
+    (last row 0 0 0 1; None = identity).  points float64 [n,3] CUDA; polygon [k,3] vertices (k <= 128); orthogonal_axis
+    0 / 1 / 2 for "X" / "Y" / "Z".  -> (transformed points float64 [n,3], keep bool [n]); kept points keep their order."""
+    import ctypes
+
+    import numpy as np
+
+    pts = _points_arg(points, "crop_points")
+    n = pts.shape[0]
+    poly = np.ascontiguousarray(np.asarray(polygon, dtype=np.float64).reshape(-1, 3))
+    out = torch.empty_like(pts)
+    keep = torch.empty(n, dtype=torch.uint8, device=pts.device)
+    with _device_guard(pts):
+        rc = _native.lib().pmb200_crop_polygon(pts.data_ptr(), n, _host_4x4(transform), int(orthogonal_axis), float(axis_min),
+                                               float(axis_max), (ctypes.c_double * max(poly.size, 1))(*poly.reshape(-1).tolist()),
+                                               poly.shape[0], out.data_ptr(), keep.data_ptr(), _stream(pts))
+    _native.check(rc, "crop_points")
+    return out, keep.bool()
+
+
+def voxel_downsample(points: Tensor, voxel_size: float) -> Tensor:
+    """Open3D's VoxelDownSample (include/patchmatch_b200.h, pmb200_voxel_downsample): one point per occupied voxel of edge
+    voxel_size anchored at the cloud's min bound - voxel_size / 2, the mean of its points, voxels in ascending (x, y, z)
+    index order.  points float64 [n,3] CUDA -> float64 [m,3].  Two host reads: the cloud's bounds and the voxel count."""
+    import ctypes
+
+    pts = _points_arg(points, "voxel_downsample")
+    n = pts.shape[0]
+    if n == 0:
+        return pts.new_empty((0, 3))
+    lo, hi = torch.aminmax(pts, dim=0)
+    bounds = (ctypes.c_double * 6)(*torch.cat([lo, hi]).cpu().tolist())
+    out = torch.empty_like(pts)
+    count = torch.empty(1, dtype=torch.int64, device=pts.device)
+    lib = _native.lib()
+    ws = _workspace(lib.pmb200_voxel_downsample_workspace_bytes(n), "voxel_downsample_workspace_bytes", pts.device)
+    with _device_guard(pts):
+        rc = lib.pmb200_voxel_downsample(pts.data_ptr(), n, bounds, float(voxel_size), out.data_ptr(), count.data_ptr(),
+                                         ws.data_ptr(), ws.numel(), _stream(pts))
+    _native.check(rc, "voxel_downsample")
+    return out[: int(count.item())]
+
+
+def umeyama_from_moments(m) -> "np.ndarray":
+    """The similarity (with scaling) that best maps the correspondences' source points onto their targets (Umeyama 1991, the
+    estimate of Eigen::umeyama with scaling), from the 18 sums of pmb200_icp_query taken relative to an origin o:
+        mu_p = S_p / n, mu_q = S_q / n, Sigma = S_qp / n - mu_q mu_p^T, var_p = S_pp / n - |mu_p|^2,
+        Sigma = U D V^T (numpy's SVD), S = diag(1, 1, -1 if det(U) det(V) < 0 else 1),
+        R = U S V^T, c = trace(D S) / var_p, t = mu_q - c R mu_p.
+    -> float64 [4,4] acting on coordinates relative to o.  The identity when there is no correspondence."""
+    import numpy as np
+
+    m = np.asarray(m, dtype=np.float64)
+    n = m[0]
+    if n == 0:
+        return np.eye(4)
+    mu_p, mu_q = m[2:5] / n, m[5:8] / n
+    sigma = m[8:17].reshape(3, 3) / n - np.outer(mu_q, mu_p)
+    var_p = m[17] / n - mu_p @ mu_p
+    u, d, vt = np.linalg.svd(sigma)
+    s = np.ones(3)
+    if np.linalg.det(u) * np.linalg.det(vt) < 0:
+        s[2] = -1.0
+    r = (u * s) @ vt
+    c = (d @ s) / var_p
+    out = np.eye(4)
+    out[:3, :3] = c * r
+    out[:3, 3] = mu_q - c * (r @ mu_p)
+    return out
+
+
+def icp(source: Tensor, target: Tensor, max_dist: float, max_iteration: int = 30, init=None, relative_fitness: float = 1e-6,
+        relative_rmse: float = 1e-6, cell: Optional[float] = None, return_correspondences: bool = False) -> dict:
+    """Point-to-point ICP with scaling, Open3D's registration_icp loop (INTEGRATION.md "Tanks and Temples evaluation"):
+    correspondences of T = init (nearest target point within distance <= max_dist, ties to the smallest target index),
+    fitness = |C| / |source| and inlier RMSE = sqrt(sum d^2 / |C|) (0 without correspondences); then per iteration the
+    Umeyama similarity of the correspondences is composed onto T and the correspondences are recomputed, stopping once
+    |delta fitness| < relative_fitness and |delta RMSE| < relative_rmse, or after max_iteration updates.  The target is
+    sorted into its cell hash once; each evaluation is one query launch (the source transformed in the kernel) and one
+    device-to-host copy of 18 sums.  source [n,3], target [m,3] float64 CUDA ->
+    {"transformation" float64 [4,4], "fitness", "inlier_rmse", "iterations", "correspondences" (final |C|),
+     "history" [(|C|, sum d^2)] of every evaluation, and "correspondence_set" int32 [n] (-1 = none) when asked}."""
+    import ctypes
+    import math
+
+    import numpy as np
+
+    src = _points_arg(source, "icp (source)")
+    tgt = _points_arg(target, "icp (target)")
+    if src.device != tgt.device:
+        raise RuntimeError("icp: both clouds must be on the same device")
+    if not (max_dist > 0 and math.isfinite(max_dist)):
+        raise ValueError("icp: max_dist must be positive and finite")
+    n_src, n_tgt = src.shape[0], tgt.shape[0]
+    lib = _native.lib()
+    if n_tgt > 0:
+        lo, hi = torch.aminmax(tgt, dim=0)
+        lo, hi = lo.cpu().numpy(), hi.cpu().numpy()
+    else:
+        lo = hi = np.zeros(3)
+    origin = (ctypes.c_double * 3)(*((lo + hi) / 2).tolist())
+    if cell is None:
+        cell = default_search_cell(n_tgt, [lo, hi], max_dist)
+    tws = _workspace(lib.pmb200_icp_target_workspace_bytes(n_tgt), "icp_target_workspace_bytes", src.device)
+    qws = _workspace(lib.pmb200_icp_query_workspace_bytes(n_src), "icp_query_workspace_bytes", src.device)
+    moments = torch.empty(18, dtype=torch.float64, device=src.device)
+    corr = torch.empty(n_src, dtype=torch.int32, device=src.device) if return_correspondences else None
+    with _device_guard(src):
+        _native.check(lib.pmb200_icp_target(tgt.data_ptr(), n_tgt, float(cell), tws.data_ptr(), tws.numel(), _stream(tgt)), "icp_target")
+
+    def evaluate(t):
+        with _device_guard(src):
+            rc = lib.pmb200_icp_query(src.data_ptr(), n_src, _host_4x4(t), origin, float(max_dist), tws.data_ptr(), n_tgt, float(cell),
+                                      corr.data_ptr() if corr is not None else None, moments.data_ptr(), qws.data_ptr(), qws.numel(),
+                                      _stream(src))
+        _native.check(rc, "icp_query")
+        m = moments.cpu().numpy()
+        fit = m[0] / n_src if n_src else 0.0
+        return m, fit, (math.sqrt(m[1] / m[0]) if m[0] > 0 else 0.0)
+
+    t = np.eye(4) if init is None else np.asarray(init, dtype=np.float64).reshape(4, 4).copy()
+    m, fitness, rmse = evaluate(t)
+    history = [(int(m[0]), float(m[1]))]
+    o = np.asarray(origin[:])
+    iterations = 0
+    for _ in range(max_iteration):
+        rel = umeyama_from_moments(m)  # acts on coordinates relative to the origin
+        upd = np.eye(4)
+        upd[:3, :3] = rel[:3, :3]
+        upd[:3, 3] = rel[:3, 3] + o - rel[:3, :3] @ o
+        t = upd @ t
+        m, f2, r2 = evaluate(t)
+        history.append((int(m[0]), float(m[1])))
+        iterations += 1
+        done = abs(fitness - f2) < relative_fitness and abs(rmse - r2) < relative_rmse
+        fitness, rmse = f2, r2
+        if done:
+            break
+    out = {"transformation": t, "fitness": fitness, "inlier_rmse": rmse, "iterations": iterations,
+           "correspondences": int(m[0]), "history": history}
+    if corr is not None:
+        out["correspondence_set"] = corr
+    return out
+
+
 def _model_args(xyz: Tensor, obs_offsets: Tensor, obs_points: Tensor, per_image: Tensor, per_image_shape, name: str):
     """Checks of a sparse model held on the device (ops.view_scores / ops.depth_ranges) -> contiguous tensors and N, M."""
     for t, what in ((xyz, "xyz"), (obs_offsets, "obs_offsets"), (obs_points, "obs_points"), (per_image, "per-image cameras")):

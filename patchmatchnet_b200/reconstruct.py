@@ -48,6 +48,7 @@ surface (ops.tsdf_mesh; definition in include/patchmatch_b200.h).  --mesh-voxel-
 reference views of (median valid depth / fx), a heuristic; --mesh-trunc (voxels, 1..4) and --mesh-min-weight (views) set
 the truncation and the observations a voxel needs.  The volume needs blocks * 512 * 12 bytes besides the kept maps
 (n_ref * H * W * 4 bytes).  dtu_eval scores the mesh's vertices with --ply-template "{outputs}/scan{scan}/mesh.ply".
+tnt_eval scores a Tanks and Temples training scene's fused.ply (or its mesh.ply) by precision, recall and F-score.
 
 Device memory held besides the engines, for a scan of n_img images of H x W and n_ref reference views:
     image bank   n_img * 3 * H * W * 4 bytes
