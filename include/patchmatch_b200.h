@@ -424,6 +424,39 @@ int pmb200_depth_ranges(const double *xyz, int64_t n_points, const int *obs_offs
                         int n_images, int64_t n_obs, double *ranges_out, void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------
+ * Undistortion of COLMAP cameras (beyond the reference; INTEGRATION.md "Undistortion (beyond the reference)"), float64
+ * throughout, every operation rounded on its own (no fused multiply-add).  The camera models are COLMAP's 11, with its model
+ * ids and parameter order (patchmatchnet_b200/csrc/pm_camera_math.cuh).  A camera is valid when its model is 0..10,
+ * 1 <= width, height <= 2^20, its parameters are finite and its focal lengths non-zero; PMB200_EINVAL otherwise.
+ *
+ * pmb200_undistort_extents: for each camera c of cameras_host (HOST, n_cameras <= 65535), the border extents of COLMAP's
+ *   UndistortCamera: with P the PINHOLE camera of the same fx, fy, cx, cy, each border pixel centre is mapped through
+ *   P.WorldToImage(c.ImageToWorld(.)); extents_out [n_cameras,8] (device) = min and max of the mapped x over the left points
+ *   (0.5, y + 0.5), min and max over the right points (W - 0.5, y + 0.5), then min and max of the mapped y over the top points
+ *   (x + 0.5, 0.5) and the bottom points (x + 0.5, H - 0.5).  A point whose Newton iteration breaks down (NaN) is skipped.
+ *   The call copies the cameras into cameras_device (device, room for n_cameras), then one launch, one block per camera.
+ * pmb200_undistort_image: src uint8 [H,W,3] RGB (device; W, H = the camera's size), dst uint8 [out_height,out_width,3].
+ *   pinhole_host: HOST (fx', fy', cx', cy') of the target PINHOLE camera.  Per target pixel (x, y):
+ *     u = (x + 0.5 - cx') / fx', v = (y + 0.5 - cy') / fy';  (xs, ys) = c.WorldToImage(u, v) - 0.5;
+ *     valid when xs, ys are finite, 0 <= xs <= W - 1 and 0 <= ys <= H - 1;
+ *     x0 = floor(xs), dx = xs - x0, x1 = min(x0 + 1, W - 1), likewise y;
+ *     channel = (1 - dy)((1 - dx) p00 + dx p01) + dy((1 - dx) p10 + dx p11) (p_ab = src[y_a, x_b]), rounded half away from
+ *     zero and clamped to 0..255;  an invalid pixel is 0 in every channel.
+ *   Offsets are int64.  One launch.
+ * Enqueue only. */
+typedef struct pmb200_camera {
+    int32_t model;          /* COLMAP model id, 0..10 */
+    int32_t width, height;
+    int32_t reserved;       /* 0 */
+    double params[12];      /* COLMAP's parameter order; entries past the model's count are ignored */
+} pmb200_camera;
+
+int pmb200_undistort_extents(const pmb200_camera *cameras_host, int n_cameras, pmb200_camera *cameras_device, double *extents_out,
+                             void *stream);
+int pmb200_undistort_image(const unsigned char *src, const pmb200_camera *camera_host, const double *pinhole_host, int out_width,
+                           int out_height, unsigned char *dst, void *stream);
+
+/* ------------------------------------------------------------------------------------
  * Training loss and metrics (reference models/net.py:321-342 patchmatchnet_loss, train.py:174-180 create_stage_images,
  * utils.py:187-221 absolute_depth_error_metrics / threshold_metrics; DESIGN.md K-L).
  *   depth_gt [B,H,W] float32 and mask [B,H,W] uint8 (0 / non-0) at full resolution.  The level-l ground truth and mask at

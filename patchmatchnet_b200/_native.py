@@ -17,12 +17,13 @@ from typing import Optional
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 _REPO_DIR = os.path.dirname(_PKG_DIR)
 LIB_PATH = os.path.join(_PKG_DIR, "libpmb200.so")
-SOURCES = [os.path.join(_PKG_DIR, "csrc", f) for f in ("pm_kernels.cu", "pm_backward.cu", "pm_conv.cu", "pm_conv5.cu", "pm_stem.cu", "pm_refine.cu", "pm_geo.cu", "pm_cloud.cu", "pm_colmap.cu", "pm_mesh.cu", "pm_train.cu", "pm_mapio.cpp")]
+SOURCES = [os.path.join(_PKG_DIR, "csrc", f) for f in ("pm_kernels.cu", "pm_backward.cu", "pm_conv.cu", "pm_conv5.cu", "pm_stem.cu", "pm_refine.cu", "pm_geo.cu", "pm_cloud.cu", "pm_colmap.cu", "pm_undistort.cu", "pm_mesh.cu", "pm_train.cu", "pm_mapio.cpp")]
 HEADERS = [
     os.path.join(_PKG_DIR, "csrc", "pm_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_warpcorr4.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_geo_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_mesh_math.cuh"),
+    os.path.join(_PKG_DIR, "csrc", "pm_camera_math.cuh"),
     os.path.join(_REPO_DIR, "include", "patchmatch_b200.h"),
 ]
 NVCC_FLAGS = [
@@ -119,6 +120,14 @@ class TsdfView(ctypes.Structure):
     _fields_ = [("K", c_double * 9), ("Rt", c_double * 12), ("depth_offset", c_int64), ("image_offset", c_int64),
                 ("height", c_int), ("width", c_int)]
 
+
+class CameraStruct(ctypes.Structure):
+    """pmb200_camera (include/patchmatch_b200.h): one COLMAP camera of the undistortion."""
+
+    _fields_ = [("model", c_int), ("width", c_int), ("height", c_int), ("reserved", c_int), ("params", c_double * 12)]
+
+
+_PCAM = POINTER(CameraStruct)
 _SIGNATURES = {
     "pmb200_abi_version": (c_int, []),
     "pmb200_last_error": (c_char_p, []),
@@ -168,6 +177,8 @@ _SIGNATURES = {
                                    c_void_p, c_void_p, c_int64, c_void_p]),
     "pmb200_depth_ranges_workspace_bytes": (c_int64, [c_int, c_int64]),
     "pmb200_depth_ranges": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pmb200_undistort_extents": (c_int, [_PCAM, c_int, c_void_p, c_void_p, c_void_p]),
+    "pmb200_undistort_image": (c_int, [c_void_p, _PCAM, POINTER(c_double), c_int, c_int, c_void_p, c_void_p]),
     "pmb200_depth_loss_workspace_bytes": (c_int64, [POINTER(c_int), c_int, c_int, c_int, c_int]),
     "pmb200_depth_loss": (c_int, [_PPF, POINTER(c_int), c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int64,
                                   c_void_p]),

@@ -1,18 +1,23 @@
 """COLMAP sparse model -> scene folder (pair.txt, cams/%08d_cam.txt, images/%08d.jpg): the counterpart of the reference's
 colmap_input.py, with view selection and depth ranges on the GPU.
 
-    colmap image_undistorter --image_path photos --input_path sparse/0 --output_path undistorted
-    python -m patchmatchnet_b200.colmap_input --input-folder undistorted
-    python -m patchmatchnet_b200.reconstruct --input-folder undistorted --checkpoint-path model.pt
+    python -m patchmatchnet_b200.colmap_input --input-folder project --undistort
+    python -m patchmatchnet_b200.reconstruct --input-folder project --checkpoint-path model.pt
 
 Input: <input folder>/sparse/{cameras,images,points3D}.bin (or .txt when there is no .bin) and <input folder>/images/<name>.
 The view index of an image is its position in the images file, as in the reference.
 
 Host side (reference expressions, so the text written from them is byte-identical): the readers, the rotation of each
-quaternion, the intrinsics of all 11 COLMAP camera models (distortion parameters are ignored, as in the reference, with a
-warning: undistort with COLMAP first), the extrinsics and the camera centres -R^T t.
+quaternion, the intrinsics of all 11 COLMAP camera models (without --undistort, distortion parameters are ignored, as in the
+reference, with a warning: undistort first), the extrinsics and the camera centres -R^T t.
 Device side (csrc/pm_colmap.cu through ops.view_scores / ops.depth_ranges): the pairwise view scores, whose cost follows the
 co-visibility of the model instead of the reference's N^2 x obs^2 list scans, and the per-image depth ranges.
+
+--undistort (beyond the reference; INTEGRATION.md "Undistortion (beyond the reference)"): every camera with a non-zero
+distortion parameter becomes the PINHOLE camera of COLMAP's UndistortCamera (border extents on the GPU, ops.undistort_extents;
+scale on the host, ops.undistorted_camera), and each of its images is resampled on the GPU (ops.undistort_image) and written
+in its source's codec (PNG stays PNG, JPEG is written at quality 95 with 4:4:4 chroma, anything else becomes PNG).  Cameras
+without distortion keep the byte-for-byte copy.  cams/ gets the new intrinsics; pair.txt and the depth ranges do not change.
 
 Differences from the reference (INTEGRATION.md "COLMAP interop"): the cosine of the triangulation angle is clamped to [-1, 1]
 and a point on a camera centre contributes 0 (the reference writes nan); ties between scores are ordered by descending view
@@ -351,12 +356,114 @@ def write_scene(output_folder: str, model: SceneModel, depth_ranges: Sequence[Tu
         f.write(pair_text(view_sel))
 
 
-def copy_images(input_folder: str, output_folder: str, images: List[Image]) -> None:
-    """images/<name> -> images/%08d.jpg, byte for byte (reconstruct decodes by content, whatever the extension says)."""
+def copy_images(input_folder: str, output_folder: str, images: List[Image], skip: Sequence[int] = ()) -> None:
+    """images/<name> -> images/%08d.jpg, byte for byte (reconstruct decodes by content, whatever the extension says), except
+    the view indices in `skip`."""
     out_dir = os.path.join(output_folder, "images")
     os.makedirs(out_dir, exist_ok=True)
+    skip = set(skip)
     for i, im in enumerate(images):
-        shutil.copyfile(os.path.join(input_folder, "images", im.name), os.path.join(out_dir, "%08d.jpg" % i))
+        if i not in skip:
+            shutil.copyfile(os.path.join(input_folder, "images", im.name), os.path.join(out_dir, "%08d.jpg" % i))
+
+
+# ---- undistortion -------------------------------------------------------------------------------------------------------------
+
+UNDISTORT_JPEG_QUALITY = 95
+
+
+def undistortion_plan(input_folder: str, cameras: Dict[int, Camera], images: List[Image], blank_pixels: float,
+                      device="cuda:0") -> Dict[int, Camera]:
+    """The PINHOLE camera of every camera with distortion, by camera ID (ops.undistort_extents, ops.undistorted_camera).
+    Raises ValueError, naming the image or camera, for blank_pixels outside [0, 1], an image of such a camera that is not RGB
+    or whose size differs from its camera's, and a camera whose scale is not finite.  Reads image headers only; writes
+    nothing."""
+    from PIL import Image as PILImage
+
+    from . import ops
+
+    if not 0.0 <= blank_pixels <= 1.0:
+        raise ValueError(f"--blank-pixels must be in [0, 1], got {blank_pixels}")
+    distorted = [cameras[c] for c in sorted(cameras) if has_distortion(cameras[c])]
+    if not distorted:
+        return {}
+    ids = {c.id for c in distorted}
+    for i, im in enumerate(images):
+        if im.camera_id not in ids:
+            continue
+        cam = cameras[im.camera_id]
+        with PILImage.open(os.path.join(input_folder, "images", im.name)) as f:
+            size, mode = f.size, f.mode
+        if mode != "RGB":
+            raise ValueError(f"image {i} ({im.name}) is {mode}, not RGB: it cannot be undistorted")
+        if size != (cam.width, cam.height):
+            raise ValueError(f"image {i} ({im.name}) is {size[0]} x {size[1]}, but its camera {cam.id} is {cam.width} x {cam.height}")
+    extents = ops.undistort_extents(distorted, device).cpu().numpy()
+    return {c.id: ops.undistorted_camera(c, e, blank_pixels) for c, e in zip(distorted, extents)}
+
+
+def _decode_pinned(path: str):
+    """(uint8 [H,W,3] pinned host tensor, source format) of an RGB image file."""
+    import torch
+    from PIL import Image as PILImage
+
+    with PILImage.open(path) as f:
+        fmt = f.format
+        arr = np.asarray(f)
+    host = torch.empty(arr.shape, dtype=torch.uint8, pin_memory=True)
+    host.numpy()[...] = arr
+    return host, fmt
+
+
+def _encode(arr: np.ndarray, fmt: str, path: str) -> None:
+    """PNG stays lossless, JPEG is written at quality 95 with 4:4:4 chroma, any other source format as PNG."""
+    from PIL import Image as PILImage
+
+    img = PILImage.fromarray(arr, "RGB")
+    if fmt == "JPEG":
+        img.save(path, format="JPEG", quality=UNDISTORT_JPEG_QUALITY, subsampling=0)
+    else:
+        img.save(path, format="PNG")
+
+
+def undistort_images(input_folder: str, output_folder: str, images: List[Image], cameras: Dict[int, Camera],
+                     plan: Dict[int, Camera], device="cuda:0", workers: Optional[int] = None) -> int:
+    """images/<name> -> images/%08d.jpg for every image whose camera is in `plan`: decode on the host, pinned upload, one warp
+    launch (ops.undistort_image), download, encode in the source's codec.  Decoding and encoding run in a thread pool of
+    `workers` threads with at most `workers` decoded and `workers` warped images in flight, so the host codec overlaps the
+    GPU and memory stays bounded.  -> the number of images written."""
+    import collections
+    from concurrent.futures import ThreadPoolExecutor
+
+    import torch
+
+    from . import ops
+
+    workers = workers or max(1, min(4, os.cpu_count() or 1))
+    out_dir = os.path.join(output_folder, "images")
+    os.makedirs(out_dir, exist_ok=True)
+    todo = [(i, im) for i, im in enumerate(images) if im.camera_id in plan]
+    dev = torch.device(device)
+    with ThreadPoolExecutor(max_workers=workers) as pool, torch.cuda.device(dev):
+        stream = torch.cuda.current_stream(dev)
+        decoded = collections.deque()
+        encoded = collections.deque()
+        nxt = 0
+        for i, im in todo:
+            while nxt < len(todo) and len(decoded) < workers:
+                decoded.append(pool.submit(_decode_pinned, os.path.join(input_folder, "images", todo[nxt][1].name)))
+                nxt += 1
+            src, fmt = decoded.popleft().result()
+            out = ops.undistort_image(src.to(dev, non_blocking=True), cameras[im.camera_id], plan[im.camera_id])
+            host = torch.empty(out.shape, dtype=torch.uint8, pin_memory=True)
+            host.copy_(out, non_blocking=True)
+            stream.synchronize()
+            encoded.append(pool.submit(_encode, host.numpy(), fmt, os.path.join(out_dir, "%08d.jpg" % i)))
+            while len(encoded) > workers:
+                encoded.popleft().result()
+        for f in encoded:
+            f.result()
+    return len(todo)
 
 
 # ---- command ------------------------------------------------------------------------------------------------------------------
@@ -371,6 +478,10 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--theta0", type=float, default=5)
     ap.add_argument("--sigma1", type=float, default=1)
     ap.add_argument("--sigma2", type=float, default=10)
+    ap.add_argument("--undistort", action="store_true",
+                    help="resample the images of every camera with distortion into COLMAP's undistorted PINHOLE camera, on the GPU")
+    ap.add_argument("--blank-pixels", type=float, default=0.0,
+                    help="with --undistort: 0 keeps only valid pixels, 1 keeps the whole view (blank borders); in [0, 1]")
     return ap
 
 
@@ -396,25 +507,39 @@ def convert(args: argparse.Namespace, *, device: str = "cuda:0", log: Callable[.
     check_args(args)
     if not torch.cuda.is_available():
         raise RuntimeError("colmap_input needs a CUDA device (H100); there is no CPU fallback")
+    undistort = getattr(args, "undistort", False)
     t0 = time.perf_counter()
     cameras, images, points = read_model(os.path.join(args.input_folder, "sparse"))
     t1 = time.perf_counter()
-    for cam_id in sorted(cameras):
-        if has_distortion(cameras[cam_id]):
-            log(f"warning: camera {cam_id} ({cameras[cam_id].model}) has distortion parameters, which are ignored; "
-                "run COLMAP's image_undistorter first")
+    if not undistort:
+        for cam_id in sorted(cameras):
+            if has_distortion(cameras[cam_id]):
+                log(f"warning: camera {cam_id} ({cameras[cam_id].model}) has distortion parameters, which are ignored; "
+                    "run COLMAP's image_undistorter first")
     model = prepare(cameras, images, points)
+    plan: Dict[int, Camera] = {}
+    if undistort:
+        with torch.cuda.device(torch.device(device)):
+            plan = undistortion_plan(args.input_folder, cameras, images, args.blank_pixels, device)
+        model = model._replace(intrinsics=[intrinsic_matrix(plan.get(im.camera_id, cameras[im.camera_id])) for im in images])
     t2 = time.perf_counter()
     with torch.cuda.device(torch.device(device)):
         scores, ranges = gpu_scores_and_ranges(model, args.theta0, args.sigma1, args.sigma2, device)
         scores_h, ranges_h = scores.cpu().numpy(), ranges.cpu().tolist()
     t3 = time.perf_counter()
     write_scene(args.output_folder, model, ranges_h, select_views(scores_h, args.num_src_images))
-    copy_images(args.input_folder, args.output_folder, images)
+    warped = [i for i, im in enumerate(images) if im.camera_id in plan]
+    copy_images(args.input_folder, args.output_folder, images, skip=warped)
+    if plan:
+        undistort_images(args.input_folder, args.output_folder, images, cameras, plan, device)
     t4 = time.perf_counter()
     log(f"colmap_input: {len(images)} images, {points.ids.size} points, {model.obs_points.size} observations -> {args.output_folder}")
-    return {"read_seconds": t1 - t0, "prepare_seconds": t2 - t1, "gpu_seconds": t3 - t2, "write_seconds": t4 - t3,
-            "total_seconds": t4 - t0, "images": len(images), "points": int(points.ids.size), "observations": int(model.obs_points.size)}
+    stats = {"read_seconds": t1 - t0, "prepare_seconds": t2 - t1, "gpu_seconds": t3 - t2, "write_seconds": t4 - t3,
+             "total_seconds": t4 - t0, "images": len(images), "points": int(points.ids.size), "observations": int(model.obs_points.size)}
+    if undistort:
+        log(f"colmap_input: undistorted {len(warped)} images of {len(plan)} cameras")
+        stats.update(undistorted_cameras=len(plan), undistorted_images=len(warped))
+    return stats
 
 
 def main(argv: Optional[Sequence[str]] = None) -> int:

@@ -1526,6 +1526,104 @@ def depth_ranges(xyz: Tensor, obs_offsets: Tensor, obs_points: Tensor, extrinsic
     return out
 
 
+def _camera_struct(camera) -> "_native.CameraStruct":
+    """A colmap_input.Camera (model name, width, height, params in COLMAP's order) -> pmb200_camera."""
+    from .colmap_input import CAMERA_MODELS
+
+    ids = {name: (k, n) for k, (name, n) in CAMERA_MODELS.items()}
+    if camera.model not in ids:
+        raise ValueError(f"camera {camera.id}: unknown model {camera.model}")
+    model_id, n = ids[camera.model]
+    if len(camera.params) != n:
+        raise ValueError(f"camera {camera.id}: {camera.model} has {n} parameters, got {len(camera.params)}")
+    s = _native.CameraStruct()
+    s.model, s.width, s.height = model_id, int(camera.width), int(camera.height)
+    for i, v in enumerate(camera.params):
+        s.params[i] = float(v)
+    return s
+
+
+def undistort_extents(cameras: Sequence, device="cuda:0") -> Tensor:
+    """Border extents of COLMAP's UndistortCamera for each camera (include/patchmatch_b200.h, pmb200_undistort_extents):
+    float64 [n,8] on `device` = (left min, left max, right min, right max) of the mapped x, then (top min, top max, bottom
+    min, bottom max) of the mapped y.  cameras: colmap_input.Camera tuples.  One upload and one launch."""
+    import ctypes
+
+    dev = torch.device(device)
+    if dev.type != "cuda":
+        raise RuntimeError(f"undistort_extents: the H100 path needs a CUDA device (got {dev}); there is no CPU fallback")
+    n = len(cameras)
+    host = (_native.CameraStruct * max(n, 1))(*[_camera_struct(c) for c in cameras])
+    staging = torch.empty(max(n, 1) * ctypes.sizeof(_native.CameraStruct), dtype=torch.uint8, device=dev)
+    out = torch.empty((n, 8), dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        rc = _native.lib().pmb200_undistort_extents(host, n, staging.data_ptr(), out.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        _native.check(rc, "undistort_extents")
+        torch.cuda.current_stream(dev).synchronize()  # `host` is pageable and goes out of scope
+    return out
+
+
+UNDISTORT_MIN_SCALE = 0.2
+UNDISTORT_MAX_SCALE = 2.0
+
+
+def undistorted_camera(camera, extents, blank_pixels: float = 0.0):
+    """COLMAP's UndistortCamera with its defaults (min_scale 0.2, max_scale 2.0, no ROI, no max_image_size): the PINHOLE
+    colmap_input.Camera (same id) with fx, fy kept, size sx W x sy H and the principal point scaled with it, from the
+    camera's 8 extents (undistort_extents).  blank_pixels in [0, 1]: 0 keeps only valid pixels, 1 keeps the whole view.
+    ValueError naming the camera when a scale is not finite."""
+    import math
+
+    import numpy as np
+
+    from .colmap_input import Camera, intrinsic_matrix
+
+    if not 0.0 <= blank_pixels <= 1.0:
+        raise ValueError(f"blank_pixels must be in [0, 1], got {blank_pixels}")
+    k = intrinsic_matrix(camera)
+    fx, fy, cx, cy = float(k[0, 0]), float(k[1, 1]), float(k[0, 2]), float(k[1, 2])
+    e = np.asarray(extents.tolist() if hasattr(extents, "tolist") else extents, dtype=np.float64).reshape(8)
+    b = np.float64(blank_pixels)
+    size = []
+    # numpy scalars divide as IEEE doubles (inf / nan, no ZeroDivisionError); Python's min / max pick like std::min / std::max
+    for c, n, (lo_min, lo_max, hi_min, hi_max) in ((np.float64(cx), camera.width, e[0:4]), (np.float64(cy), camera.height, e[4:8])):
+        with np.errstate(all="ignore"):
+            min_s = min(c / (c - lo_min), (n - 0.5 - c) / (hi_max - c))
+            max_s = max(c / (c - lo_max), (n - 0.5 - c) / (hi_min - c))
+            s = float(1.0 / (min_s * b + max_s * (1.0 - b)))
+        if not math.isfinite(s):
+            raise ValueError(f"camera {camera.id} ({camera.model}): the undistorted scale is not finite ({s}); check its "
+                             "distortion parameters")
+        s = max(UNDISTORT_MIN_SCALE, min(s, UNDISTORT_MAX_SCALE))
+        size.append(int(max(1.0, s * n)))
+    w, h = size
+    return Camera(camera.id, "PINHOLE", w, h, [fx, fy, cx * w / camera.width, cy * h / camera.height])
+
+
+def undistort_image(image: Tensor, camera, pinhole) -> Tensor:
+    """Resample an image of the distorted `camera` into the PINHOLE camera `pinhole` (include/patchmatch_b200.h,
+    pmb200_undistort_image).  image uint8 [H,W,3] RGB CUDA with H, W the camera's size; camera, pinhole: colmap_input.Camera
+    (pinhole: the result of undistorted_camera).  -> uint8 [pinhole.height, pinhole.width, 3] on image's device.  One launch."""
+    import ctypes
+
+    if not _on_device(image):
+        raise RuntimeError(f"undistort_image: the H100 path needs a CUDA tensor (got {image.device}); there is no CPU fallback")
+    if image.dtype != torch.uint8 or tuple(image.shape) != (camera.height, camera.width, 3):
+        raise RuntimeError(f"undistort_image: expected uint8 [{camera.height},{camera.width},3] for camera {camera.id}, got "
+                           f"{image.dtype} {tuple(image.shape)}")
+    if pinhole.model != "PINHOLE":
+        raise ValueError(f"undistort_image: the target camera must be PINHOLE, got {pinhole.model}")
+    src = image.contiguous()
+    out = torch.empty((pinhole.height, pinhole.width, 3), dtype=torch.uint8, device=src.device)
+    cam = _camera_struct(camera)
+    kp = (ctypes.c_double * 4)(*[float(v) for v in pinhole.params])
+    with _device_guard(src):
+        rc = _native.lib().pmb200_undistort_image(src.data_ptr(), ctypes.byref(cam), kp, int(pinhole.width), int(pinhole.height),
+                                                  out.data_ptr(), _stream(src))
+    _native.check(rc, "undistort_image")
+    return out
+
+
 DEPTH_LOSS_MAX_MAPS = 16
 DEPTH_METRICS_MAX_THRESHOLDS = 8
 
