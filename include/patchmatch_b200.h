@@ -394,6 +394,51 @@ int pmb200_icp_query(const double *source, int64_t n_source, const double *trans
                      double *moments_out, void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------
+ * ETH3D evaluation (beyond the reference; INTEGRATION.md "ETH3D evaluation (beyond the reference)"), float64 throughout,
+ * every product, sum and difference rounded on its own (no fused multiply-add).  Points are [n,3] float64 device arrays,
+ * n < 2^31, indexed with 64-bit offsets.  No call synchronises the host.
+ *
+ * Free beam.  A laser scan has an origin o and scene-frame points p (the scan's local points through its 4 x 4 matrix M, with
+ * the rounding of pmb200_crop_polygon; o = (M03, M13, M23)).  With r0 = beam_start_radius >= 0 and T = tan_half_angle >= 0
+ * (the tangent of the beam's divergence half-angle, computed once on the host), a = p - o, b = q - o, r = sqrt(a.a) and
+ * t' = a.b, a query q lies in p's free beam iff
+ *     0 < t'  and  t' < a.a  and  |a x b|^2 <= (r0 r + t' T)^2,
+ * dot products evaluated as ((x0 y0 + x1 y1) + x2 y2), cross components as (a1 b2 - a2 b1, a2 b0 - a0 b2, a0 b1 - a1 b0).
+ * A point with a = 0, or with a coordinate that is not finite, is never a beam, and a query with b = 0 or a non-finite b is
+ * in no beam.  Coordinates relative to o must stay below 1e150 in magnitude, so that no product overflows.
+ *
+ * pmb200_beam_index: the angular index of one scan around origin_host (HOST, 3 doubles), written into a caller-owned
+ *   workspace of pmb200_beam_index_workspace_bytes(n_scan) bytes (bytes or a negative PMB200_E*; the query needs a CUDA
+ *   device to size the CUB sort).  Points are binned by the direction of a on an equirectangular grid of 2 R x R bins,
+ *   R = min(1024, ceil(sqrt(n_scan / 64))), and sorted within a bin by range, farthest first.  Sort and three launches.
+ * pmb200_beam_observed: for every query i with mask[i] != 0 (mask may be NULL: every query) and observed[i] == 0, sets
+ *   observed[i] = 1 when q_i lies in the free beam of some point of the scan whose index the workspace holds (the same
+ *   n_scan and origin as the pmb200_beam_index call); other entries are left as they are, so calling it once per scan ORs
+ *   the scans together.  The index culls the points whose beams cannot hold q (by angle around b's direction and by range)
+ *   with margins far above the rounding of the predicate, and evaluates the predicate exactly as above on every other point:
+ *   the result is a brute-force evaluation's, bit for bit.  One launch.
+ *
+ * pmb200_voxel_score: the density-normalised score of one cloud at tolerance tau > 0.  Point i is good when dist[i] <= tau,
+ *   bad when dist[i] > tau and (observed is NULL or observed[i] != 0), otherwise excluded.  Its voxel is floor(x / tau) per
+ *   axis (anchored at the world origin); bounds_host (HOST, min xyz then max xyz) must enclose every point that is not
+ *   excluded, and PMB200_EINVAL is returned, nothing launched, when floor(min / tau) or floor(max / tau) lies outside
+ *   [-2^20, 2^20) on some axis.  The voxel keys are sorted in a caller-owned workspace of
+ *   pmb200_voxel_score_workspace_bytes(n) bytes.  Outputs (device): counts_out [4] int64 = good, bad, excluded points and the
+ *   number of voxels holding a good or bad point; fraction_sum_out [1] = the sum over those voxels of good / (good + bad).
+ *   The sum is per-thread partials in voxel order, a fixed tree per block, then one ordered sum: no atomics, so reruns give
+ *   the same bits. */
+int64_t pmb200_beam_index_workspace_bytes(int64_t n_scan);
+int pmb200_beam_index(const double *scan_points, int64_t n_scan, const double *origin_host, void *workspace, int64_t workspace_bytes,
+                      void *stream);
+int pmb200_beam_observed(const double *queries, int64_t n_queries, const unsigned char *mask, const void *index_workspace,
+                         int64_t n_scan, const double *origin_host, double beam_start_radius, double tan_half_angle,
+                         unsigned char *observed, void *stream);
+int64_t pmb200_voxel_score_workspace_bytes(int64_t n);
+int pmb200_voxel_score(const double *points, const double *dist, int64_t n, double tau, const unsigned char *observed,
+                       const double *bounds_host, int64_t *counts_out, double *fraction_sum_out, void *workspace,
+                       int64_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------
  * COLMAP sparse model -> scene folder (reference colmap_input.py:318-373; INTEGRATION.md "COLMAP interop"), float64 throughout.
  * The model: points xyz [n_points,3]; observations in CSR form, obs_offsets [n_images+1] (int32, obs_offsets[0] = 0) and
  * obs_points [n_obs] (int32 dense point indices in each image's own 2D-point order, -1 entries removed); camera centres

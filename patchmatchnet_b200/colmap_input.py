@@ -5,7 +5,9 @@ colmap_input.py, with view selection and depth ranges on the GPU.
     python -m patchmatchnet_b200.reconstruct --input-folder project --checkpoint-path model.pt
 
 Input: <input folder>/sparse/{cameras,images,points3D}.bin (or .txt when there is no .bin) and <input folder>/images/<name>.
-The view index of an image is its position in the images file, as in the reference.
+The view index of an image is its position in the images file, as in the reference.  --sparse-folder NAME reads the model
+from <input folder>/NAME instead; an image name may hold subfolders.  So an ETH3D training scene (dslr_calibration_undistorted/
+and images/dslr_images_undistorted/*.JPG) converts in place with --sparse-folder dslr_calibration_undistorted.
 
 Host side (reference expressions, so the text written from them is byte-identical): the readers, the rotation of each
 quaternion, the intrinsics of all 11 COLMAP camera models (without --undistort, distortion parameters are ignored, as in the
@@ -478,6 +480,8 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--theta0", type=float, default=5)
     ap.add_argument("--sigma1", type=float, default=1)
     ap.add_argument("--sigma2", type=float, default=10)
+    ap.add_argument("--sparse-folder", type=str, default="sparse",
+                    help="folder under the input folder that holds the sparse model (ETH3D: dslr_calibration_undistorted)")
     ap.add_argument("--undistort", action="store_true",
                     help="resample the images of every camera with distortion into COLMAP's undistorted PINHOLE camera, on the GPU")
     ap.add_argument("--blank-pixels", type=float, default=0.0,
@@ -509,7 +513,7 @@ def convert(args: argparse.Namespace, *, device: str = "cuda:0", log: Callable[.
         raise RuntimeError("colmap_input needs a CUDA device (H100); there is no CPU fallback")
     undistort = getattr(args, "undistort", False)
     t0 = time.perf_counter()
-    cameras, images, points = read_model(os.path.join(args.input_folder, "sparse"))
+    cameras, images, points = read_model(os.path.join(args.input_folder, getattr(args, "sparse_folder", "sparse")))
     t1 = time.perf_counter()
     if not undistort:
         for cam_id in sorted(cameras):

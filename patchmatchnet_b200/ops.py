@@ -1354,6 +1354,82 @@ def voxel_downsample(points: Tensor, voxel_size: float) -> Tensor:
     return out[: int(count.item())]
 
 
+def beam_observed(queries: Tensor, scan_points: Tensor, origin, beam_start_radius: float, tan_half_angle: float,
+                  observed: Optional[Tensor] = None, mask: Optional[Tensor] = None) -> Tensor:
+    """Which queries lie in the free beam of some point of one laser scan (include/patchmatch_b200.h, pmb200_beam_observed):
+    the scan's angular index around `origin` (3 numbers) is built, then every query under `mask` (bool or uint8 [n], None =
+    all) that `observed` does not already mark is tested.  queries [n,3] and scan_points [m,3] float64 CUDA, scan points in
+    the scene frame; beam_start_radius r0 and tan_half_angle T >= 0.  -> observed uint8 [n], updated in place when given (so
+    one call per scan ORs the scans).  Exact: the result equals a brute-force evaluation of the predicate, bit for bit."""
+    import ctypes
+
+    q = _points_arg(queries, "beam_observed (queries)")
+    s = _points_arg(scan_points, "beam_observed (scan points)")
+    if s.device != q.device:
+        raise RuntimeError("beam_observed: queries and scan points must be on the same device")
+    o = [float(v) for v in origin]
+    if len(o) != 3:
+        raise RuntimeError("beam_observed: origin must have 3 coordinates")
+    n = q.shape[0]
+    if observed is None:
+        observed = torch.zeros(n, dtype=torch.uint8, device=q.device)
+    elif observed.dtype != torch.uint8 or observed.shape != (n,) or observed.device != q.device or not observed.is_contiguous():
+        raise RuntimeError("beam_observed: observed must be a contiguous uint8 [n] tensor on the queries' device")
+    m = None
+    if mask is not None:
+        if mask.shape != (n,) or mask.device != q.device or mask.dtype not in (torch.bool, torch.uint8):
+            raise RuntimeError("beam_observed: mask must be a bool or uint8 [n] tensor on the queries' device")
+        m = mask.to(torch.uint8).contiguous()
+    lib = _native.lib()
+    ws = _workspace(lib.pmb200_beam_index_workspace_bytes(s.shape[0]), "beam_index_workspace_bytes", q.device)
+    o_host = (ctypes.c_double * 3)(*o)
+    with _device_guard(q):
+        rc = lib.pmb200_beam_index(s.data_ptr(), s.shape[0], o_host, ws.data_ptr(), ws.numel(), _stream(q))
+        _native.check(rc, "beam_index")
+        rc = lib.pmb200_beam_observed(q.data_ptr(), n, m.data_ptr() if m is not None else None, ws.data_ptr(), s.shape[0], o_host,
+                                      float(beam_start_radius), float(tan_half_angle), observed.data_ptr(), _stream(q))
+    _native.check(rc, "beam_observed")
+    return observed
+
+
+def voxel_score(points: Tensor, dist: Tensor, tau: float, observed: Optional[Tensor] = None) -> dict:
+    """Density-normalised score of a cloud at tolerance tau (include/patchmatch_b200.h, pmb200_voxel_score): a point is good
+    when dist <= tau, bad when dist > tau and `observed` marks it (every such point when observed is None), else excluded;
+    voxels of edge tau anchored at the world origin.  points float64 [n,3], dist float64 [n], observed uint8/bool [n] or None,
+    all CUDA.  -> {"good", "bad", "excluded", "voxels", "fraction_sum"}: the counts and the sum over voxels holding a good or
+    bad point of good / (good + bad).  Two host reads: the counted points' bounds and the result."""
+    import ctypes
+
+    pts = _points_arg(points, "voxel_score")
+    n = pts.shape[0]
+    if dist.dtype != torch.float64 or dist.shape != (n,) or dist.device != pts.device:
+        raise RuntimeError("voxel_score: dist must be a float64 [n] tensor on the points' device")
+    d = dist.contiguous()
+    obs = None
+    if observed is not None:
+        if observed.shape != (n,) or observed.device != pts.device or observed.dtype not in (torch.bool, torch.uint8):
+            raise RuntimeError("voxel_score: observed must be a bool or uint8 [n] tensor on the points' device")
+        obs = observed.to(torch.uint8).contiguous()
+    counted = (d <= tau) | (obs.bool() if obs is not None else True)
+    inf = torch.tensor(float("inf"), dtype=torch.float64, device=pts.device)
+    lo = torch.where(counted[:, None], pts, inf).amin(0) if n else inf.expand(3)
+    hi = torch.where(counted[:, None], pts, -inf).amax(0) if n else -inf.expand(3)
+    b = torch.cat([lo, hi]).cpu().tolist()
+    if not b[0] <= b[3]:  # nothing counts: any valid box
+        b = [0.0] * 6
+    counts = torch.empty(4, dtype=torch.int64, device=pts.device)
+    fsum = torch.empty(1, dtype=torch.float64, device=pts.device)
+    lib = _native.lib()
+    ws = _workspace(lib.pmb200_voxel_score_workspace_bytes(n), "voxel_score_workspace_bytes", pts.device)
+    with _device_guard(pts):
+        rc = lib.pmb200_voxel_score(pts.data_ptr(), d.data_ptr(), n, float(tau), obs.data_ptr() if obs is not None else None,
+                                    (ctypes.c_double * 6)(*b), counts.data_ptr(), fsum.data_ptr(), ws.data_ptr(), ws.numel(),
+                                    _stream(pts))
+    _native.check(rc, "voxel_score")
+    c = counts.cpu().tolist()
+    return {"good": c[0], "bad": c[1], "excluded": c[2], "voxels": c[3], "fraction_sum": float(fsum.cpu())}
+
+
 def umeyama_from_moments(m) -> "np.ndarray":
     """The similarity (with scaling) that best maps the correspondences' source points onto their targets (Umeyama 1991, the
     estimate of Eigen::umeyama with scaling), from the 18 sums of pmb200_icp_query taken relative to an origin o:
