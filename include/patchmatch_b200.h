@@ -328,6 +328,56 @@ int pmb200_tsdf_mesh_write(const uint64_t *block_keys, int64_t n_blocks, double 
                            int *faces_out, void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------
+ * Rendering of point clouds and triangle meshes (beyond the reference, whose only viewer is an Open3D window; INTEGRATION.md
+ * "Rendering (beyond the reference)").  This project's own definition, float32 throughout, every product, sum and
+ * difference rounded on its own (no fused multiply-add); `/` and sqrt are IEEE.  Reruns give the same bits.
+ *
+ * Camera.  P_host (HOST, 12 floats) = K [R | t] composed in float64 and rounded to float32, row-major 3 x 4; centre_host
+ * (HOST, 3 floats) = the camera centre -R^T t, rounded likewise.  A world point (x, y, z) maps to
+ * u' = ((P00 x + P01 y) + P02 z) + P03, likewise v' (row 1) and z (row 2); u = u' / z, v = v' / z.  Pixel (x, y) is sampled
+ * at (x, y), the convention of the cams files.  near_z > 0 (finite); anything with z <= near_z, or z, u or v not finite, is
+ * skipped.
+ * Z-buffer.  One uint64 per pixel, cleared to all ones; a fragment of primitive i at depth z writes
+ * atomicMin((float_bits(z) << 32) | i): the nearest fragment wins, an exact depth tie goes to the lower index.
+ * Points.  Point i covers the s x s square (s = point_size, odd, 1..15) centred on (rint(u), rint(v)) (round half to even),
+ * clipped to the image; its depth is z.
+ * Triangles.  A face is skipped when a vertex index is outside 0..n_vertices-1, when a vertex has z <= near_z, |u| or
+ * |v| > 2^22 or a value that is not finite (no clipping), or when A = (u1 - u0)(v2 - v0) - (v1 - v0)(u2 - u0) is 0.  When
+ * A < 0 vertices 1 and 2 swap and A = -A.  The box is ceil(min u) .. floor(max u) (and v), clipped to the image.  Edge i
+ * (opposite vertex i) runs a -> b = 1 -> 2, 2 -> 0, 0 -> 1; its function at pixel p is
+ * e = (b.u - a.u)(p.v - a.v) - (b.v - a.v)(p.u - a.u), evaluated from the edge's lower endpoint (smaller v, then smaller u)
+ * and negated when that endpoint is b, so the two faces of a shared edge get the same magnitude.  p is covered when every
+ * e_i > 0, or e_i == 0 on a top-left edge (b.v - a.v < 0, or == 0 and b.u - a.u > 0): faces sharing an edge cover each
+ * pixel on it once.  b_i = e_i / A; z = 1 / ((b0 / z0 + b1 / z1) + b2 / z2), the fragment kept when 0 < z < inf.  No
+ * back-face culling.  Perspective-correct weights w_i = (b_i / z_i) z.
+ * Resolve.  A pixel no fragment reached gets the background (background_host, HOST, 3 bytes) and depth 0.  Otherwise the
+ * depth is the winner's z and the colour c per channel is the point's colour, or ((w0 c0 + w1 c1) + w2 c2) over the face's
+ * vertex colours; 160 where rgb is NULL.  With shade != 0 c is multiplied by f = 0.25 + 0.75 |n . d| / (|n| |d|), d = centre -
+ * X: for a point X is the point and n its normal (normals NULL: f = 1); for a face X = ((w0 X0 + w1 X1) + w2 X2) and n is the
+ * face normal (X1 - X0) x (X2 - X0) in the face's own vertex order, components (a1 b2 - a2 b1, a2 b0 - a0 b2, a0 b1 - a1 b0),
+ * dot products ((x0 y0 + x1 y1) + x2 y2).  f = 1 when |n| |d| is not finite and > 0.  Channel = clamp(rint(c f), 0, 255).
+ *
+ * pmb200_render_points: xyz [n,3] float32, rgb [n,3] uint8 or NULL, normals [n,3] float32 or NULL, n < 2^32; out_rgb
+ *   [H,W,3] uint8, out_depth [H,W] float32; workspace of pmb200_render_points_workspace_bytes(W, H) bytes (the z-buffer).
+ *   A clear, one splat launch (a thread per point) and one resolve launch.
+ * pmb200_render_mesh: vertices xyz [nv,3] float32, rgb [nv,3] uint8 or NULL; faces int32 [nf,3]; nv, nf < 2^31; workspace
+ *   of pmb200_render_mesh_workspace_bytes(W, H, nv, nf) bytes.  The vertices are projected once; one thread per face
+ *   rasterises faces whose clipped box is at most 16 x 16 pixels and appends larger ones to a list (atomic counter) that a
+ *   second launch rasterises one face per CTA; then the resolve.
+ * 1 <= W, H <= 16384.  PMB200_EINVAL, nothing launched, for a null pointer, a bad size or point size, a camera that is not
+ * finite, or near_z not finite and > 0.  Enqueue only; no host synchronisation. */
+int64_t pmb200_render_points_workspace_bytes(int width, int height);
+int pmb200_render_points(const float *xyz, const unsigned char *rgb, const float *normals, int64_t n, const float *P_host,
+                         const float *centre_host, int width, int height, int point_size, float near_z, int shade,
+                         const unsigned char *background_host, unsigned char *out_rgb, float *out_depth, void *workspace,
+                         int64_t workspace_bytes, void *stream);
+int64_t pmb200_render_mesh_workspace_bytes(int width, int height, int64_t n_vertices, int64_t n_faces);
+int pmb200_render_mesh(const float *xyz, const unsigned char *rgb, int64_t n_vertices, const int *faces, int64_t n_faces,
+                       const float *P_host, const float *centre_host, int width, int height, float near_z, int shade,
+                       const unsigned char *background_host, unsigned char *out_rgb, float *out_depth, void *workspace,
+                       int64_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------
  * DTU point-cloud evaluation (reference evaluations/dtu/*.m; INTEGRATION.md "DTU evaluation"), float64 throughout.
  * Both calls sort the cloud into a fine / coarse cell hash held in a caller-owned device workspace of
  * *_workspace_bytes(n) bytes (O(n), whatever the extent of the cloud; the size query returns bytes or a negative PMB200_E*).

@@ -346,3 +346,142 @@ def read_ply_points(path: str) -> np.ndarray:
         for a, axis in enumerate(("x", "y", "z")):
             out[:, a] = data[axis]
         return out
+
+
+_PLY_FACE_LISTS = ("vertex_indices", "vertex_index")
+
+
+def _ply_header(f, path: str):
+    """(format, [(element name, count, [(property name, numpy type or ("list", count type, item type))])]) of an open PLY."""
+    if f.readline().strip() != b"ply":
+        raise ValueError(f"{path}: not a PLY file")
+    fmt, elements, current = None, [], None
+    while True:
+        line = f.readline()
+        if not line:
+            raise ValueError(f"{path}: PLY header has no end_header")
+        words = line.decode("ascii", "replace").split()
+        if not words or words[0] in ("comment", "obj_info"):
+            continue
+        if words[0] == "end_header":
+            break
+        if words[0] == "format":
+            fmt = words[1]
+        elif words[0] == "element":
+            current = (words[1], int(words[2]), [])
+            elements.append(current)
+        elif words[0] == "property":
+            if current is None:
+                raise ValueError(f"{path}: PLY property outside an element")
+            types = words[2:4] if words[1] == "list" else words[1:2]
+            for t in types:
+                if t not in _PLY_TYPES:
+                    raise ValueError(f"{path}: unknown PLY property type {t!r}")
+            if words[1] == "list":
+                current[2].append((words[4], ("list", _PLY_TYPES[words[2]], _PLY_TYPES[words[3]])))
+            else:
+                current[2].append((words[2], _PLY_TYPES[words[1]]))
+    if fmt not in ("binary_little_endian", "ascii"):
+        raise ValueError(f"{path}: PLY format {fmt!r} is not supported (binary_little_endian or ascii)")
+    return fmt, elements
+
+
+def _ply_colour(v: np.ndarray) -> np.ndarray:
+    """One colour channel -> uint8: integer types clamped to 0..255, floating types as 255 * v rounded and clamped."""
+    if v.dtype.kind == "f":
+        v = np.rint(v.astype(np.float64) * 255.0)
+    return np.clip(v, 0, 255).astype(np.uint8)
+
+
+def read_ply(path: str):
+    """A point cloud or triangle mesh from a PLY file -> (xyz float32 [n,3], colours uint8 [n,3] or None, normals float32
+    [n,3] or None, faces int32 [nf,3] or None).
+
+    Reads `binary_little_endian` and `ascii` files: this project's fused.ply (plain and oriented), mesh.ply and the coloured
+    class clouds of the evaluations, and ground-truth scans such as DTU's stl*.ply.  The `vertex` element comes first with
+    scalar properties x, y, z and optionally red, green, blue (uchar as they are; other integer types clamped to 0..255,
+    floating types in [0,1] scaled by 255 and rounded) and nx, ny, nz.  Double coordinates are narrowed to float32, which
+    rounds ground-truth scans to float32.  A `face` element holds one list property `vertex_indices` (or `vertex_index`)
+    with an integer count type (uchar, int, uint, ...).  Other elements after the vertices are skipped.  ValueError on a
+    polygon that is not a triangle, a vertex index out of range, and on every malformed file read_ply_points rejects."""
+    with open(path, "rb") as f:
+        fmt, elements = _ply_header(f, path)
+        if not elements or elements[0][0] != "vertex":
+            for name, count, _ in elements:
+                if name == "vertex":
+                    break
+                if count:
+                    raise ValueError(f"{path}: PLY element {name!r} precedes the vertex element")
+            else:
+                raise ValueError(f"{path}: PLY file has no vertex element")
+            elements = [e for e in elements if e[1] or e[0] == "vertex"]
+            elements = elements[[e[0] for e in elements].index("vertex"):]
+        ascii_rows = None
+        if fmt == "ascii":
+            ascii_rows = iter(f.read().decode("ascii", "replace").splitlines())
+        xyz = colours = normals = faces = None
+        for name, count, props in elements:
+            lists = [p for p, t in props if isinstance(t, tuple)]
+            if name == "vertex":
+                if lists:
+                    raise ValueError(f"{path}: list properties in the vertex element are not supported")
+                names = [p for p, _ in props]
+                if not all(a in names for a in ("x", "y", "z")):
+                    raise ValueError(f"{path}: PLY vertex element lacks x, y or z")
+                data = _ply_scalar_rows(f, ascii_rows, props, count, path)
+                xyz = np.stack([data[a] for a in ("x", "y", "z")], axis=1).astype(np.float32)
+                if all(a in names for a in ("red", "green", "blue")):
+                    colours = np.stack([_ply_colour(data[a]) for a in ("red", "green", "blue")], axis=1)
+                if all(a in names for a in ("nx", "ny", "nz")):
+                    normals = np.stack([data[a] for a in ("nx", "ny", "nz")], axis=1).astype(np.float32)
+            elif name == "face":
+                if len(props) != 1 or props[0][0] not in _PLY_FACE_LISTS:
+                    raise ValueError(f"{path}: the face element must hold one list property vertex_indices (or vertex_index)")
+                _, count_t, item_t = props[0][1]
+                if count_t[0] not in "iu" or item_t[0] not in "iu":
+                    raise ValueError(f"{path}: face lists need integer count and index types")
+                faces = _ply_triangles(f, ascii_rows, count_t, item_t, count, path)
+                if faces.size and (faces.min() < 0 or faces.max() >= xyz.shape[0]):
+                    raise ValueError(f"{path}: a face refers to a vertex outside 0..{xyz.shape[0] - 1}")
+                faces = faces.astype(np.int32)
+            else:
+                if lists:
+                    raise ValueError(f"{path}: list properties in the PLY element {name!r} are not supported")
+                _ply_scalar_rows(f, ascii_rows, props, count, path)
+        return xyz, colours, normals, faces
+
+
+def _ply_scalar_rows(f, ascii_rows, props, count: int, path: str) -> np.ndarray:
+    dtype = np.dtype([(p, "<" + t) for p, t in props])
+    if ascii_rows is None:
+        data = np.fromfile(f, dtype=dtype, count=count)
+        if data.shape[0] != count:
+            raise ValueError(f"{path}: PLY body holds {data.shape[0]} rows, header says {count}")
+        return data
+    lines = [next(ascii_rows, "") for _ in range(count)]
+    vals = np.array(" ".join(lines).split(), dtype=np.float64)
+    if vals.size != count * len(props) or any(len(line.split()) != len(props) for line in lines):
+        raise ValueError(f"{path}: PLY body does not hold {count} rows of {len(props)} values")
+    out = np.zeros(count, dtype=dtype)
+    for k, (p, _) in enumerate(props):
+        out[p] = vals[k::len(props)]
+    return out
+
+
+def _ply_triangles(f, ascii_rows, count_t: str, item_t: str, count: int, path: str) -> np.ndarray:
+    if ascii_rows is None:
+        rows = np.fromfile(f, dtype=np.dtype([("n", "<" + count_t), ("v", "<" + item_t, (3,))]), count=count)
+        bad = np.flatnonzero(rows["n"] != 3)
+        if bad.size:  # rows up to the first non-triangle are aligned, so its count is read where it is
+            raise ValueError(f"{path}: face {int(bad[0])} has {int(rows['n'][bad[0]])} vertices; only triangles are supported")
+        if rows.shape[0] != count:
+            raise ValueError(f"{path}: PLY body holds {rows.shape[0]} faces, header says {count}")
+        v = rows["v"].astype(np.int64)
+    else:
+        v = np.zeros((count, 3), dtype=np.int64)
+        for i in range(count):
+            words = next(ascii_rows, "").split()
+            if not words or int(words[0]) != 3 or len(words) != 4:
+                raise ValueError(f"{path}: face {i} is not a triangle ({' '.join(words) or 'missing'})")
+            v[i] = [int(w) for w in words[1:]]
+    return v

@@ -1219,6 +1219,117 @@ def tsdf_mesh(points: Tensor, depths: Sequence[Tensor], images: Sequence[Tensor]
     return tsdf_extract(keys, tsdf, weight, colour, voxel_size, min_weight)
 
 
+def render_camera_arrays(P):
+    """A 3 x 4 float64 camera K [R | t] -> (P rounded to float32, row-major [12]; camera centre -M^-1 p4 computed in float64
+    and rounded to float32 [3]), the HOST values pmb200_render_points / _mesh take.  ValueError for a camera that is not
+    finite or whose left 3 x 3 is singular."""
+    import numpy as np
+
+    P64 = np.asarray(P.detach().cpu().numpy() if isinstance(P, Tensor) else P, dtype=np.float64)
+    if P64.shape != (3, 4) or not np.isfinite(P64).all():
+        raise ValueError(f"render: the camera must be a finite 3 x 4 matrix K [R | t], got shape {P64.shape}")
+    try:
+        centre = -np.linalg.solve(P64[:, :3], P64[:, 3])
+    except np.linalg.LinAlgError:
+        raise ValueError("render: the camera's left 3 x 3 is singular") from None
+    return P64.astype(np.float32).ravel(), centre.astype(np.float32)
+
+
+def _render_args(P, width: int, height: int, near: float, background, what: str):
+    import ctypes
+    import math
+
+    for name, v in (("width", width), ("height", height)):
+        if isinstance(v, bool) or not isinstance(v, int) or not 1 <= v <= 16384:
+            raise ValueError(f"{what}: {name} must be an int in 1..16384, got {v!r}")
+    if not (isinstance(near, (int, float)) and math.isfinite(near) and near > 0):
+        raise ValueError(f"{what}: near must be a positive finite number, got {near!r}")
+    bg = [int(c) for c in background]
+    if len(bg) != 3 or any(not 0 <= c <= 255 for c in bg):
+        raise ValueError(f"{what}: background must be three values in 0..255, got {background!r}")
+    p, c = render_camera_arrays(P)
+    return (ctypes.c_float * 12)(*p.tolist()), (ctypes.c_float * 3)(*c.tolist()), (ctypes.c_ubyte * 3)(*bg)
+
+
+def _render_attr(t: Optional[Tensor], n: int, dtype, device, name: str, what: str) -> Optional[Tensor]:
+    if t is None:
+        return None
+    if not isinstance(t, Tensor) or not _on_device(t) or t.dtype != dtype or tuple(t.shape) != (n, 3) or t.device != device:
+        raise ValueError(f"{what}: {name} must be a CUDA {dtype} [{n},3] tensor on the vertices' device")
+    return t.contiguous()
+
+
+def _render_xyz(xyz: Tensor, what: str) -> Tensor:
+    if not isinstance(xyz, Tensor) or not _on_device(xyz) or xyz.dtype != torch.float32 or xyz.dim() != 2 or xyz.shape[1] != 3:
+        raise ValueError(f"{what}: xyz must be a CUDA float32 [n,3] tensor (there is no CPU fallback)")
+    return xyz.contiguous()
+
+
+def render_points(xyz: Tensor, rgb: Optional[Tensor], normals: Optional[Tensor], P, width: int, height: int, near: float,
+                  point_size: int = 1, shade: bool = False, background=(255, 255, 255)) -> Tuple[Tensor, Tensor]:
+    """Z-buffered square splats of a point cloud (pmb200_render_points; definition in include/patchmatch_b200.h).  xyz CUDA
+    float32 [n,3]; rgb uint8 [n,3] or None (grey); normals float32 [n,3] or None (used by shade=True); P the 3 x 4 float64
+    camera K [R | t] (pixel (x, y) sampled at (x, y)); near > 0 the depth at or below which points are skipped; point_size
+    odd 1..15.  -> (rgb uint8 [H,W,3], depth float32 [H,W], 0 where nothing was drawn) on the device.  Bit-identical to
+    tests/render_oracle.py and from run to run.  ValueError before any launch on bad arguments."""
+    what = "render_points"
+    pts = _render_xyz(xyz, what)
+    n = pts.shape[0]
+    if n >= 2 ** 32:
+        raise ValueError(f"{what}: at most 2^32 - 1 points, got {n}")
+    if isinstance(point_size, bool) or not isinstance(point_size, int) or not (1 <= point_size <= 15 and point_size % 2 == 1):
+        raise ValueError(f"{what}: point_size must be an odd int in 1..15, got {point_size!r}")
+    col = _render_attr(rgb, n, torch.uint8, pts.device, "rgb", what)
+    nrm = _render_attr(normals, n, torch.float32, pts.device, "normals", what)
+    p_host, c_host, bg = _render_args(P, width, height, near, background, what)
+    lib = _native.lib()
+    ws = _workspace(lib.pmb200_render_points_workspace_bytes(width, height), "render_points_workspace_bytes", pts.device)
+    out_rgb = torch.empty((height, width, 3), dtype=torch.uint8, device=pts.device)
+    out_depth = torch.empty((height, width), dtype=torch.float32, device=pts.device)
+    with _device_guard(pts):
+        rc = lib.pmb200_render_points(pts.data_ptr(), None if col is None else col.data_ptr(), None if nrm is None else nrm.data_ptr(),
+                                      n, p_host, c_host, width, height, point_size, float(near), 1 if shade else 0, bg,
+                                      out_rgb.data_ptr(), out_depth.data_ptr(), ws.data_ptr(), ws.numel(), _stream(pts))
+    _native.check(rc, what)
+    return out_rgb, out_depth
+
+
+def render_mesh(xyz: Tensor, rgb: Optional[Tensor], faces: Tensor, P, width: int, height: int, near: float, shade: bool = False,
+                background=(255, 255, 255), check_faces: bool = True) -> Tuple[Tensor, Tensor]:
+    """Z-buffered rasterisation of a triangle mesh with perspective-correct colours and flat headlight shading
+    (pmb200_render_mesh; definition in include/patchmatch_b200.h).  xyz CUDA float32 [nv,3]; rgb uint8 [nv,3] or None (grey);
+    faces int32 [nf,3]; P, near, shade and background as for render_points.  -> (rgb uint8 [H,W,3], depth float32 [H,W]) on
+    the device.  A face with a vertex at or behind `near` is dropped, not clipped.  With check_faces (the default) a face
+    index outside 0..nv-1 raises ValueError (one host read); without it such faces are skipped by the kernel."""
+    what = "render_mesh"
+    pts = _render_xyz(xyz, what)
+    nv = pts.shape[0]
+    if not isinstance(faces, Tensor) or not _on_device(faces) or faces.dtype != torch.int32 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError(f"{what}: faces must be a CUDA int32 [nf,3] tensor")
+    if faces.device != pts.device:
+        raise ValueError(f"{what}: faces must be on the vertices' device")
+    fc = faces.contiguous()
+    nf = fc.shape[0]
+    if nv >= 2 ** 31 or nf >= 2 ** 31:
+        raise ValueError(f"{what}: at most 2^31 - 1 vertices and faces, got {nv} and {nf}")
+    if check_faces and nf:
+        lo, hi = (int(v) for v in torch.aminmax(fc))
+        if lo < 0 or hi >= nv:
+            raise ValueError(f"{what}: a face refers to a vertex outside 0..{nv - 1}")
+    col = _render_attr(rgb, nv, torch.uint8, pts.device, "rgb", what)
+    p_host, c_host, bg = _render_args(P, width, height, near, background, what)
+    lib = _native.lib()
+    ws = _workspace(lib.pmb200_render_mesh_workspace_bytes(width, height, nv, nf), "render_mesh_workspace_bytes", pts.device)
+    out_rgb = torch.empty((height, width, 3), dtype=torch.uint8, device=pts.device)
+    out_depth = torch.empty((height, width), dtype=torch.float32, device=pts.device)
+    with _device_guard(pts):
+        rc = lib.pmb200_render_mesh(pts.data_ptr(), None if col is None else col.data_ptr(), nv, fc.data_ptr(), nf, p_host, c_host,
+                                    width, height, float(near), 1 if shade else 0, bg, out_rgb.data_ptr(), out_depth.data_ptr(),
+                                    ws.data_ptr(), ws.numel(), _stream(pts))
+    _native.check(rc, what)
+    return out_rgb, out_depth
+
+
 def split_ply_body(body: Tensor):
     """uint8 [n,15] vertex records -> (vertices float32 [n,3], colours uint8 [n,3]) on the CPU."""
     b = body.detach().cpu().contiguous()
