@@ -53,6 +53,11 @@ const char *pmb200_last_error(void);
  * The reference has no counterpart (its launch shapes are ATen's). */
 int pmb200_set_tuning(const char *key, int value);
 
+/* Measurement aid: which fused warp+correlation kernel the calling thread's last pmb200_warp_corr* call launched: 4 (fourth
+ * generation), 3 (third generation; the *_views entry points launch its per-view form) or 0 (the generic kernel of other
+ * channel / group counts); -1 before any such call and after a call that failed its checks. */
+int pmb200_last_warp_corr_kernel(void);
+
 /* ------------------------------------------------------------------------------------
  * K-D5: channels-last convolution on Hopper's warpgroup tensor cores (wgmma / TMA), fp32-accurate (3xTF32 split).
  * Replaces, for the FLOP-bound layers in the fp32-accurate mode, the nn.Conv2d calls of reference models/net.py:9-70 (FeatureNet

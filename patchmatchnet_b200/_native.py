@@ -132,6 +132,7 @@ _SIGNATURES = {
     "pmb200_abi_version": (c_int, []),
     "pmb200_last_error": (c_char_p, []),
     "pmb200_set_tuning": (c_int, [c_char_p, c_int]),
+    "pmb200_last_warp_corr_kernel": (c_int, []),
     "pmb200_relative_projection": (c_int, [c_void_p, c_int64, _PPF, c_int64, c_int, c_int, c_void_p, c_void_p]),
     "pmb200_pack_nhwc": (c_int, [_PPF, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "pmb200_photometric_confidence": (c_int, [c_void_p] * 2 + [c_int] * 6 + [c_void_p]),

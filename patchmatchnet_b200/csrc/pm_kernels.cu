@@ -2,12 +2,12 @@
 // (backward kernels: pm_backward.cu; per-element formulas shared with the CPU formula tests: pm_math.cuh).
 //
 // Kernel map (DESIGN.md has the byte/flop budgets and the measured numbers):
-//   wc4::warp_corr4_kernel<C,G,EPI,NW,MINB>  K-A, fourth generation (default, pm_warpcorr4.cuh): homography warp + bilinear
+//   wc4::warp_corr4_kernel<C,G,EPI,NW,MINB>  K-A, fourth generation (ka_gen = 4, pm_warpcorr4.cuh): homography warp + bilinear
 //                                  gather + group-wise correlation + view-weighted aggregation + (eval) 1x1x1 head epilogue
 //                                  as a persistent producer/consumer pipeline over TMA-staged shared-memory windows
 //                                  pmb200_warp_corr / _score / _view_weights
-//   warp_corr3_kernel<C,G,EPI,DC,PIPE,MINB>  K-A, third generation: register/L1 gather; taken for shapes generation 4
-//                                  declines and selectable for A/B measurements (pmb200_set_tuning("ka_gen", 3));
+//   warp_corr3_kernel<C,G,EPI,DC,PIPE,MINB>  K-A, third generation: register/L1 gather; the default (kTuneDefaults:
+//                                  ka_gen = 3), and taken for shapes generation 4 declines when ka_gen = 4 asks for it;
 //                                  warp_corr_generic_kernel: any C % G == 0
 //   warp_corr3_views_kernel / warp_corr_generic_views_kernel   the same bodies with a size per source view (ragged pack)
 //                                  pmb200_warp_corr_views / _score_views / _view_weights_views
@@ -38,6 +38,7 @@
 namespace {
 
 thread_local char g_err[256] = "";
+thread_local int g_last_ka = -1;  // pmb200_last_warp_corr_kernel
 
 int fail(int code, const char *msg) {
     snprintf(g_err, sizeof(g_err), "%s", msg);
@@ -1352,8 +1353,12 @@ bool launch_wc4(const WarpCorrParams &p, const MlpParams &m, float *sims_out, cu
 // K-A dispatch: generation 4 unless the knob or the shape says otherwise
 template <int C, int G, int EPI>
 void launch_ka(const WarpCorrParams &p, const MlpParams &m, float *sims_out, cudaStream_t st) {
-    if (tune(kTuneKaGen) != 3 && launch_wc4<C, G, EPI>(p, m, sims_out, st)) return;
+    if (tune(kTuneKaGen) != 3 && launch_wc4<C, G, EPI>(p, m, sims_out, st)) {
+        g_last_ka = 4;
+        return;
+    }
     launch_wc3_auto<C, G, EPI>(p, m, sims_out, st);
+    g_last_ka = 3;
 }
 
 }  // namespace
@@ -1390,6 +1395,8 @@ int pmb200_set_tuning(const char *key, int value) {
 }
 
 const char *pmb200_last_error(void) { return g_err; }
+
+int pmb200_last_warp_corr_kernel(void) { return g_last_ka; }
 
 int pmb200_relative_projection(const float *ref_proj, int64_t ref_batch_stride, const float *const *src_projs_host,
                                int64_t src_batch_stride, int V, int B, float *rt_out, void *stream) {
@@ -1456,6 +1463,7 @@ int pmb200_upsample2x_add_nhwc(const float *x_nhwc, const float *y_nhwc, const f
 int pmb200_warp_corr(const float *ref_nhwc, const float *src_nhwc, const float *rt, const float *depth,
                      const float *view_weights, float *out, int V, int B, int C, int G, int H, int W, int Hs,
                      int Ws, int D, void *stream) {
+    g_last_ka = -1;
     if (!ref_nhwc || !src_nhwc || !rt || !depth || !out) return fail(PMB200_EINVAL, "warp_corr: null pointer");
     if (V < 1 || V > PMB200_MAX_VIEWS || B < 1 || B > 65535 || H < 1 || W < 1 || Hs < 1 || Ws < 1 || D < 1)
         return fail(PMB200_EINVAL, "warp_corr: bad size");
@@ -1485,6 +1493,7 @@ int pmb200_warp_corr(const float *ref_nhwc, const float *src_nhwc, const float *
     else {
         const size_t total = (size_t)B * D * HW;
         warp_corr_generic_kernel<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(p, C, G);
+        g_last_ka = 0;
     }
 #undef PMB200_LAUNCH_WC
     return launch_status("warp_corr");
@@ -1495,6 +1504,7 @@ int warp_corr_head(const char *what, int epi, const float *ref_nhwc, const float
                    const float *depth, const float *view_weights, const pmb200_mlp *head_host, float *out,
                    float *sims_out, int out_stride, int V, int B, int C, int G, int H, int W, int Hs, int Ws, int D,
                    void *stream) {
+    g_last_ka = -1;
     if (!ref_nhwc || !src_nhwc || !rt || !depth || !out || !head_host) return fail(PMB200_EINVAL, "warp_corr head: null pointer");
     if (epi == kEpiScore && !view_weights) return fail(PMB200_EINVAL, "warp_corr_score: view_weights missing");
     if (V < 1 || V > PMB200_MAX_VIEWS || B < 1 || B > 65535 || H < 1 || W < 1 || Hs < 1 || Ws < 1 || D < 1)
@@ -1552,6 +1562,7 @@ int warp_corr_views(const char *what, int epi, const float *ref_nhwc, const floa
                     const float *rt, const float *depth, const float *view_weights, const pmb200_mlp *head_host, float *out,
                     float *sims_out, int out_stride, int V, int B, int C, int G, int H, int W, int D, void *stream) {
     const bool head = epi == kEpiScore || epi == kEpiViewW;
+    g_last_ka = -1;
     if (!ref_nhwc || !src_flat || !views_host || !rt || !depth || !out || (head && !head_host))
         return fail(PMB200_EINVAL, "warp_corr views: null pointer");
     if (epi == kEpiScore && !view_weights) return fail(PMB200_EINVAL, "warp_corr_score_views: view_weights missing");
@@ -1596,6 +1607,7 @@ int warp_corr_views(const char *what, int epi, const float *ref_nhwc, const floa
         else if (epi == kEpiScore) launch_wc3_views<CC, GG, kEpiScore>(p, vt, m, nullptr, st);     \
         else launch_wc3_views<CC, GG, kEpiViewW>(p, vt, m, sims_out, st);                          \
     } while (0)
+    g_last_ka = fast ? 3 : 0;
     if (C == 64 && G == 8) PMB200_LAUNCH_WV(64, 8);
     else if (C == 32 && G == 8) PMB200_LAUNCH_WV(32, 8);
     else if (C == 16 && G == 4) PMB200_LAUNCH_WV(16, 4);

@@ -73,6 +73,13 @@ def set_tuning(key: str, value: int = 0) -> None:
     _native.check(_native.lib().pmb200_set_tuning(key.encode(), int(value)), "set_tuning")
 
 
+def last_warp_corr_kernel() -> int:
+    """Measurement aid: the fused warp+correlation kernel the calling thread's last K-A call launched (warp_corr,
+    warp_corr_score, warp_corr_view_weights, with a ViewPack too): 4 or 3 (its generation), 0 (the generic kernel), -1
+    before any such call.  pmb200_last_warp_corr_kernel."""
+    return int(_native.lib().pmb200_last_warp_corr_kernel())
+
+
 def relative_projection(ref_proj: Tensor, src_projs: Sequence[Tensor]) -> Tensor:
     """[V,B,12] rotation/translation of src_proj @ inv(ref_proj); reference module.py:148-150."""
     B = ref_proj.shape[0]

@@ -28,6 +28,15 @@ def plane_depth(K, E, H, W, n, d0):
     return (num / den).reshape(H, W).astype(np.float32)
 
 
+def source_pose(i):
+    """[R | t] (3x4) of source camera i >= 1.  Sources past the fourth repeat the first four baselines (their principal
+    points and corruptions still differ), so that every source of a scene with many sources overlaps the reference."""
+    k = (i - 1) % 4 + 1
+    sgn = 1.0 if k % 2 else -1.0
+    return np.concatenate([_rot_y(math.radians(2.0 * k) * sgn) @ _rot_x(math.radians(0.7 * k)),
+                           np.array([[40.0 * sgn * k], [-15.0 * (k % 3)], [5.0 * k]])], axis=1)
+
+
 def make_scene(H=96, W=128, n_src=4, seed=0):
     rng = np.random.default_rng(seed)
     K = np.array([[1.2 * W, 0, W / 2], [0, 1.2 * W, H / 2], [0, 0, 1]], dtype=np.float32)
@@ -38,9 +47,7 @@ def make_scene(H=96, W=128, n_src=4, seed=0):
     for i in range(n_src + 1):
         E = np.eye(4, dtype=np.float64)
         if i:
-            sgn = 1.0 if i % 2 else -1.0
-            E[:3, :3] = _rot_y(math.radians(2.0 * i) * sgn) @ _rot_x(math.radians(0.7 * i))
-            E[:3, 3] = [40.0 * sgn * i, -15.0 * (i % 3), 5.0 * i]
+            E[:3, :] = source_pose(i)
         Ki = K.copy()
         Ki[0, 2] += 1.5 * i
         cams.append((Ki, E.astype(np.float32)))

@@ -40,21 +40,19 @@ def make_net_inputs(sizes=NET_SIZES, seed: int = NET_SEED) -> Dict[str, object]:
             "depth_max": torch.full((1,), synthetic.DEPTH_MAX), "rand48": rand48}
 
 
-def make_geo_scene(seed: int = 0) -> Dict[str, object]:
+def make_geo_scene(seed: int = 0, ref_hw: Tuple[int, int] = GEO_REF_HW, src_hw: Sequence[Tuple[int, int]] = GEO_SRC_HW) -> Dict[str, object]:
     """geo_cases.make_scene with a size per source view: the plane rendered into each source camera at that camera's own
     size (principal point at its centre), then corrupted the same way."""
     rng = np.random.default_rng(seed)
-    H, W = GEO_REF_HW
+    H, W = ref_hw
     n = np.array([0.12, -0.08, 1.0])
     n = n / np.linalg.norm(n)
     d0 = 600.0
-    cams, sizes = [], [GEO_REF_HW] + GEO_SRC_HW
+    cams, sizes = [], [tuple(ref_hw)] + list(src_hw)
     for i, (h, w) in enumerate(sizes):
         E = np.eye(4, dtype=np.float64)
         if i:
-            sgn = 1.0 if i % 2 else -1.0
-            E[:3, :3] = geo_cases._rot_y(math.radians(2.0 * i) * sgn) @ geo_cases._rot_x(math.radians(0.7 * i))
-            E[:3, 3] = [40.0 * sgn * i, -15.0 * (i % 3), 5.0 * i]
+            E[:3, :] = geo_cases.source_pose(i)
         f = 1.2 * W  # one focal length in pixels of the reference's size: views differ in extent, not in scale
         K = np.array([[f, 0, w / 2 + 1.5 * i], [0, f, h / 2], [0, 0, 1]], dtype=np.float32)
         cams.append((K, E.astype(np.float32)))

@@ -140,6 +140,15 @@ KA_SHAPES = [
     (16, 4, 5, 6, 5, 1, 1),  # single view, odd hypothesis count
     (64, 8, 3, 3, 1, 1, 2),  # single hypothesis, tiny map
 ]
+# Source-view counts the evaluation configurations run (DTU 5, ETH3D / Tanks and Temples 7, a 10-source pair.txt) and the
+# limit PMB200_MAX_VIEWS = 16.  K-A4's producer gives lane v view v's footprint box, and its consumers read view v's
+# weight from s_vw[v * PIX + pixel]; with 4 consumer warps (PIX = 32) V = 16 fills all 16 view-weight registers of a lane.
+KA_VIEW_SHAPES = [
+    (32, 8, 6, 9, 10, 1, 6),  # 6 views: a multiple of the 2- and 3-slot rings, so every item starts in the same slot
+    (64, 8, 5, 7, 9, 1, 9),  # 9 views: more footprint boxes than a tile row has pixels (8), odd against the 2- and 4-slot rings
+    (16, 4, 6, 11, 8, 1, 16),  # the view limit: every view-weight register of a lane carries a view
+]
+KA_SHAPES += KA_VIEW_SHAPES
 
 
 def _configs(C):
@@ -183,7 +192,7 @@ def _random_head(cls, G, seed):
     return head.eval()
 
 
-@pytest.mark.parametrize("C,G,H,W,D,B,V", KA_SHAPES[:4])
+@pytest.mark.parametrize("C,G,H,W,D,B,V", KA_SHAPES[:4] + KA_VIEW_SHAPES)
 def test_emulated_fused_heads_match_unfused(emu, C, G, H, W, D, B, V):
     from patchmatchnet_b200.patchmatch import PixelwiseNet, SimilarityNet
 
@@ -274,7 +283,7 @@ def test_emulated_warp_corr4_equals_generation_3(emu):
         assert maxabs(g4, g3) <= 1e-5 * max(1.0, float(g3.abs().max()))
 
 
-@pytest.mark.parametrize("C,G,H,W,D,B,V", KA_SHAPES[:4])
+@pytest.mark.parametrize("C,G,H,W,D,B,V", KA_SHAPES[:4] + KA_VIEW_SHAPES)
 def test_emulated_warp_corr4_fused_heads_match_unfused(emu, C, G, H, W, D, B, V):
     from patchmatchnet_b200.patchmatch import PixelwiseNet, SimilarityNet
 

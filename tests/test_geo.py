@@ -15,7 +15,7 @@ import pytest
 import torch
 
 from oracle import geo_oracle as go
-from tests import geo_cases
+from tests import geo_cases, multisize_cases
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "geo_case.npz")
 REFERENCE_VECTORS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "geo_reference.npz")
@@ -155,8 +155,17 @@ def test_kernel_pixel_function_matches_the_oracle(hostmath, H, W, n_src, seed):
     _compare(got, (want[0], want[1], want[2], w3))
 
 
+# A 1920x1080 reference with 7 sources of mixed orientation and one smaller camera: the per-view filter
+# (pmb200_geometric_filter_views) with more sources than the multi-size scene of tests/test_gpu_multisize.py has
+MIXED_SOURCES = ((1080, 1920), (1920, 1080), (1080, 1920), (720, 1280), (1920, 1080), (1080, 1920), (1920, 1080))
+
+
 def _oracle_case(H, W, n_src, seed):
-    sc = geo_cases.make_scene(seed=seed, H=H, W=W, n_src=n_src)
+    """n_src: the number of sources (all of the reference's size), or their (height, width) sizes"""
+    if isinstance(n_src, int):
+        sc = geo_cases.make_scene(seed=seed, H=H, W=W, n_src=n_src)
+    else:
+        sc = multisize_cases.make_geo_scene(seed=seed, ref_hw=(H, W), src_hw=n_src)
     if H * W < 8000:  # degenerate inputs: zero depth, NaN confidence
         sc["ref_depth"][0, :5] = 0.0
         sc["confidence"][1, :3] = np.nan
@@ -170,8 +179,11 @@ def _run_gpu(sc):
 
     dev = "cuda:0"
     cams = ops.compose_filter_cameras(sc["ref_K"], sc["ref_E"], list(sc["src_Ks"]), list(sc["src_Es"]))
-    out = ops.geometric_filter(torch.from_numpy(sc["ref_depth"]).to(dev), torch.from_numpy(sc["confidence"]).to(dev),
-                               torch.from_numpy(np.stack(list(sc["src_depths"]))).to(dev), cams)
+    if len({d.shape for d in sc["src_depths"]}) == 1:
+        srcs = torch.from_numpy(np.stack(list(sc["src_depths"]))).to(dev)
+    else:  # sources of different sizes: the per-view filter
+        srcs = [torch.from_numpy(d).to(dev) for d in sc["src_depths"]]
+    out = ops.geometric_filter(torch.from_numpy(sc["ref_depth"]).to(dev), torch.from_numpy(sc["confidence"]).to(dev), srcs, cams)
     torch.cuda.synchronize()
     return [o.cpu().numpy() for o in out]
 
@@ -196,8 +208,11 @@ def test_gpu_filter_matches_the_reference_fixture(golden):
     _compare(_run_gpu(sc), (golden["photo_mask"], golden["geo_mask_sum"], golden["final_mask"], golden["depth_est_averaged"]))
 
 
+# the image sizes and source counts reconstruct filters at: an ETH3D high-res view (2688x1792) against the
+# 10 sources of a usual pair.txt, a Tanks and Temples view against 7 (the oracle takes ~20 s and ~6 s on one CPU core)
 @pytest.mark.gpu
-@pytest.mark.parametrize("H,W,n_src,seed", [(72, 100, 3, 3), (33, 47, 1, 5), (512, 640, 4, 7)])
+@pytest.mark.parametrize("H,W,n_src,seed", [(72, 100, 3, 3), (33, 47, 1, 5), (512, 640, 4, 7), (1792, 2688, 10, 11), (1080, 1920, 7, 13),
+                                             pytest.param(1080, 1920, MIXED_SOURCES, 17, id="1080-1920-mixed7-17")])
 def test_gpu_filter_matches_the_oracle(H, W, n_src, seed):
     sc, want = _oracle_case(H, W, n_src, seed)
     got = _run_gpu(sc)
@@ -278,7 +293,7 @@ def test_save_ply_layout(tmp_path):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("H,W,n_src,seed", [(72, 100, 3, 3), (33, 47, 1, 5), (512, 640, 4, 7)])
+@pytest.mark.parametrize("H,W,n_src,seed", [(72, 100, 3, 3), (33, 47, 1, 5), (512, 640, 4, 7), (1792, 2688, 10, 11), (1080, 1920, 7, 13)])
 def test_gpu_fusion_matches_the_oracle(H, W, n_src, seed):
     from patchmatchnet_b200 import ops
 

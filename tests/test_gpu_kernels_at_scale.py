@@ -75,14 +75,15 @@ def stage_iterations(stage):
     return out
 
 
-def shape_table():
+def shape_table(views=VIEWS, V=N_SRC):
+    """Every iteration of every stage of each (name, B, image height, image width) in `views`, with V source views."""
     rows = []
-    for view, B, Hi, Wi in VIEWS:
+    for view, B, Hi, Wi in views:
         for stage in (3, 2, 1):
             c = stage_config(stage)
             for it, itc in enumerate(stage_iterations(stage), 1):
                 rows.append(dict(name=f"{view}/s{stage}/it{it}", B=B, H=Hi // STAGE_DOWN[stage], W=Wi // STAGE_DOWN[stage],
-                                 V=N_SRC, C=c["C"], G=c["G"], dil=c["dil"], K=c["K"], scale=c["scale"], **itc))
+                                 V=V, C=c["C"], G=c["G"], dil=c["dil"], K=c["K"], scale=c["scale"], **itc))
     return rows
 
 
@@ -383,14 +384,15 @@ def random_head(cls, G, seed):
     return head.eval()
 
 
-def ka_case(r, seed, Hs=None, Ws=None):
+def ka_case(r, seed, Hs=None, Ws=None, sizes=None):
     """Inputs of one K-A call at the shape of table row r: smooth features, the synthetic rig's relative projections at
-    this stage (computed in float64, rounded once), sorted hypotheses over the depth range, view weights."""
+    this stage (computed in float64, rounded once), sorted hypotheses over the depth range, view weights.  sizes: one
+    (Hs, Ws) per source view (a list of source maps of different sizes instead of one stacked tensor)."""
     g = torch.Generator().manual_seed(seed)
     B, V, C, H, W, D = r["B"], r["V"], r["C"], r["H"], r["W"], r["D"]
     Hs, Ws = Hs or H, Ws or W
     ref = smooth(g, B, C, H=H, W=W)
-    srcs = smooth(g, V, B, C, H=Hs, W=Ws)
+    srcs = smooth(g, V, B, C, H=Hs, W=Ws) if sizes is None else [smooth(g, B, C, H=h, W=w) for h, w in sizes]
     down = {64: 8, 32: 4, 16: 2}[C]
     Kc, Ec = synthetic.make_cameras(B, V + 1, H * down, W * down)
     ref_proj, src_projs = synthetic.stage_projections(Kc.double(), Ec.double(), {8: 3, 4: 2, 2: 1}[down])
@@ -406,26 +408,29 @@ def ka_references(case, G):
     dev = DEV
     ref64, depth64 = case["ref"].to(dev, F64), case["depth"].to(dev, F64)
     sims, bounds = [], []
-    for v in range(case["src"].shape[0]):
+    for v in range(len(case["src"])):
         s, b = ka_reference(ref64, case["src"][v].to(dev, F64), case["rt"][v].to(dev, F64), depth64, G)
         sims.append(s)
         bounds.append(b)
     return sims, bounds
 
 
-def ka_device(case):
+def ka_device(case, stack=True):
     nhwc = lambda x: x.permute(0, 2, 3, 1).contiguous()
-    return (nhwc(case["ref"].to(DEV)), torch.stack([nhwc(s.to(DEV)) for s in case["src"]]), case["rt"].to(DEV),
+    return (nhwc(case["ref"].to(DEV)), torch.stack([nhwc(s.to(DEV)) for s in case["src"]]) if stack else None, case["rt"].to(DEV),
             case["depth"].to(DEV), case["vw"].to(DEV))
 
 
 SIM_DIMS = ("view", "b", "g", "d", "y", "x")
 
 
-def check_ka_ops(tag, r, case, sims, bounds, heads, knobs=None, fp32_oracle=True):
-    """Every K-A entry point at one shape against the float64 references."""
+def check_ka_ops(tag, r, case, sims, bounds, heads, knobs=None, fp32_oracle=True, src=None):
+    """Every K-A entry point at one shape against the float64 references.  src: the sources as the kernels take them, in
+    place of the stacked case["src"] (an ops.ViewPack for sources of different sizes)."""
     G, V = r["G"], r["V"]
-    ref_n, src_n, rt, depth, vw = ka_device(case)
+    ref_n, src_n, rt, depth, vw = ka_device(case, stack=src is None)
+    if src is not None:
+        src_n = src
     sim_head, pw_head = heads
     vw64 = case["vw"].to(DEV, F64)
     want = torch.stack(sims)
@@ -554,19 +559,30 @@ def test_warp_corr_edges():
     assert float(got[3, :, :, 9].abs().max()) > 0.1  # Z = 1.1e-3, tx = 0: samples the pixel itself
 
 
-def ka_kernel_args(fn):
-    """Run fn under the CUDA profiler -> [(generation, [template arguments])] of the K-A kernels it launched."""
+def ka_kernel_args(fn, sessions=5):
+    """Run fn under the CUDA profiler -> [(generation, [template arguments])] of the K-A kernels it launched.
+
+    A profiler session now and then comes back without any device activity at all (its CUPTI records are lost, not the
+    launches: fn launches kernels every time and raises when a launch fails).  Such a session says nothing about which
+    kernels ran, so fn is profiled again, at most `sessions` times; a session with device activity is taken as it is."""
+    from torch.autograd import DeviceType
     from torch.profiler import ProfilerActivity, profile
 
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    out = []
-    for e in prof.events():
-        m = re.search(r"warp_corr([34])_kernel<([^>]*)>", e.name)
-        if m:
-            out.append((int(m.group(1)), [a.strip() for a in m.group(2).split(",")]))
-    return out
+    for _ in range(sessions):
+        torch.cuda.synchronize()  # nothing launched before the session runs inside it
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        names = [e.name for e in prof.events() if e.device_type == DeviceType.CUDA]
+        if names:
+            out = []
+            for name in names:
+                m = re.search(r"warp_corr([34])_kernel<([^>]*)>", name)
+                if m:
+                    out.append((int(m.group(1)), [a.strip() for a in m.group(2).split(",")]))
+            return out
+        print("[profiler] a session recorded no device activity; profiling again")
+    raise AssertionError(f"{sessions} profiler sessions recorded no device activity")
 
 
 def knob_took_effect(knobs, launched):
@@ -685,9 +701,13 @@ OC_ROWS = ["1600x1200/s3/it1", "1200x1600/s2/it1", "1600x1200/s1/it1", "320x256/
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", OC_ROWS)
 def test_offset_corr_at_scale(name):
+    check_offset_corr(name, row(name))
+
+
+def check_offset_corr(name, r):
+    """K-A' and its fused head at the shape of row r against the float64 references."""
     from patchmatchnet_b200.patchmatch import FeatureWeightNet
 
-    r = row(name)
     B, C, G, K, dil, H, W = r["B"], r["C"], r["G"], r["K"], r["dil"], r["H"], r["W"]
     g = torch.Generator().manual_seed(H + K)
     ref = smooth(g, B, C, H=H, W=W)
@@ -698,7 +718,16 @@ def test_offset_corr_at_scale(name):
         got = ops.offset_corr(ref_n, off.to(DEV), G, K, dil)
         assert_within(f"{name} offset_corr", got, want, bnd, ("b", "g", "k", "y", "x"))
         grid32 = pm_oracle.sampling_grid(pm_oracle.neighbour_table("evaluation", K, dil), off.to(DEV).view(B, 2 * K, H * W), H, W)
-        assert_tight(f"{name} offset_corr", got, pm_oracle._FeatureWeightHead(K, G).to(DEV).neighbour_correlation(ref.to(DEV), grid32))
+        want32 = pm_oracle._FeatureWeightHead(K, G).to(DEV).neighbour_correlation(ref.to(DEV), grid32)
+        if max(H, W) <= 800:
+            assert_tight(f"{name} offset_corr", got, want32)
+        else:
+            # the fp32 oracle's own position rounding grows with the map width (its normalised grid, as in
+            # check_ka_ops); past the 800 px of the widest rows above it exceeds the 2e-5 check by itself (2.1e-4 at
+            # 1344 px, with the kernel within 0.12 of its float64 bound): its distance from float64 is printed instead
+            print(f"[fp32 oracle] {name} offset_corr: fp32 oracle vs float64 max-abs {float((want32.double() - want).abs().max()):.3e}, "
+                  f"kernel vs float64 max-abs {float((got.double() - want).abs().max()):.3e}")
+        del want32
         head = random_head(lambda gg: FeatureWeightNet(K, gg), G, 9).to(DEV)
         o, do = head_reference(head_layers(head), want, bnd)
         s, ds = sigmoid_bound(o, do)
@@ -761,7 +790,11 @@ def kc_inputs(r, g):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", KC_ROWS)
 def test_init_propagate_at_scale(name):
-    r = row(name)
+    check_init_propagate(name, row(name))
+
+
+def check_init_propagate(name, r):
+    """K-C (hypotheses, xnorm, the interleaved xs buffer) at the shape of row r against the float64 references."""
     print(f"[plan] {name}: K-C kernel {kc_kernel(r['Ns'], r['Kp'])}")
     B, H, W, Ns, Kp = r["B"], r["H"], r["W"], r["Ns"], r["Kp"]
     g = torch.Generator().manual_seed(H + Ns + Kp)
@@ -882,7 +915,12 @@ def check_kb(tag, r, inputs, refs, sms):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", KB_ROWS)
 def test_adaptive_eval_at_scale(name):
-    r = row(name)
+    check_adaptive_eval(name, row(name))
+
+
+def check_adaptive_eval(name, r):
+    """K-B in its three input forms at the shape of row r against the float64 references, and against the fp32 oracle
+    on maps up to 200 px."""
     g = torch.Generator().manual_seed(r["H"] + r["D"])
     inputs = kb_inputs(r, g)
     score0, depth, off, fw, dmin, dmax = inputs
