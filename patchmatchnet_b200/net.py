@@ -74,14 +74,6 @@ class _FoldCache:
 
 _FUSED_CONV_RELU = hasattr(torch, "cudnn_convolution_relu")
 
-def _native_convs(x: Tensor) -> bool:
-    """Eval mode on CUDA: every conv of the shell (FeatureNet, Refinement) runs through the native channels-last
-    tensor-core conv (csrc/pm_conv.cu, ops.conv2d_nhwc) instead of cuDNN, unless ops.NATIVE_CONVS is False
-    (PMB200_NATIVE_CONVS=0), which keeps the folded cuDNN calls -- bench.py uses that for an A/B line."""
-    from . import ops
-
-    return ops.NATIVE_CONVS and _fast(x) and not torch.is_grad_enabled()
-
 
 def ops_prefers(conv: nn.Conv2d) -> bool:
     from . import ops
@@ -91,8 +83,8 @@ def ops_prefers(conv: nn.Conv2d) -> bool:
 
 # ---- TorchScript -------------------------------------------------------------------------------------------------------------
 # A scripted network runs the eval-mode launch sequence of the eager one through `torch.ops.pmb200.*` (csrc/torch_binding.cpp).
-# What eager decides per call from module-level switches (ops.NATIVE_CONVS, ops.conv_precision(), ops.conv_tc5_mode, ...) and
-# the folded / packed weights it caches are frozen when the module goes to eval mode (eval(), or load_state_dict in eval mode):
+# What eager decides per call (LIBRARY_FAST_PATH, ops.conv_precision(), ops.conv_form, ...) and the folded / packed weights it
+# caches are frozen when the module goes to eval mode (eval(), or load_state_dict in eval mode):
 # the call the reference makes right before torch.jit.script (train.py:52-53).  Frozen values are plain HOST tensors and Python
 # scalars, never state-dict entries; the operators keep device copies of the host tensors (one upload per device).
 # Native conv forms: 0 = the mma.sync kernel (conv2d_nhwc, fragment-ordered filter), 1 = the wgmma tap form, 2 = the wgmma
@@ -107,18 +99,6 @@ def _freezing() -> bool:
 
 def _host(t: Tensor) -> Tensor:
     return t.detach().float().cpu()
-
-
-def _freeze_native(weight: Tensor, stride: int, transposed: bool = False) -> Tuple[int, Tensor]:
-    """(form, host filter image) of the native conv eager runs for this filter."""
-    from . import ops
-
-    cout, cin, ks = weight.shape[0], weight.shape[1], weight.shape[2]
-    mode = "" if transposed else ops.conv_tc5_mode(cin, cout, ks, stride)
-    with torch.no_grad():
-        if mode:
-            return (2 if mode == "halo" else 1), _host(ops.pack_conv_filter_tc5_for(weight, mode))
-        return 0, _host(ops.pack_conv_filter(weight, ops.conv_precision(), transposed=transposed))
 
 
 def _script_conv(x: Tensor, form: int, filt: Tensor, bias: Optional[Tensor], cout: int, ks: int, stride: int, pad: int, dil: int,
@@ -147,28 +127,43 @@ def _nonempty(t: Tensor) -> Optional[Tensor]:
     return t
 
 
-class _PackedConv:
-    """Fragment-ordered filter (+ bias) of a plain nn.Conv2d, cached until the weights change or move."""
+class PackedConv:
+    """The native form of one nn.Conv2d (ops.conv_form), its filter packed for that form (ops.pack_conv_filter_for) with an
+    eval-mode BatchNorm folded in when given, and its bias; cached per form and precision until a source tensor is modified or
+    moved.  The modules are passed at each call, so that module replicas sharing the object use their own weights."""
 
     def __init__(self) -> None:
         self._cache = _FoldCache()
 
-    def __call__(self, conv: nn.Conv2d, x: Tensor, relu: bool = False, with_bias: bool = True) -> Tensor:
+    def packed(self, conv: nn.Conv2d, bn: Optional[nn.BatchNorm2d] = None) -> Tuple[int, Tensor, Optional[Tensor]]:
+        """(form, filter image, bias or None)."""
         from . import ops
 
-        srcs = [conv.weight] + ([conv.bias] if conv.bias is not None else [])
-        mode = ops.conv_tc5_mode(conv.in_channels, conv.out_channels, conv.kernel_size[0], conv.stride[0])
-        if mode:
-            frag, bias = self._cache.get(
-                srcs, lambda: (ops.pack_conv_filter_tc5_for(conv.weight, mode), None if conv.bias is None else conv.bias.detach().clone()),
-                key="tc5" + mode)
-            return ops.conv2d_tc5(x, frag, bias if with_bias else None, conv.out_channels, conv.kernel_size[0], conv.stride[0],
-                                  conv.padding[0], conv.dilation[0], relu=relu, halo=mode == "halo")
+        form = ops.conv_form(conv.in_channels, conv.out_channels, conv.kernel_size[0], conv.stride[0])
         prec = ops.conv_precision()
-        frag, bias = self._cache.get(
-            srcs, lambda: (ops.pack_conv_filter(conv.weight, prec), None if conv.bias is None else conv.bias.detach().clone()), key=prec)
-        return ops.conv2d_nhwc(x, frag, bias if with_bias else None, conv.out_channels, conv.kernel_size[0], conv.stride[0],
-                               conv.padding[0], conv.dilation[0], relu=relu)
+        if bn is None:
+            srcs = [conv.weight] + ([conv.bias] if conv.bias is not None else [])
+        else:
+            srcs = [conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var]
+
+        def make():
+            w, b = (conv.weight, conv.bias) if bn is None else _fold_bn(conv.weight, bn)
+            return ops.pack_conv_filter_for(w, form, prec), None if b is None else b.detach().clone()
+
+        filt, bias = self._cache.get(srcs, make, key=(form, prec))
+        return form, filt, bias
+
+    def __call__(self, conv: nn.Conv2d, x: Tensor, bn: Optional[nn.BatchNorm2d] = None, relu: bool = False, with_bias: bool = True,
+                 out: Optional[Tensor] = None, out_channel_offset: int = 0) -> Tensor:
+        """The conv on the native kernel of its form (what _script_conv runs in the scripted forward)."""
+        from . import ops
+
+        form, filt, bias = self.packed(conv, bn)
+        args = (x, filt, bias if with_bias else None, conv.out_channels, conv.kernel_size[0], conv.stride[0], conv.padding[0],
+                conv.dilation[0])
+        if form == 0:
+            return ops.conv2d_nhwc(*args, relu=relu, out=out, out_channel_offset=out_channel_offset)
+        return ops.conv2d_tc5(*args, relu=relu, out=out, out_channel_offset=out_channel_offset, halo=form == 2)
 
 
 class _ConvBnReLU2d(nn.Module):
@@ -183,9 +178,8 @@ class _ConvBnReLU2d(nn.Module):
         super().__init__()
         self.conv = nn.Conv2d(cin, cout, k, stride=stride, padding=pad, bias=False)
         self.bn = nn.BatchNorm2d(cout)
-        self._cache = _FoldCache()
-        self._frag_cache = _FoldCache()
-        self._tc5_cache = _FoldCache()
+        self._cache = _FoldCache()  # folded weights for ATen's convolution
+        self._packed = PackedConv()
         self._k, self._stride, self._pad, self._cout = k, stride, pad, cout
         # scripted forward, frozen by freeze_script (see "TorchScript" above)
         self._s_mode = 0
@@ -201,18 +195,14 @@ class _ConvBnReLU2d(nn.Module):
         """Freeze the layer's eval-mode decisions and folded weights for the scripted forward."""
         from . import ops
 
-        native = ops.NATIVE_CONVS and ops_prefers(self.conv)
-        self._s_mode = 0 if not LIBRARY_FAST_PATH else (2 if native else 1)
+        self._s_mode = 0 if not LIBRARY_FAST_PATH else (2 if ops_prefers(self.conv) else 1)
         self._s_precision = ops.conv_precision()
-        with torch.no_grad():
-            if ops.NATIVE_CONVS:  # Refinement's native tail calls the native form whatever the layer prefers
-                mode = ops.conv_tc5_mode(self.conv.in_channels, self.conv.out_channels, self._k, self._stride)
-                frag, b = self.folded_tc5(mode) if mode else self.folded_frag()
-                self._s_form = (2 if mode == "halo" else 1) if mode else 0
-                self._s_native_w, self._s_native_b = _host(frag), _host(b)
-            if self._s_mode == 1:
-                w, b = self.folded()
-                self._s_lib_w, self._s_lib_b = _host(w), _host(b)
+        # Refinement's native tail calls the native form whatever the layer prefers
+        self._s_form, frag, b = self._packed.packed(self.conv, self.bn)
+        self._s_native_w, self._s_native_b = _host(frag), _host(b)
+        if self._s_mode == 1:
+            w, b = self.folded()
+            self._s_lib_w, self._s_lib_b = _host(w), _host(b)
 
     def native_script(self, x: Tensor, out: Optional[Tensor] = None, out_channel_offset: int = 0) -> Tensor:
         return _script_conv(x, self._s_form, self._s_native_w, self._s_native_b, self._cout, self._k, self._stride, self._pad, 1, True,
@@ -230,46 +220,8 @@ class _ConvBnReLU2d(nn.Module):
             return F.relu_(F.conv2d(x, w, b, s, p, [1, 1]))
         return F.relu(self.bn(self.conv(x)), inplace=True)
 
-    def folded_frag(self):
-        """(fragment-ordered folded filter, folded bias) for the native conv."""
-        from . import ops
-
-        bn = self.bn
-        srcs = [self.conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var]
-
-        prec = ops.conv_precision()
-
-        def make():
-            w, b = _fold_bn(self.conv.weight, bn)
-            return ops.pack_conv_filter(w, prec), b.contiguous()
-
-        return self._frag_cache.get(srcs, make, key=prec)
-
-    def folded_tc5(self, mode: str):
-        """(filter image for the wgmma conv in the given form, folded bias)."""
-        from . import ops
-
-        bn = self.bn
-        srcs = [self.conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var]
-
-        def make():
-            w, b = _fold_bn(self.conv.weight, bn)
-            return ops.pack_conv_filter_tc5_for(w, mode), b.contiguous()
-
-        return self._tc5_cache.get(srcs, make, key=mode)
-
     def native(self, x: Tensor, out: Tensor = None, out_channel_offset: int = 0) -> Tensor:
-        from . import ops
-
-        c = self.conv
-        mode = ops.conv_tc5_mode(c.in_channels, c.out_channels, c.kernel_size[0], c.stride[0])
-        if mode:
-            frag, b = self.folded_tc5(mode)
-            return ops.conv2d_tc5(x, frag, b, c.out_channels, c.kernel_size[0], c.stride[0], c.padding[0], c.dilation[0],
-                                  relu=True, out=out, out_channel_offset=out_channel_offset, halo=mode == "halo")
-        frag, b = self.folded_frag()
-        return ops.conv2d_nhwc(x, frag, b, c.out_channels, c.kernel_size[0], c.stride[0], c.padding[0], c.dilation[0],
-                               relu=True, out=out, out_channel_offset=out_channel_offset)
+        return self._packed(self.conv, x, self.bn, relu=True, out=out, out_channel_offset=out_channel_offset)
 
     def folded(self):
         bn = self.bn
@@ -291,10 +243,9 @@ class _ConvBnReLU2d(nn.Module):
         if self.training or not _fast(x):
             return F.relu(self.bn(self.conv(x)), inplace=True)
         c = self.conv
-        if _native_convs(x) and ops_prefers(c):
+        if ops_prefers(c):
             return self.native(x)
         w, b = self.folded()
-        c = self.conv
         if _FUSED_CONV_RELU:
             return torch.cudnn_convolution_relu(x, w, b, c.stride, c.padding, c.dilation, 1)
         return F.relu_(F.conv2d(x, w, b, c.stride, c.padding, c.dilation))
@@ -319,16 +270,15 @@ class FeatureNet(nn.Module):
         self.inner2 = nn.Conv2d(16, 64, 1, bias=True)
         self.output2 = nn.Conv2d(64, 32, 1, bias=False)
         self.output3 = nn.Conv2d(64, 16, 1, bias=False)
-        self._packed = {n: _PackedConv() for n in ("output1", "inner1", "inner2", "output2", "output3")}
+        self._packed = {n: PackedConv() for n in ("output1", "inner1", "inner2", "output2", "output3")}
         self._composed_cache = _FoldCache()
         self._stem_cache = _FoldCache()
         self.fuse_top_down = True  # eval mode on CUDA: composed 1x1 heads (see composed_heads); False = layer by layer
         # scripted forward, frozen by freeze_script (see "TorchScript" above)
         self._s_fast = True
-        self._s_native = True
         self._s_stem_fused = False
         self._s_stem = [torch.zeros(0)] * 4  # stem_weights()
-        self._s_top_down = 0  # 0 = the reference's, 1 = layer by layer (native or ATen lateral conv), 2 = composed heads
+        self._s_top_down = 0  # 0 = the reference's, 1 = layer by layer (native lateral conv), 2 = composed heads
         self._s_precision = 3
         self._s_plain_form: Dict[str, int] = {}  # the plain 1x1 convs (_plain), by name: form, filter image, bias (empty: none)
         self._s_plain_w: Dict[str, Tensor] = {}
@@ -350,17 +300,16 @@ class FeatureNet(nn.Module):
         for i in range(11):
             getattr(self, f"conv{i}").freeze_script()
         self._s_fast = LIBRARY_FAST_PATH
-        self._s_native = LIBRARY_FAST_PATH and ops.NATIVE_CONVS
         self._s_precision = ops.conv_precision()
-        self._s_stem_fused = self._s_native and ops.STEM_FUSED and self._s_precision == 3
+        self._s_stem_fused = self._s_fast and self._s_precision == 3
         self._s_stem = [_host(t) for t in self.stem_weights()] if self._s_stem_fused else [torch.zeros(0)] * 4
-        self._s_top_down = 0 if not LIBRARY_FAST_PATH else (2 if self._s_native and self.fuse_top_down else 1)
+        self._s_top_down = 0 if not LIBRARY_FAST_PATH else (2 if self.fuse_top_down else 1)
         self._s_plain_form, self._s_plain_w, self._s_plain_b, self._s_composed = {}, {}, {}, {}
-        if self._s_native:
-            for name in ("output1", "inner1", "inner2", "output2", "output3"):
-                conv = getattr(self, name)
-                self._s_plain_form[name], self._s_plain_w[name] = _freeze_native(conv.weight, 1)
-                self._s_plain_b[name] = torch.zeros(0) if conv.bias is None else _host(conv.bias)
+        if self._s_fast:
+            for name, packed in self._packed.items():
+                form, filt, bias = packed.packed(getattr(self, name))
+                self._s_plain_form[name], self._s_plain_w[name] = form, _host(filt)
+                self._s_plain_b[name] = torch.zeros(0) if bias is None else _host(bias)
         if self._s_top_down == 2:
             with torch.no_grad():
                 for k, v in self.composed_heads().items():
@@ -394,7 +343,7 @@ class FeatureNet(nn.Module):
         return out
 
     def _plain_script(self, name: str, x: Tensor) -> Tensor:
-        if self._s_native:
+        if self._s_fast:
             cout = 64 if name == "output1" else (32 if name == "output2" else 16)
             return _script_conv(x, self._s_plain_form[name], self._s_plain_w[name], _nonempty(self._s_plain_b[name]), cout, 1, 1, 0, 1,
                                 False, self._s_precision)
@@ -405,23 +354,17 @@ class FeatureNet(nn.Module):
         return self.output3(x)
 
     def _top_down_script(self, coarse: Tensor, lateral_name: str, fine: Tensor) -> Tensor:
-        if lateral_name == "inner1":
-            weight, bias = self.inner1.weight, self.inner1.bias
-        else:
-            weight, bias = self.inner2.weight, self.inner2.bias
         if self._s_top_down == 0:
             lateral = self.inner1(fine) if lateral_name == "inner1" else self.inner2(fine)
             return F.interpolate(coarse, scale_factor=2.0, mode="bilinear", align_corners=False) + lateral
-        if self._s_native:
-            lateral = _script_conv(fine, self._s_plain_form[lateral_name], self._s_plain_w[lateral_name], None, 64, 1, 1, 0, 1, False,
-                                   self._s_precision)
-        else:
-            lateral = F.conv2d(fine, weight, None)
+        lateral = _script_conv(fine, self._s_plain_form[lateral_name], self._s_plain_w[lateral_name], None, 64, 1, 1, 0, 1, False,
+                               self._s_precision)
+        bias = self.inner1.bias if lateral_name == "inner1" else self.inner2.bias
         return torch.ops.pmb200.upsample2x_add(coarse, lateral, bias)
 
     def _plain(self, name: str, x: Tensor) -> Tensor:
         """One of the bias-free / lateral 1x1 convs: native in eval mode on CUDA, else the module itself."""
-        if not self.training and _native_convs(x):
+        if not self.training and _fast(x):
             return self._packed[name](getattr(self, name), x)
         return getattr(self, name)(x)
 
@@ -486,7 +429,7 @@ class FeatureNet(nn.Module):
         place (K-S, csrc/pm_stem.cu); otherwise the two layers one after the other."""
         from . import ops
 
-        if (not self.training and _native_convs(x) and ops.STEM_FUSED and ops.conv_precision() == 3 and x.dim() == 4 and x.shape[1] == 3
+        if (not self.training and _fast(x) and ops.conv_precision() == 3 and x.dim() == 4 and x.shape[1] == 3
                 and x.dtype == torch.float32):
             return ops.conv_stem(x, *self.stem_weights())
         if _fast(x) and not x.is_contiguous(memory_format=torch.channels_last):
@@ -503,7 +446,7 @@ class FeatureNet(nn.Module):
         half = self._trunk(self._stem(x), 2, 4)
         quarter = self._trunk(half, 5, 7)
         eighth = self._trunk(quarter, 8, 10)
-        if not self.training and _native_convs(x) and self.fuse_top_down:
+        if not self.training and _fast(x) and self.fuse_top_down:
             return self._fused_top_down(eighth, quarter, half)
         out: Dict[int, Tensor] = {3: self._plain("output1", eighth)}
         top = self._top_down(eighth, "inner1", quarter)
@@ -517,13 +460,10 @@ class FeatureNet(nn.Module):
         add and the lateral conv's bias are ONE native launch (ATen's channels-last bilinear kernel was the single
         largest launch of the forward, the bias add another full pass over the largest tensor)."""
         lateral_conv = getattr(self, lateral_name)
-        if _fast(coarse) and not self.training and not torch.is_grad_enabled():
+        if _fast(coarse) and not self.training:
             from . import ops
 
-            if _native_convs(fine):
-                lateral = self._packed[lateral_name](lateral_conv, fine, with_bias=False)
-            else:
-                lateral = F.conv2d(fine, lateral_conv.weight, None)
+            lateral = self._packed[lateral_name](lateral_conv, fine, with_bias=False)
             return ops.upsample2x_add(coarse, lateral, lateral_conv.bias)
         return F.interpolate(coarse, scale_factor=2.0, mode="bilinear", align_corners=False) + lateral_conv(fine)
 
@@ -540,13 +480,11 @@ class Refinement(nn.Module):
         self.bn = nn.BatchNorm2d(8)
         self.conv3 = _ConvBnReLU2d(16, 8)
         self.res = nn.Conv2d(8, 1, 3, padding=1, bias=False)
-        self._cache = _FoldCache()
         self._deconv_frag = _FoldCache()
         self._host_cache = _FoldCache()
-        self._res_packed = _PackedConv()
+        self._res_packed = PackedConv()
         # scripted forward, frozen by freeze_script (see "TorchScript" above)
         self._s_fast = True
-        self._s_native = True
         self._s_fused = False
         self._s_host = [torch.zeros(0)] * 11  # host_weights() for K-R
         self._s_precision = 3
@@ -554,8 +492,6 @@ class Refinement(nn.Module):
         self._s_deconv_b = torch.zeros(0)
         self._s_res_form = 0
         self._s_res_w = torch.zeros(0)
-        self._s_up_w = torch.zeros(0)  # ATen tail: folded transposed conv
-        self._s_up_b = torch.zeros(0)
         self.register_load_state_dict_post_hook(_freeze_after_load)
 
     def train(self, mode: bool = True):
@@ -571,18 +507,15 @@ class Refinement(nn.Module):
         for m in (self.conv0, self.conv1, self.conv2, self.conv3):
             m.freeze_script()
         self._s_fast = LIBRARY_FAST_PATH
-        self._s_native = LIBRARY_FAST_PATH and ops.NATIVE_CONVS
         self._s_precision = ops.conv_precision()
-        self._s_fused = self._s_native and ops.REFINE_FUSED and self._s_precision == 3 and self.res.bias is None
+        self._s_fused = self._s_fast and self._s_precision == 3 and self.res.bias is None
         self._s_host = [_host(t) for t in self.host_weights()] if self._s_fused else [torch.zeros(0)] * 11
-        with torch.no_grad():
-            if self._s_native:
+        if self._s_fast:
+            with torch.no_grad():
                 w, b = _fold_bn(self.deconv.weight, self.bn, out_dim=1)
                 self._s_deconv_w, self._s_deconv_b = _host(ops.pack_conv_filter(w, self._s_precision, transposed=True)), _host(b)
-                self._s_res_form, self._s_res_w = _freeze_native(self.res.weight, 1)
-            if self._s_fast:
-                w, b = _fold_bn(self.deconv.weight, self.bn, out_dim=1)
-                self._s_up_w, self._s_up_b = _host(w), _host(b)
+            self._s_res_form, filt, _ = self._res_packed.packed(self.res)
+            self._s_res_w = _host(filt)
 
     def _forward_script(self, img: Tensor, depth_half: Tensor, depth_min: Tensor, depth_max: Tensor) -> Tensor:
         if self.training:
@@ -599,7 +532,7 @@ class Refinement(nn.Module):
         d = (depth_half - lo) / span
         if self._s_fast:
             img = img.contiguous(memory_format=torch.channels_last)
-        if self._s_native and img.size(-2) == 2 * d.size(-2) and img.size(-1) == 2 * d.size(-1):  # _native_tail
+        if self._s_fast and img.size(-2) == 2 * d.size(-2) and img.size(-1) == 2 * d.size(-1):  # _native_tail
             low = self.conv2.native_script(self.conv1.native_script(d))
             both = torch.empty([low.size(0), 16, 2 * low.size(2), 2 * low.size(3)], dtype=torch.float32, device=low.device,
                                memory_format=torch.channels_last)
@@ -608,13 +541,8 @@ class Refinement(nn.Module):
             self.conv0.native_script(img, both, 8)
             res = _script_conv(self.conv3.native_script(both), self._s_res_form, self._s_res_w, None, 1, 3, 1, 1, 1, False,
                                self._s_precision)
-        else:
-            x = self.conv2(self.conv1(d))
-            if self._s_fast:
-                up = F.relu_(F.conv_transpose2d(x, torch.ops.pmb200.device_copy(self._s_up_w, x),
-                                                torch.ops.pmb200.device_copy(self._s_up_b, x), stride=2, padding=1, output_padding=1))
-            else:
-                up = F.relu(self.bn(self.deconv(x)), inplace=True)
+        else:  # the reference's layers; torch.cat needs the image at exactly twice the depth map's size
+            up = F.relu(self.bn(self.deconv(self.conv2(self.conv1(d)))), inplace=True)
             res = self.res(self.conv3(torch.cat((up, self.conv0(img)), dim=1)))
         d = F.interpolate(d, scale_factor=2.0, mode="nearest") + res
         return d * span + lo
@@ -641,14 +569,6 @@ class Refinement(nn.Module):
         ops.conv2d_nhwc(low, frag, b, 8, 3, 1, 1, 1, relu=True, transposed2x=True, out=both, out_channel_offset=0)
         self.conv0.native(img, out=both, out_channel_offset=8)
         return self._res_packed(self.res, self.conv3.native(both))
-
-    def _upsample(self, x: Tensor) -> Tensor:
-        if self.training or not _fast(x):
-            return F.relu(self.bn(self.deconv(x)), inplace=True)
-        bn = self.bn
-        srcs = [self.deconv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var]
-        w, b = self._cache.get(srcs, lambda: _fold_bn(self.deconv.weight, bn, out_dim=1))
-        return F.relu_(F.conv_transpose2d(x, w, b, stride=2, padding=1, output_padding=1))
 
     def host_weights(self):
         """BatchNorm-folded weights of the six layers as HOST tensors, in the argument order of ops.refine_low (first four) and
@@ -685,19 +605,20 @@ class Refinement(nn.Module):
     def _forward_eager(self, img: Tensor, depth_half: Tensor, depth_min: Tensor, depth_max: Tensor) -> Tensor:
         from . import ops
 
-        if (not self.training and _native_convs(img) and ops.REFINE_FUSED and ops.conv_precision() == 3 and img.dtype == torch.float32
+        fast = not self.training and _fast(img)
+        if (fast and ops.conv_precision() == 3 and img.dtype == torch.float32
                 and img.shape[-2:] == (2 * depth_half.shape[-2], 2 * depth_half.shape[-1]) and self.res.bias is None):
             return self._fused(img, depth_half.float(), depth_min.float(), depth_max.float())
         B = depth_min.size(0)
         lo = depth_min.view(B, 1, 1, 1)
         span = (depth_max - depth_min).view(B, 1, 1, 1)
         d = (depth_half - lo) / span
-        if _fast(img) and not self.training:
+        if fast:
             img = img.contiguous(memory_format=torch.channels_last)
-        if not self.training and _native_convs(img) and img.shape[-2:] == (2 * d.shape[-2], 2 * d.shape[-1]):
+        if fast and img.shape[-2:] == (2 * d.shape[-2], 2 * d.shape[-1]):
             res = self._native_tail(img, d)
-        else:
-            up = self._upsample(self.conv2(self.conv1(d)))
+        else:  # the reference's layers; torch.cat needs the image at exactly twice the depth map's size
+            up = F.relu(self.bn(self.deconv(self.conv2(self.conv1(d)))), inplace=True)
             res = self.res(self.conv3(torch.cat((up, self.conv0(img)), dim=1)))
         d = F.interpolate(d, scale_factor=2.0, mode="nearest") + res
         return d * span + lo
@@ -800,7 +721,7 @@ class PatchmatchNet(nn.Module):
         from . import ops
 
         self._s_fast = LIBRARY_FAST_PATH
-        self._s_ref_channels_last = LIBRARY_FAST_PATH and not (ops.REFINE_FUSED and ops.NATIVE_CONVS and ops.conv_precision() == 3)
+        self._s_ref_channels_last = LIBRARY_FAST_PATH and ops.conv_precision() != 3
 
     def extract_features(self, images: List[Tensor]) -> List[Dict[int, Tensor]]:
         """One FeatureNet pass per view (reference net.py:203-208).  In eval mode the
@@ -814,13 +735,13 @@ class PatchmatchNet(nn.Module):
             x = torch.as_strided(first, (n * b,) + tuple(first.shape[1:]), first.stride())  # views of one buffer: no copy
         else:
             x = torch.cat(images, dim=0)
-        if _fast(x):  # the pyramid comes out channels-last, the layout the fused PatchMatch kernels read in place.  FeatureNet's
-            # first layers read the NCHW planes themselves (K-S) or convert; only the reference view is needed channels-last
-            # again, by Refinement's conv-family path; its fused form (K-R) reads the NCHW planes itself
-            from . import ops
+        from . import ops
 
-            if not (ops.REFINE_FUSED and ops.NATIVE_CONVS and ops.conv_precision() == 3):
-                self._ref_image_cl = first.contiguous(memory_format=torch.channels_last)
+        # the pyramid comes out channels-last, the layout the fused PatchMatch kernels read in place.  FeatureNet's first layers
+        # read the NCHW planes themselves (K-S) or convert; only the reference view is needed channels-last again, by
+        # Refinement's layer-by-layer path in the TF32 mode; its fused form (K-R) reads the NCHW planes itself
+        if _fast(x) and ops.conv_precision() != 3:
+            self._ref_image_cl = first.contiguous(memory_format=torch.channels_last)
         stacked = self.feature(x)
         return [{k: v[i * b:(i + 1) * b] for k, v in stacked.items()} for i in range(n)]
 

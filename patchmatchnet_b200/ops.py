@@ -8,7 +8,6 @@ an error (there is no fallback path).
 """
 from __future__ import annotations
 
-import os
 from typing import List, Optional, Sequence, Tuple, Union
 
 import torch
@@ -234,23 +233,15 @@ def upsample2x_add(x: Tensor, y: Tensor, bias: Optional[Tensor] = None) -> Tenso
     return out
 
 
-# The small learned convs (offset convs of the hot path, FeatureNet, Refinement) run through csrc/pm_conv.cu in eval
-# mode.  False (or PMB200_NATIVE_CONVS=0) hands them back to cuDNN -- kept only for A/B measurements.
-NATIVE_CONVS = os.environ.get("PMB200_NATIVE_CONVS", "1") != "0"
-NATIVE_CONVS_ALL = os.environ.get("PMB200_NATIVE_CONVS", "1") == "all"  # A/B aid: native even where the library is faster
-
-
 def conv_prefers_native(cin: int, cout: int, ks: int) -> bool:
     """Which implementation runs a small conv in eval mode (per-layer timings: tools/convbench.py).  The native
     channels-last kernel takes the memory-bound layers -- every 1x1 conv and every layer with at most 3200 multiply-adds
     per output pixel (full-resolution 3->8 / 8->8 / 8->16 convs, the refinement head, the stage-1 offset conv) -- while in
     the TF32 mode the FLOP-heavy 16..64-channel 3x3 / 5x5 layers stay with cuDNN's implicit-GEMM kernels."""
-    if not NATIVE_CONVS:
-        return False
     # fp32-accurate mode (cudnn.allow_tf32 off): the library's fp32 kernels for the FLOP-bound layers do not use the tensor
     # cores at all, the native 3xTF32 kernels do -> every conv native.  The parity configuration and the bench default are
     # this mode (the depth maps of the TF32 mode are outside north_star's 1e-3: tests/test_gpu_bench_mode.py).
-    return NATIVE_CONVS_ALL or conv_precision() == 3 or ks == 1 or cin * cout * ks * ks <= 3200
+    return conv_precision() == 3 or ks == 1 or cin * cout * ks * ks <= 3200
 
 
 def _round_kcin(cin: int) -> int:
@@ -299,49 +290,39 @@ def pack_conv_filter(weight: Tensor, precision: int, transposed: bool = False) -
     return torch.cat((hi, lo), dim=-1).contiguous().view(-1)
 
 
-# K-D5 (csrc/pm_conv5.cu): wgmma / TMA implicit-GEMM convolution, fp32-accurate (3xTF32).  Used in the
-# fp32-accurate mode for the layers it serves when TC5_CONVS is on (PMB200_TC5=0 hands them back to the mma.sync kernel).
-TC5_CONVS = os.environ.get("PMB200_TC5", "1") != "0"
-
-
-# (Cin, Cout, KS, stride) of the layers a wgmma form serves instead of the mma.sync kernel's 3xTF32 mode (cold time per launch
-# at the 640x512 sizes: tools/convbench.py).  Per-tap form K-D5 (the only one for stride 2): the 16->32 and 32->64 5x5 stride-2
-# layers; not conv2 (Cin = 8: one K slice per tap, the instruction count is the cost).  PMB200_TC5=all takes every supported
-# layer (A/B measurements), PMB200_TC5=0 none.
+# (Cin, Cout, KS, stride) of the layers a wgmma form (csrc/pm_conv5.cu, fp32-accurate 3xTF32) serves instead of the mma.sync
+# kernel's 3xTF32 mode (cold time per launch at the 640x512 sizes: tools/convbench.py).  Per-tap form K-D5 (the only one for
+# stride 2): the 16->32 and 32->64 5x5 stride-2 layers; not conv2 (Cin = 8: one K slice per tap, the instruction count is the
+# cost).
 TC5_LAYERS = {(16, 32, 5, 2), (32, 64, 5, 2)}
-TC5_ALL = os.environ.get("PMB200_TC5", "1") == "all"
 # Stride-1 layers served by the halo-tile form K-D5h (one TMA box + one split per output tile, taps as shifted descriptors,
 # [w_hi | w_lo] as one operand): FeatureNet conv3/4, conv6/7, conv9/10, output2/3 and the offset convs of every stage.  Not
 # where Cin = 8 (conv1: one K slice per tap, the instruction count is the cost) nor Refinement.
-# PMB200_TC5H=all: every stride-1 layer the kernel takes (A/B measurements); =0: none.
 TC5H_LAYERS = {(16, 16, 3, 1), (32, 32, 3, 1), (64, 64, 3, 1), (64, 32, 1, 1), (64, 16, 1, 1),
                (64, 32, 3, 1), (64, 18, 3, 1), (32, 16, 3, 1), (32, 18, 3, 1), (16, 18, 3, 1)}
-TC5H_ALL = os.environ.get("PMB200_TC5H", "1") == "all"
-TC5H_OFF = os.environ.get("PMB200_TC5H", "1") == "0"
 
 
-def conv_tc5_mode(cin: int, cout: int, ks: int, stride: int = 1, transposed: bool = False, fused_add: bool = False) -> str:
-    """"" (mma.sync kernel), "halo" (K-D5h) or "tap" (K-D5): which wgmma form, if any, runs this conv.  Only in the
-    fp32-accurate mode (the arithmetic of both IS the 3xTF32 split), never with a fused transposed / upsample-add epilogue, and
-    only for layers on the measured lists above."""
-    if not (NATIVE_CONVS and TC5_CONVS) or transposed or fused_add or conv_precision() != 3:
-        return ""
-    if not _native.lib().pmb200_conv2d_tc5_supported(cin, cout, ks, stride):
-        return ""
+def conv_form(cin: int, cout: int, ks: int, stride: int = 1) -> int:
+    """Which native kernel runs a conv of this shape: 0 = the mma.sync kernel (conv2d_nhwc), 1 = the wgmma tap form K-D5,
+    2 = the wgmma halo-tile form K-D5h (conv2d_tc5).  The wgmma forms only in the fp32-accurate mode (the arithmetic of both
+    IS the 3xTF32 split) and only for layers on the measured lists above; a fused transposed / upsample-add epilogue exists
+    in form 0 alone."""
+    if conv_precision() != 3 or not _native.lib().pmb200_conv2d_tc5_supported(cin, cout, ks, stride):
+        return 0
     key = (cin, cout, ks, stride)
-    if stride == 1 and not TC5H_OFF and (TC5H_ALL or key in TC5H_LAYERS):
-        return "halo"
-    if TC5_ALL or key in TC5_LAYERS:
-        return "tap"
-    return ""
+    if stride == 1 and key in TC5H_LAYERS:
+        return 2
+    return 1 if key in TC5_LAYERS else 0
 
 
-def conv_uses_tc5(cin: int, cout: int, ks: int, stride: int = 1, transposed: bool = False, fused_add: bool = False) -> bool:
-    return conv_tc5_mode(cin, cout, ks, stride, transposed, fused_add) != ""
-
-
-def pack_conv_filter_tc5_for(weight: Tensor, mode: str) -> Tensor:
-    return pack_conv_filter_tc5h(weight) if mode == "halo" else pack_conv_filter_tc5(weight)
+def pack_conv_filter_for(weight: Tensor, form: int, precision: int) -> Tensor:
+    """The filter image the kernel of `form` (conv_form) reads: pack_conv_filter for `precision` (form 0),
+    pack_conv_filter_tc5 (form 1) or pack_conv_filter_tc5h (form 2)."""
+    if form == 2:
+        return pack_conv_filter_tc5h(weight)
+    if form == 1:
+        return pack_conv_filter_tc5(weight)
+    return pack_conv_filter(weight, precision)
 
 
 def pack_conv_filter_tc5(weight: Tensor) -> Tensor:
@@ -393,10 +374,6 @@ def pack_conv_filter_tc5h(weight: Tensor) -> Tensor:
     return t.contiguous().view(-1)
 
 
-# K-S (csrc/pm_stem.cu): FeatureNet's conv0 -> conv1 as one exact-fp32 launch; PMB200_STEM=0 keeps the two K-D launches.
-STEM_FUSED = os.environ.get("PMB200_STEM", "1") != "0"
-
-
 def conv_stem(x: Tensor, w0: Tensor, b0: Tensor, w1: Tensor, b1: Tensor) -> Tensor:
     """relu(conv1(relu(conv0(x)))) of FeatureNet (3 -> 8 -> 8, 3x3, pad 1; reference models/net.py:18-19, :44) in one launch.
     `x` [N,3,H,W] contiguous NCHW on the device; the BatchNorm-folded weights `w0` [8,3,3,3], `b0` [8], `w1` [8,8,3,3], `b1` [8]
@@ -415,11 +392,6 @@ def conv_stem(x: Tensor, w0: Tensor, b0: Tensor, w1: Tensor, b1: Tensor) -> Tens
                                             _stream(x))
     _native.check(rc, "conv_stem")
     return y
-
-
-# K-R (csrc/pm_refine.cu + the one-plane form of csrc/pm_stem.cu): Refinement as two exact-fp32 launches; PMB200_REFINE=0 keeps
-# the six conv-family launches and the ATen tail.
-REFINE_FUSED = os.environ.get("PMB200_REFINE", "1") != "0"
 
 
 def _host_weights(name: str, pairs) -> None:

@@ -30,11 +30,12 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _native, ops
+from .net import PackedConv
 
 Tensor = torch.Tensor
 
 
-_FOLD_CACHE: "weakref.WeakKeyDictionary" = weakref.WeakKeyDictionary()
+_HEAD_CACHE: "weakref.WeakKeyDictionary" = weakref.WeakKeyDictionary()
 _HEAD_FLOATS = 16 * 8 + 16 + 8 * 16 + 8 + 8 + 1  # sizeof(pmb200_mlp) / 4
 
 
@@ -43,27 +44,13 @@ def _refresh_after_load(module, incompatible_keys) -> None:
         module.refresh_script_heads()
 
 
-def _offset_conv(conv: nn.Conv2d, x: Tensor, native: bool) -> Tensor:
-    """propa_conv / eval_conv (reference patchmatch.py:288-311, called at :486 / :498).  `native`: the channels-last
-    tensor-core conv of csrc/pm_conv.cu (its channels-last output is what the fused kernels consume in place); the
-    fragment-ordered filter is cached off the module (TorchScript would try to type the attribute)."""
+def _offset_conv(conv: nn.Conv2d, packed: PackedConv, x: Tensor, native: bool) -> Tensor:
+    """propa_conv / eval_conv (reference patchmatch.py:288-311, called at :486 / :498).  `native`: the conv's native form
+    (its channels-last output is what the fused kernels consume in place), filter cached in `packed`."""
     if (not native or max(conv.in_channels, conv.out_channels) > 64
             or not ops.conv_prefers_native(conv.in_channels, conv.out_channels, conv.kernel_size[0])):
         return conv(x)
-    srcs = (conv.weight, conv.bias)
-    tc5 = ops.conv_tc5_mode(conv.in_channels, conv.out_channels, conv.kernel_size[0], 1)
-    prec = "tc5" + tc5 if tc5 else ops.conv_precision()
-    stamp = (prec,) + tuple((t.data_ptr(), t._version, t.device) for t in srcs)
-    cached = _FOLD_CACHE.get(conv)
-    if cached is None or cached[0] != stamp:
-        with torch.no_grad():
-            pack = ops.pack_conv_filter_tc5_for(conv.weight, tc5) if tc5 else ops.pack_conv_filter(conv.weight, prec)
-            cached = (stamp, (pack, conv.bias.detach().clone()))
-        _FOLD_CACHE[conv] = cached
-    frag, bias = cached[1]
-    if tc5:  # wgmma implicit GEMM (csrc/pm_conv5.cu); its channels-last output is consumed in place like the other's
-        return ops.conv2d_tc5(x, frag, bias, conv.out_channels, conv.kernel_size[0], 1, conv.padding[0], conv.dilation[0], halo=tc5 == "halo")
-    return ops.conv2d_nhwc(x, frag, bias, conv.out_channels, conv.kernel_size[0], 1, conv.padding[0], conv.dilation[0])
+    return packed(conv, x)
 
 
 def is_empty(x: Tensor) -> bool:
@@ -111,7 +98,7 @@ class _PointwiseHead(nn.Module):
         (DepthEngine warms up before capturing)."""
         tensors = list(self.parameters()) + list(self.buffers())
         stamp = tuple((t.data_ptr(), t._version) for t in tensors)
-        cached = _FOLD_CACHE.get(self)  # kept off the module: TorchScript would try to type a ctypes attribute
+        cached = _HEAD_CACHE.get(self)  # kept off the module: TorchScript would try to type a ctypes attribute
         if cached is not None and cached[0] == stamp:
             return cached[1]
         with torch.no_grad():
@@ -138,7 +125,7 @@ class _PointwiseHead(nn.Module):
         m.b1[:] = b1.tolist()
         m.w2[:] = w2.tolist()
         m.b2 = b2
-        _FOLD_CACHE[self] = (stamp, m)
+        _HEAD_CACHE[self] = (stamp, m)
         return m
 
 
@@ -234,6 +221,7 @@ class PatchMatch(nn.Module):
         for conv in (self.propa_conv, self.eval_conv):
             nn.init.constant_(conv.weight, 0.0)
             nn.init.constant_(conv.bias, 0.0)
+        self._propa_packed, self._eval_packed = PackedConv(), PackedConv()  # their native filters (eval mode)
         self.feature_weight_net = FeatureWeightNet(evaluate_neighbors, G)
         # Folded heads as plain CPU tensors for the TorchScript path (not buffers: the state dict must keep exactly
         # the reference's keys).  Refreshed on eval() / load_state_dict, i.e. before the reference scripts the model
@@ -249,7 +237,7 @@ class PatchMatch(nn.Module):
         self._conv_precision = 3
         self._native_propa = False  # ops.conv_prefers_native(...) for the two offset convs, frozen likewise
         self._native_eval = False
-        # which native form runs each offset conv, as ops.conv_tc5_mode picks it for the eager path: 0 = the mma.sync kernel
+        # which native form runs each offset conv, as ops.conv_form picks it for the eager path: 0 = the mma.sync kernel
         # (conv2d_nhwc, filter in fragment order), 1 = the wgmma tap form, 2 = the wgmma halo-tile form (conv2d_tc5)
         self._off_propa_form = 0
         self._off_eval_form = 0
@@ -268,18 +256,15 @@ class PatchMatch(nn.Module):
         fits = lambda conv: max(conv.in_channels, conv.out_channels) <= 64
         self._native_propa = fits(self.propa_conv) and ops.conv_prefers_native(self.propa_conv.in_channels, self.propa_conv.out_channels, 3)
         self._native_eval = fits(self.eval_conv) and ops.conv_prefers_native(self.eval_conv.in_channels, self.eval_conv.out_channels, 3)
-        self._off_propa_form, self._off_propa_frag = self._freeze_offset_conv(self.propa_conv, self._native_propa)
-        self._off_eval_form, self._off_eval_frag = self._freeze_offset_conv(self.eval_conv, self._native_eval)
+        self._off_propa_form, self._off_propa_frag = self._freeze_offset_conv(self.propa_conv, self._propa_packed, self._native_propa)
+        self._off_eval_form, self._off_eval_frag = self._freeze_offset_conv(self.eval_conv, self._eval_packed, self._native_eval)
 
-    def _freeze_offset_conv(self, conv: nn.Conv2d, native: bool) -> Tuple[int, Tensor]:
+    def _freeze_offset_conv(self, conv: nn.Conv2d, packed: PackedConv, native: bool) -> Tuple[int, Tensor]:
         """(form, host filter image) of one offset conv for the scripted forward: the form `_offset_conv` takes in eager mode."""
         if not native:
             return 0, torch.zeros(1)
-        tc5 = ops.conv_tc5_mode(conv.in_channels, conv.out_channels, conv.kernel_size[0], 1)
-        with torch.no_grad():
-            if tc5:
-                return (2 if tc5 == "halo" else 1), ops.pack_conv_filter_tc5_for(conv.weight, tc5).cpu()
-            return 0, ops.pack_conv_filter(conv.weight, self._conv_precision).cpu()
+        form, filt, _ = packed.packed(conv)
+        return form, filt.cpu()
 
     def train(self, mode: bool = True):
         super().train(mode)
@@ -467,11 +452,11 @@ class PatchMatch(nn.Module):
         depth_max = depth_max.reshape(B).float()
 
         # learned 2-D offsets: native channels-last tensor-core conv (inference), cuDNN + autograd (training)
-        native_conv = ops.NATIVE_CONVS and not need_grad and not torch.is_grad_enabled()
+        native_conv = not torch.is_grad_enabled()
         propa_off: Optional[Tensor] = None
         if Kp > 0 and not (self.stage == 1 and iters == 1):
-            propa_off = _offset_conv(self.propa_conv, ref_feature, native_conv)
-        eval_off = _offset_conv(self.eval_conv, ref_feature, native_conv)
+            propa_off = _offset_conv(self.propa_conv, self._propa_packed, ref_feature, native_conv)
+        eval_off = _offset_conv(self.eval_conv, self._eval_packed, ref_feature, native_conv)
 
         # channels-last feature pack [1+V,B,H,W,C] (zero-copy if the producer already emitted it)
         same_size = all(f.shape == ref_feature.shape for f in src_features)

@@ -332,8 +332,9 @@ def test_gpu_transposed_conv_and_channel_slices(fp32_library):
 
 
 @pytest.mark.gpu
-def test_gpu_net_native_convs_match_library_convs(fp32_library, golden_weights):
-    """Whole network, eval mode: native convs (3xTF32) vs the folded cuDNN convs in fp32 -- same depth map."""
+def test_gpu_net_native_convs_match_the_reference_op_sequence(fp32_library, golden_weights):
+    """Whole network, eval mode: native convs (3xTF32) vs the reference's op sequence on cuDNN in fp32 -- same depth map."""
+    from patchmatchnet_b200 import net as pm_net
     from patchmatchnet_b200 import synthetic
     from patchmatchnet_b200.net import PatchmatchNet, load_reference_state
 
@@ -345,16 +346,15 @@ def test_gpu_net_native_convs_match_library_convs(fp32_library, golden_weights):
     args = lambda: ([i.to(dev) for i in inp["images"]], inp["intrinsics"].to(dev), inp["extrinsics"].to(dev),
                     inp["depth_min"].to(dev), inp["depth_max"].to(dev))
     outs = {}
-    old = ops.NATIVE_CONVS
     try:
         for flag in (True, False):
-            ops.NATIVE_CONVS = flag
+            pm_net.LIBRARY_FAST_PATH = flag
             torch.manual_seed(0)
             with torch.no_grad():
                 depth, conf, _ = net(*args())
             outs[flag] = (depth, conf)
     finally:
-        ops.NATIVE_CONVS = old
+        pm_net.LIBRARY_FAST_PATH = True
     rel = float((outs[True][0] - outs[False][0]).abs().sum() / outs[False][0].abs().sum())
     assert rel <= 1e-4, rel
 
@@ -440,9 +440,9 @@ def test_gpu_conv_stem_matches_cudnn_fp32(fp32_library):
 
 
 @pytest.mark.gpu
-def test_gpu_fused_refinement_matches_the_layerwise_path(fp32_library, monkeypatch):
+def test_gpu_fused_refinement_matches_the_native_tail_and_the_reference(fp32_library, monkeypatch):
     """K-R (two exact-fp32 launches) against the same module run layer by layer on cuDNN fp32 kernels, and against the
-    conv-family path it replaces; bench size and a ragged one."""
+    six native conv launches it replaces (Refinement._native_tail, the TF32 mode's path); bench size and a ragged one."""
     from patchmatchnet_b200 import net as pm_net
     from tests.test_emulated_conv import _random_refinement
 
@@ -454,15 +454,15 @@ def test_gpu_fused_refinement_matches_the_layerwise_path(fp32_library, monkeypat
         dmin = torch.tensor([400.0, 425.0][:N], device=dev)
         dmax = torch.tensor([900.0, 935.0][:N], device=dev)
         depth = dmin.view(N, 1, 1, 1) + torch.rand(N, 1, h, w, generator=g).to(dev) * (dmax - dmin).view(N, 1, 1, 1)
-        span = (dmax - dmin).view(N, 1, 1, 1)
+        lo, span = dmin.view(N, 1, 1, 1), (dmax - dmin).view(N, 1, 1, 1)
         with torch.no_grad():
             got = m(img, depth, dmin, dmax)
-            monkeypatch.setattr(ops, "REFINE_FUSED", False)
-            family = m(img, depth, dmin, dmax)                 # conv-family launches + ATen tail
+            d = (depth - lo) / span                            # six native conv launches, then Refinement's own tail
+            res = m._native_tail(img.contiguous(memory_format=torch.channels_last), d)
+            family = (F.interpolate(d, scale_factor=2.0, mode="nearest") + res) * span + lo
             monkeypatch.setattr(pm_net, "LIBRARY_FAST_PATH", False)
             want = m(img, depth, dmin, dmax)                   # the reference's own op sequence on cuDNN fp32
             monkeypatch.setattr(pm_net, "LIBRARY_FAST_PATH", True)
-            monkeypatch.setattr(ops, "REFINE_FUSED", True)
         torch.cuda.synchronize()
         assert got.shape == want.shape == (N, 1, 2 * h, 2 * w)
         assert float(((got - want).abs() / span).max()) <= 5e-6, (N, h, w)

@@ -94,21 +94,19 @@ def test_network_scripts_with_native_calls_only_and_keeps_the_reference_keys(gol
         assert torch.equal(v, net.state_dict()[k]), k
 
 
-def test_frozen_decisions_are_what_eager_picks(golden_weights, tf32):
+def test_frozen_decisions_are_the_conv_forms_eager_picks(golden_weights, tf32):
     net = _net(golden_weights)
     pairs = [(net.feature, f"conv{i}") for i in range(11)] + [(net.upsample_net, f"conv{i}") for i in range(4)]
     for owner, name in pairs:
         layer = getattr(owner, name)
         c = layer.conv
         prefers = ops.conv_prefers_native(c.in_channels, c.out_channels, c.kernel_size[0])
-        mode = ops.conv_tc5_mode(c.in_channels, c.out_channels, c.kernel_size[0], c.stride[0])
         assert layer._s_mode == (2 if prefers else 1), name
-        assert layer._s_form == {"": 0, "tap": 1, "halo": 2}[mode], name
+        assert layer._s_form == ops.conv_form(c.in_channels, c.out_channels, c.kernel_size[0], c.stride[0]), name
         assert layer._s_precision == ops.conv_precision()
     for name in ("output1", "inner1", "inner2", "output2", "output3"):
         c = getattr(net.feature, name)
-        mode = ops.conv_tc5_mode(c.in_channels, c.out_channels, 1, 1)
-        assert net.feature._s_plain_form[name] == {"": 0, "tap": 1, "halo": 2}[mode], name
+        assert net.feature._s_plain_form[name] == ops.conv_form(c.in_channels, c.out_channels, 1, 1), name
     assert net.feature._s_stem_fused == (not tf32) and net.upsample_net._s_fused == (not tf32)
     assert net.feature._s_top_down == 2
     for stage in (net.patchmatch_1, net.patchmatch_2, net.patchmatch_3):
@@ -116,8 +114,7 @@ def test_frozen_decisions_are_what_eager_picks(golden_weights, tf32):
                                    (stage.eval_conv, stage._native_eval, stage._off_eval_form)):
             assert native == ops.conv_prefers_native(conv.in_channels, conv.out_channels, 3)
             if native:
-                mode = ops.conv_tc5_mode(conv.in_channels, conv.out_channels, 3, 1)
-                assert form == {"": 0, "tap": 1, "halo": 2}[mode]
+                assert form == ops.conv_form(conv.in_channels, conv.out_channels, 3, 1)
     if not tf32:  # the stage offset convs of ops.TC5H_LAYERS take the halo-tile form, as in eager
         assert net.patchmatch_3._off_eval_form == 2 and net.patchmatch_2._off_eval_form == 2
     assert not any(k.startswith("_s_") or "._s_" in k for k in net.state_dict())
@@ -241,7 +238,7 @@ def _cl(t):
 
 
 @pytest.mark.gpu
-def test_new_ops_equal_the_ctypes_wrappers():
+def test_new_ops_equal_the_ctypes_wrappers_in_every_conv_form():
     g = torch.Generator().manual_seed(5)
     P = torch.ops.pmb200
     x = _cl(torch.randn(2, 32, 24, 40, generator=g))
@@ -254,14 +251,14 @@ def test_new_ops_equal_the_ctypes_wrappers():
             out = torch.empty_like(want)
             P.conv2d_nhwc_out(x, frag, b, cout, ks, stride, pad, dil, True, prec, False, None, out, 0)  # host filter and bias
             assert torch.equal(out, want)
-        for mode in ("tap", "halo"):
-            if mode == "halo" and stride != 1:
+        for form in (1, 2):
+            if form == 2 and stride != 1:
                 continue
-            filt = ops.pack_conv_filter_tc5_for(w, mode)
-            want = ops.conv2d_tc5(x, filt.to(DEV), b.to(DEV), cout, ks, stride, pad, dil, relu=True, halo=mode == "halo")
-            assert torch.equal(P.conv2d_tc5(x, filt, b, cout, ks, stride, pad, dil, True, mode == "halo"), want)
+            filt = ops.pack_conv_filter_for(w, form, 3)
+            want = ops.conv2d_tc5(x, filt.to(DEV), b.to(DEV), cout, ks, stride, pad, dil, relu=True, halo=form == 2)
+            assert torch.equal(P.conv2d_tc5(x, filt, b, cout, ks, stride, pad, dil, True, form == 2), want)
             wide = torch.zeros(want.shape[0], cout + 8, *want.shape[2:], device=DEV).contiguous(memory_format=torch.channels_last)
-            P.conv2d_tc5_out(x, filt, b.to(DEV), cout, ks, stride, pad, dil, True, mode == "halo", wide, 8)
+            P.conv2d_tc5_out(x, filt, b.to(DEV), cout, ks, stride, pad, dil, True, form == 2, wide, 8)
             assert torch.equal(wide[:, 8:], want) and not wide[:, :8].any()
     # add_up2x, transposed2x and a channel window of a wider output
     fine = _cl(torch.randn(2, 16, 24, 40, generator=g))

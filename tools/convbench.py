@@ -135,7 +135,8 @@ c, cmin, wm = timeit(lambda: ops.conv_stem(x3, w0, b0, w1, b1))
 stem = {"pixels_per_thread_ab_us": stem_ab, "layer": "feature.conv0+conv1 fused (K-S)", "shape": f"N5 3->8->8 k3 {H}x{W}", "stem_us": {"cold": round(c, 1), "cold_min": round(cmin, 1), "warm": round(wm, 1)},
         "replaces_us_cold": sum(r["native_p3_mt0_us"]["cold"] for r in rows if r["layer"] in ("feature.conv0", "feature.conv1")),
         "gbs_in_plus_out": round(4 * 5 * H * W * (3 + 8) / (c * 1e-6) / 1e9, 1)}
-# K-R: Refinement fused into two exact-fp32 launches against its conv-family path (six launches + the ATen tail), one view
+# K-R: Refinement fused into two exact-fp32 launches against its conv-family path (the six native conv launches of
+# Refinement._native_tail, without the elementwise depth tail), one view
 from patchmatchnet_b200.net import Refinement  # noqa: E402
 
 torch.backends.cudnn.allow_tf32 = False
@@ -144,12 +145,12 @@ rimg = torch.rand(1, 3, H, W, generator=g).to(dev)
 rlo, rhi = torch.tensor([425.0], device=dev), torch.tensor([935.0], device=dev)
 rdepth = 425.0 + 510.0 * torch.rand(1, 1, H // 2, W // 2, generator=g).to(dev)
 refine = {"layer": "Refinement (K-R)", "shape": f"N1 {H}x{W}"}
+rd = (rdepth - rlo) / (rhi - rlo)
+rimg_cl = rimg.contiguous(memory_format=torch.channels_last)
 with torch.no_grad():
-    for flag, key in ((True, "fused_us"), (False, "conv_family_us")):
-        ops.REFINE_FUSED = flag
-        c, cmin, wm = timeit(lambda: ref_mod(rimg, rdepth, rlo, rhi))
+    for key, fn in (("fused_us", lambda: ref_mod(rimg, rdepth, rlo, rhi)), ("conv_family_us", lambda: ref_mod._native_tail(rimg_cl, rd))):
+        c, cmin, wm = timeit(fn)
         refine[key] = {"cold": round(c, 1), "cold_min": round(cmin, 1), "warm": round(wm, 1)}
-ops.REFINE_FUSED = True
 torch.backends.cudnn.allow_tf32 = True
 tot_lib = sum(r["cudnn_tf32_us"]["cold"] for r in rows)
 tot_nat = sum(r["native_p1_mt0_us"]["cold"] for r in rows if isinstance(r.get("native_p1_mt0_us"), dict))

@@ -1,7 +1,7 @@
 """e2e (pinned host in -> pinned host out) through DepthEngine.infer_stream at several request counts, with the host-side
 enqueue time of the loop measured separately: separates pipeline fill / drain, host-bound and GPU-bound regimes.
 
-    PMB200_REFINE=0 python tools/e2e_probe.py
+    python tools/e2e_probe.py
 """
 import json
 import os
@@ -22,7 +22,7 @@ net, _ = bench.build_net()
 net = net.to(dev)
 wl = bench.Workload(net, 1, 5, 512, 640, dev, 3, 0)
 stream = torch.cuda.current_stream()
-out = {"refine_fused": os.environ.get("PMB200_REFINE", "1") != "0", "stem_fused": os.environ.get("PMB200_STEM", "1") != "0", "numa": numa, "rows": []}
+out = {"numa": numa, "rows": []}
 for steps in (20, 20, 60, 200, 200):
     reqs = [wl.host_pinned] * steps
     torch.cuda.synchronize()
