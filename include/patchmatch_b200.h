@@ -186,6 +186,12 @@ int pmb200_conv2d_nhwc(const float *x, const float *filter_frag, const float *bi
                        int N, int H, int W, int Cin, int Cout, int KS, int stride, int pad, int dil,
                        int relu, int precision, int transposed2x, int y_channel_stride, int y_channel_offset,
                        int rows_per_warp, void *stream);
+/* The launch plan pmb200_conv2d_nhwc uses for a layer on a device of `sms` SMs (H, W: the input as the conv sees it, i.e.
+ * 2H x 2W for the transposed2x form): plan[0] warp groups sharing a halo tile (1 or 2), plan[1] output rows per warp (1, 2
+ * or 4), plan[2] halo buffers (1, or 2 when each CTA prefetches its next tile), plan[3] CTAs launched, plan[4] dynamic
+ * shared-memory bytes.  Non-zero when the halo tile does not fit in shared memory. */
+int pmb200_conv2d_nhwc_plan(int N, int H, int W, int Cin, int Cout, int KS, int stride, int pad, int dil, int rows_per_warp, int sms,
+                            int *plan);
 
 /* One source view of a ragged pack (the *_views entry points): the view's first float is src_flat + offset, and batch item b
  * of it is [height, width(, C)] row-major starting at src_flat + offset + b * height * width (* C). */

@@ -139,6 +139,7 @@ _SIGNATURES = {
     "pmb200_upsample2x_add_nhwc": (c_int, [c_void_p] * 4 + [c_int] * 4 + [c_void_p]),
     "pmb200_conv2d_filter_floats": (c_int, [c_int] * 4),
     "pmb200_conv2d_nhwc": (c_int, [c_void_p] * 5 + [c_int] * 15 + [c_void_p]),
+    "pmb200_conv2d_nhwc_plan": (c_int, [c_int] * 11 + [POINTER(c_int)]),
     "pmb200_conv2d_tc5_supported": (c_int, [c_int] * 4),
     "pmb200_conv2d_tc5_filter_floats": (c_int, [c_int] * 3),
     "pmb200_conv2d_tc5": (c_int, [c_void_p] * 4 + [c_int] * 12 + [c_void_p]),

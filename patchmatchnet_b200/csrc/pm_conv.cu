@@ -571,6 +571,69 @@ inline int effective_mt(int nt, int nsplit, int mt) {
     return 1;
 }
 
+struct NhwcPlan {
+    int nsplit, ntw, mt, nbuf, ctas;
+    int tiles_y, rh, buf_floats, total_tiles;
+    size_t smem;
+};
+
+// Work decomposition of one launch over an Ho x Wo output (Hv x Wv the input as the conv sees it: zero-stuffed for the
+// transposed form).  8 (and, when the map is small, 4) output-channel tiles are split over two warp groups that share one
+// halo tile: twice the warps per tile for the layers with few pixels and many channels.  Rows per warp: as many as the
+// accumulator budget allows while there are still several tiles per SM; two halo buffers (prefetch of the CTA's next tile)
+// only when a CTA will see more than ~2 tiles anyway.  Non-zero when the halo tile does not fit in shared memory.
+int plan_nhwc(int N, int Ho, int Wo, int Cin, int Cout, int KS, int stride, int dil, int rows_per_warp, int sms, NhwcPlan &q) {
+    const int nt = round_nt(Cout), ps = pixel_stride(round_kcin(Cin), stride);
+    const int tiles_x = (Wo + 15) / 16, rw = 15 * stride + dil * (KS - 1) + 1;
+    const long px_tiles16x8 = (long)tiles_x * ((Ho + 7) / 8) * N;
+    q.nsplit = 1;
+    q.ntw = nt;
+    if (nt == 8 || (nt == 4 && px_tiles16x8 < 8L * sms)) {
+        q.nsplit = 2;
+        q.ntw = nt / 2;
+    }
+    if (rows_per_warp < 0) {  // negative: force rows_per_warp = -value with ONE warp group (measurement aid)
+        q.nsplit = 1;
+        q.ntw = nt;
+        rows_per_warp = -rows_per_warp;
+    }
+    int mt = rows_per_warp > 0 ? rows_per_warp : 4;
+    for (;;) {
+        mt = effective_mt(q.ntw, q.nsplit, mt);
+        const int rows = 4 * mt;
+        q.tiles_y = (Ho + rows - 1) / rows;
+        q.rh = (rows - 1) * stride + dil * (KS - 1) + 1;
+        q.buf_floats = ((q.rh * rw * ps + 3) / 4) * 4;
+        const size_t one = (size_t)q.buf_floats * sizeof(float);
+        const long tiles = (long)tiles_x * q.tiles_y * N;
+        const bool fits = one <= 200 * 1024;
+        const bool enough = rows_per_warp > 0 || tiles >= 6L * sms || mt == 1;
+        const bool roomy = rows_per_warp > 0 || one <= 56 * 1024 || mt == 1;  // >= 4 single-buffered CTAs per SM
+        if (fits && enough && roomy) {
+            q.mt = mt;
+            q.total_tiles = (int)tiles;
+            const long reg_cap = q.nsplit == 2 ? 3 : 5;  // resident CTAs per SM the register file allows (<= ~100 regs/thread)
+            long cap1 = (long)(224 * 1024) / (long)(one + 1024);
+            if (cap1 > reg_cap) cap1 = reg_cap;
+            if (cap1 < 1) cap1 = 1;
+            long cap2 = (long)(224 * 1024) / (long)(2 * one + 1024);
+            if (cap2 > reg_cap) cap2 = reg_cap;
+            if (tiles > 2 * cap1 * sms && cap2 >= 1 && 2 * one <= 200 * 1024) {
+                q.nbuf = 2;
+                q.smem = 2 * one;
+                q.ctas = (int)(cap2 * sms < tiles ? cap2 * sms : tiles);
+            } else {
+                q.nbuf = 1;
+                q.smem = one;
+                q.ctas = (int)(cap1 * sms < tiles ? cap1 * sms : tiles);
+            }
+            return 0;
+        }
+        if (mt == 1) return conv_fail(PMB200_EINVAL, "conv2d_nhwc: halo tile does not fit in shared memory (dilation too large)");
+        mt /= 2;
+    }
+}
+
 }  // namespace
 
 extern "C" {
@@ -578,6 +641,24 @@ extern "C" {
 int pmb200_conv2d_filter_floats(int Cin, int Cout, int KS, int precision) {
     if (Cin < 1 || Cin > 64 || Cout < 1 || Cout > 64 || KS < 1 || (precision != 1 && precision != 3)) return PMB200_EINVAL;
     return KS * KS * (round_kcin(Cin) / 8) * round_nt(Cout) * 32 * (precision == 1 ? 2 : 4);
+}
+
+int pmb200_conv2d_nhwc_plan(int N, int H, int W, int Cin, int Cout, int KS, int stride, int pad, int dil, int rows_per_warp, int sms,
+                            int *plan) {
+    if (!plan || N < 1 || H < 1 || W < 1 || Cin < 1 || Cout < 1 || Cin > 64 || Cout > 64 || KS < 1 || KS > 7 || stride < 1 || stride > 2 ||
+        dil < 1 || pad < 0 || sms < 1)
+        return conv_fail(PMB200_EINVAL, "conv2d_nhwc_plan: bad size");
+    const int Ho = (H + 2 * pad - dil * (KS - 1) - 1) / stride + 1;
+    const int Wo = (W + 2 * pad - dil * (KS - 1) - 1) / stride + 1;
+    if (Ho < 1 || Wo < 1) return conv_fail(PMB200_EINVAL, "conv2d_nhwc_plan: empty output");
+    NhwcPlan q;
+    if (const int rc = plan_nhwc(N, Ho, Wo, Cin, Cout, KS, stride, dil, rows_per_warp, sms, q)) return rc;
+    plan[0] = q.nsplit;
+    plan[1] = q.mt;
+    plan[2] = q.nbuf;
+    plan[3] = q.ctas;
+    plan[4] = (int)q.smem;
+    return 0;
 }
 
 int pmb200_conv2d_nhwc(const float *x, const float *filter_frag, const float *bias, const float *add_up2x, float *y, int N,
@@ -607,7 +688,7 @@ int pmb200_conv2d_nhwc(const float *x, const float *filter_frag, const float *bi
         if ((Ho & 1) || (Wo & 1) || (Cout & 1)) return conv_fail(PMB200_EINVAL, "conv2d_nhwc: add_up2x needs even Ho, Wo and Cout");
         if (reinterpret_cast<uintptr_t>(add_up2x) & 7u) return conv_fail(PMB200_EINVAL, "conv2d_nhwc: add_up2x must be 8-byte aligned");
     }
-    const int kcin = round_kcin(Cin), nt = round_nt(Cout);
+    const int kcin = round_kcin(Cin);
     ConvParams p;
     p.up = add_up2x;
     p.x = x; p.wf = filter_frag; p.bias = bias; p.y = y;
@@ -622,61 +703,18 @@ int pmb200_conv2d_nhwc(const float *x, const float *filter_frag, const float *bi
     for (int sft = 0; sft < 7; ++sft)
         if ((1 << sft) == p.cpp) p.cpp_shift = sft;
 
-    // Work decomposition.  8 (and, when the map is small, 4) output-channel tiles are split over two warp groups that
-    // share one halo tile: twice the warps per tile for the layers with few pixels and many channels.
     int dev = 0;
     cudaGetDevice(&dev);
-    const int sms = sm_count(dev);
-    const long px_tiles16x8 = (long)p.tiles_x * ((Ho + 7) / 8) * N;
-    int nsplit = 1, ntw = nt;
-    if (nt == 8 || (nt == 4 && px_tiles16x8 < 8L * sms)) {
-        nsplit = 2;
-        ntw = nt / 2;
-    }
-    if (rows_per_warp < 0) {  // negative: force rows_per_warp = -value with ONE warp group (measurement aid)
-        nsplit = 1;
-        ntw = nt;
-        rows_per_warp = -rows_per_warp;
-    }
-    p.nt_total = nt;
-
-    // rows per warp: as many as the accumulator budget allows while there are still several tiles per SM; two halo
-    // buffers (prefetch of the CTA's next tile) only when a CTA will see more than ~2 tiles anyway
-    int mt = rows_per_warp > 0 ? rows_per_warp : 4;
-    LaunchPlan plan{0, 0};
-    for (;;) {
-        mt = effective_mt(ntw, nsplit, mt);
-        const int rows = 4 * mt;
-        p.tiles_y = (Ho + rows - 1) / rows;
-        p.rh = (rows - 1) * stride + dil * (KS - 1) + 1;
-        p.buf_floats = ((p.rh * p.rw * p.ps + 3) / 4) * 4;
-        const size_t one = (size_t)p.buf_floats * sizeof(float);
-        const long tiles = (long)p.tiles_x * p.tiles_y * N;
-        const bool fits = one <= 200 * 1024;
-        const bool enough = rows_per_warp > 0 || tiles >= 6L * sms || mt == 1;
-        const bool roomy = rows_per_warp > 0 || one <= 56 * 1024 || mt == 1;  // >= 4 single-buffered CTAs per SM
-        if (fits && enough && roomy) {
-            p.total_tiles = (int)tiles;
-            const long reg_cap = nsplit == 2 ? 3 : 5;  // resident CTAs per SM the register file allows (<= ~100 regs/thread)
-            long cap1 = (long)(224 * 1024) / (long)(one + 1024);
-            if (cap1 > reg_cap) cap1 = reg_cap;
-            if (cap1 < 1) cap1 = 1;
-            long cap2 = (long)(224 * 1024) / (long)(2 * one + 1024);
-            if (cap2 > reg_cap) cap2 = reg_cap;
-            if (tiles > 2 * cap1 * sms && cap2 >= 1 && 2 * one <= 200 * 1024) {
-                p.nbuf = 2;
-                plan.smem = 2 * one;
-                plan.ctas = (int)(cap2 * sms < tiles ? cap2 * sms : tiles);
-            } else {
-                p.nbuf = 1;
-                plan.smem = one;
-                plan.ctas = (int)(cap1 * sms < tiles ? cap1 * sms : tiles);
-            }
-            break;
-        }
-        if (mt == 1) return conv_fail(PMB200_EINVAL, "conv2d_nhwc: halo tile does not fit in shared memory (dilation too large)");
-        mt /= 2;
-    }
+    NhwcPlan q;
+    if (const int rc = plan_nhwc(N, Ho, Wo, Cin, Cout, KS, stride, dil, rows_per_warp, sm_count(dev), q)) return rc;
+    p.nt_total = round_nt(Cout);
+    p.tiles_y = q.tiles_y;
+    p.rh = q.rh;
+    p.buf_floats = q.buf_floats;
+    p.total_tiles = q.total_tiles;
+    p.nbuf = q.nbuf;
+    const LaunchPlan plan{q.smem, q.ctas};
+    const int ntw = q.ntw, nsplit = q.nsplit, mt = q.mt;
     p.row_chunks = p.rw * p.cpp;
     p.tile_chunks = p.rh * p.row_chunks;
     p.magic_row = (unsigned)((1ull << 32) / (unsigned)p.row_chunks + 1ull);
