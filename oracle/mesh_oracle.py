@@ -6,6 +6,7 @@ from __future__ import annotations
 
 import os
 import re
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
@@ -113,11 +114,14 @@ def marching_cubes(keys, s: float, tsdf, weight, colour, min_weight: int = 1, ta
     colour = np.asarray(colour)[:, :3]
 
     def lookup(c):
-        """voxel indices of coordinates [m,3] -> global index or -1"""
-        k = block_key(c >> 3)
+        """voxel indices of coordinates [m,3] -> global index or -1 (a block outside the key range would alias another
+        key: its coordinate field overflows into the next one)"""
+        b = c >> 3
+        inside = ((b >= -KEY_BIAS) & (b < KEY_BIAS)).all(-1)
+        k = block_key(np.where(inside[:, None], b, 0))
         pos = np.searchsorted(keys, k)
         posc = np.minimum(pos, len(keys) - 1)
-        hit = (pos < len(keys)) & (keys[posc] == k)
+        hit = inside & (pos < len(keys)) & (keys[posc] == k)
         local = (c[:, 0] & 7) + 8 * (c[:, 1] & 7) + 64 * (c[:, 2] & 7)
         return np.where(hit, posc * 512 + local, -1)
 
@@ -173,6 +177,163 @@ def marching_cubes(keys, s: float, tsdf, weight, colour, min_weight: int = 1, ta
     faces = tri[tri[:, 0] != -2]
     assert (faces >= 0).all(), "a meshed cube refers to an edge without a vertex"
     return pos, col, faces.astype(np.int32)
+
+
+# ---- chunked forms: any subset of a large volume, memory linear in the chunk ------------------------------------------------
+
+def integrate_blocks(keys, s: float, trunc: int, depths, images, Ks, Es, chunk: int = 256):
+    """integrate() of the blocks `keys` (any subset of a volume's keys, in any order), `chunk` blocks at a time: every voxel's
+    sums depend on that voxel alone, so the result is integrate(keys, ...) bit for bit."""
+    keys = np.asarray(keys, np.uint64)
+    parts = [integrate(keys[i : i + chunk], s, trunc, depths, images, Ks, Es) for i in range(0, len(keys), chunk)]
+    if not parts:
+        return np.zeros(0, np.float32), np.zeros(0, np.float32), np.zeros((0, 3), np.uint8)
+    return tuple(np.concatenate(p) for p in zip(*parts))
+
+
+# neighbour n of a block at offset NEIGHBOURS[n] = (dx, dy, dz), n = (dx + 1) + 3 (dy + 1) + 9 (dz + 1)
+NEIGHBOURS = np.array([(dx, dy, dz) for dz in (-1, 0, 1) for dy in (-1, 0, 1) for dx in (-1, 0, 1)], dtype=np.int64)
+_TILE = np.arange(-1, 9)  # voxel coordinates -1..8 of a block's tile along one axis
+
+
+def neighbour_blocks(keys: np.ndarray, blocks: np.ndarray) -> np.ndarray:
+    """[len(blocks), 27] indices into the sorted `keys` of the neighbours of blocks keys[blocks], -1 where a neighbour is not
+    allocated or lies outside the key range."""
+    c = key_blocks(keys[blocks])[:, None, :] + NEIGHBOURS
+    inside = ((c >= -KEY_BIAS) & (c < KEY_BIAS)).all(-1)
+    k = block_key(np.where(inside[..., None], c, 0))
+    pos = np.minimum(np.searchsorted(keys, k), len(keys) - 1)
+    return np.where(inside & (keys[pos] == k), pos, -1)
+
+
+def _tiles(keys, blocks, tsdf, valid):
+    """Per block the voxels -1..8 along each axis, [B,10,10,10] indexed [z,y,x]: (global voxel index or -1, tsdf with NaN
+    where the voxel is not valid), and the neighbour table."""
+    nb = neighbour_blocks(keys, blocks)
+    n = (_TILE >> 3) + 1
+    local = _TILE & 7
+    tb = nb[:, (9 * n)[:, None, None] + (3 * n)[None, :, None] + n[None, None, :]]
+    g = np.where(tb >= 0, tb * 512 + (64 * local[:, None, None] + 8 * local[None, :, None] + local[None, None, :]), -1)
+    ok = g >= 0
+    ok[ok] = valid[g[ok]]
+    return g, np.where(ok, tsdf[np.maximum(g, 0)], np.float32(np.nan)), nb
+
+
+def _owned_and_cases(t):
+    """tsdf tiles [B,10,10,10] -> (owned [B,8,8,8,3]: the voxel's edge along x / y / z has a vertex, case int16 [B,9,9,9] of
+    the cubes with minimum corner -1..7, -1 unless the cube is meshed)."""
+    valid, neg = ~np.isnan(t), t < 0
+    allv = np.ones(t.shape[:1] + (9, 9, 9), bool)
+    case = np.zeros(t.shape[:1] + (9, 9, 9), np.int16)
+    for c, (ox, oy, oz) in enumerate(CORNERS):
+        allv &= valid[:, oz : oz + 9, oy : oy + 9, ox : ox + 9]
+        case |= neg[:, oz : oz + 9, oy : oy + 9, ox : ox + 9].astype(np.int16) << c
+    meshed = allv & (case != 0) & (case != 255)
+    owned = np.zeros(t.shape[:1] + (8, 8, 8, 3), bool)
+    a_valid, a_neg = valid[:, 1:9, 1:9, 1:9], neg[:, 1:9, 1:9, 1:9]
+    for k in range(3):
+        ux, uy, uz = UNIT[k]
+        b = (slice(None), slice(1 + uz, 9 + uz), slice(1 + uy, 9 + uy), slice(1 + ux, 9 + ux))
+        any_meshed = np.zeros_like(a_valid)
+        j, l = [a for a in range(3) if a != k]
+        for dj in (0, 1):
+            for dl in (0, 1):
+                dx, dy, dz = dj * UNIT[j] + dl * UNIT[l]
+                any_meshed |= meshed[:, 1 - dz : 9 - dz, 1 - dy : 9 - dy, 1 - dx : 9 - dx]
+        owned[..., k] = a_valid & valid[b] & (a_neg != neg[b]) & any_meshed
+    return owned, np.where(meshed, case, np.int16(-1))
+
+
+def _map_chunks(fn, blocks, chunk):
+    """[fn(part) for each chunk of blocks], the chunks on a thread pool (numpy releases the GIL in its array loops)."""
+    parts = [blocks[i : i + chunk] for i in range(0, len(blocks), chunk)]
+    with ThreadPoolExecutor(max_workers=min(len(parts), os.cpu_count() or 1) or 1) as ex:
+        return list(ex.map(fn, parts))
+
+
+def marching_cubes_blocks(keys, s: float, tsdf, weight, colour, emit, min_weight: int = 1, table=None, chunk: int = 1024):
+    """marching_cubes() restricted to the blocks keys[emit] (emit: increasing block indices): the vertices those blocks' voxels
+    own and the faces of their cubes, with the global vertex numbering of the whole volume.  A count pass over every block
+    and a prefix sum give each block's first vertex and face; each block reads its 26 neighbours from the full key array
+    and its voxels -1..8 along each axis; the faces of an emitted block read the vertex numbering of its neighbours.  Work
+    goes `chunk` blocks at a time.  -> (positions float32 [m,3], colours uint8 [m,3], faces int32 [f,3], the vertices' global
+    indices int64 [m], the faces' global indices int64 [f]).  Over emit = every block this is marching_cubes()."""
+    tab = read_table() if table is None else table
+    ntri = (tab[:, ::3] >= 0).sum(1)
+    ntri[[0, 255]] = 0
+    keys = np.asarray(keys, np.uint64)
+    tsdf = np.asarray(tsdf, np.float32)
+    valid = np.asarray(weight) >= min_weight
+    colour = np.asarray(colour)[:, :3]
+    emit = np.asarray(emit, np.int64)
+    assert (np.diff(emit) > 0).all()
+
+    def owned_of(blocks):
+        return _owned_and_cases(_tiles(keys, blocks, tsdf, valid)[1])[0].reshape(len(blocks), 1536)
+
+    def counts(blocks):
+        owned, case = _owned_and_cases(_tiles(keys, blocks, tsdf, valid)[1])
+        c = case[:, 1:, 1:, 1:].reshape(len(blocks), -1)
+        return owned.reshape(len(blocks), -1).sum(1), np.where(c >= 0, ntri[np.maximum(c, 0)], 0).sum(1)
+
+    cnt = _map_chunks(counts, np.arange(len(keys)), chunk)
+    nv = np.concatenate([c[0] for c in cnt]) if cnt else np.zeros(0, np.int64)
+    nf = np.concatenate([c[1] for c in cnt]) if cnt else np.zeros(0, np.int64)
+    vbase = np.concatenate([[0], np.cumsum(nv)])
+    fbase = np.concatenate([[0], np.cumsum(nf)])
+
+    def emit_chunk(blocks):
+        B = len(blocks)
+        g, t, nb = _tiles(keys, blocks, tsdf, valid)
+        owned, case = _owned_and_cases(t)
+        # vertices: block, voxel (x fastest), axis
+        bi, z, y, x, k = np.nonzero(owned)
+        ga = g[bi, z + 1, y + 1, x + 1]
+        gb = g[bi, z + 1 + UNIT[k, 2], y + 1 + UNIT[k, 1], x + 1 + UNIT[k, 0]]
+        ia = key_blocks(keys[blocks[bi]]) * 8 + np.stack([x, y, z], -1)
+        Xa = (ia.astype(np.float64) + 0.5) * s
+        Xb = ((ia + UNIT[k]).astype(np.float64) + 0.5) * s
+        ta, tb = tsdf[ga].astype(np.float64), tsdf[gb].astype(np.float64)
+        tt = ta / (ta - tb)
+        pos = (Xa + tt[:, None] * (Xb - Xa)).astype(np.float32)
+        cA, cB = colour[ga].astype(np.float64), colour[gb].astype(np.float64)
+        col = np.clip(np.rint(cA + tt[:, None] * (cB - cA)), 0, 255).astype(np.uint8)
+        vid = vbase[blocks[bi]] + np.cumsum(owned.reshape(B, -1), 1)[bi, 3 * (x + 8 * y + 64 * z) + k] - 1
+        # the owned edges of these blocks and their neighbours, and their exclusive prefix per block
+        near = np.unique(nb[nb >= 0])
+        own = np.zeros((len(near), 1536), bool)
+        own[np.searchsorted(near, blocks)] = owned.reshape(B, -1)
+        rest = np.setdiff1d(near, blocks)
+        if len(rest):
+            own[np.searchsorted(near, rest)] = owned_of(rest)
+        pre = np.cumsum(own, 1) - 1
+        # faces: cube (the voxel's order), then table order
+        cb, cz, cy, cx = np.nonzero(case[:, 1:, 1:, 1:] >= 0)
+        rows = tab[case[cb, cz + 1, cy + 1, cx + 1]].astype(np.int64)
+        tri = np.full((len(cb), 5, 3), -2, np.int64)
+        for q in range(5):
+            e = rows[:, 3 * q : 3 * q + 3]
+            has = e[:, 0] >= 0
+            ee = np.maximum(e, 0)
+            w = np.stack([cx, cy, cz], -1)[:, None, :] + EDGE_OFFSET[ee]  # [m, 3 vertices, xyz], each in 0..8
+            n = (w >> 3) + 1
+            blk = nb[cb[:, None], n[..., 0] + 3 * n[..., 1] + 9 * n[..., 2]]
+            lw = w & 7
+            slot = 3 * (lw[..., 0] + 8 * lw[..., 1] + 64 * lw[..., 2]) + EDGE_AXIS[ee]
+            r = np.searchsorted(near, blk)
+            assert own[r[has], slot[has]].all(), "a meshed cube refers to an edge without a vertex"
+            tri[:, q] = np.where(has[:, None], vbase[blk] + pre[r, slot], -2)
+        tri = tri.reshape(-1, 3)
+        faces = tri[tri[:, 0] != -2]
+        fid = np.repeat(fbase[blocks], nf[blocks]) + (np.arange(int(nf[blocks].sum())) - np.repeat(np.cumsum(nf[blocks]) - nf[blocks], nf[blocks]))
+        assert len(fid) == len(faces)
+        return pos, col, faces.astype(np.int32), vid, fid
+
+    out = _map_chunks(emit_chunk, emit, chunk)
+    if not out:
+        return (np.zeros((0, 3), np.float32), np.zeros((0, 3), np.uint8), np.zeros((0, 3), np.int32), np.zeros(0, np.int64),
+                np.zeros(0, np.int64))
+    return tuple(np.concatenate(p) for p in zip(*out))
 
 
 def mesh(points, depths, images, Ks, Es, s: float, trunc: int = 3, min_weight: int = 1):
