@@ -339,6 +339,64 @@ int pmb200_tsdf_mesh_write(const uint64_t *block_keys, int64_t n_blocks, double 
                            int *faces_out, void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------
+ * Mesh simplification: Garland-Heckbert quadric edge collapse in rounds of independent collapses, with removal of small
+ * components (beyond the reference; INTEGRATION.md "Mesh simplification (beyond the reference)").  Definition:
+ *
+ * Arithmetic.  float64, each operation rounded on its own (no fused multiply-add), in the order csrc/pm_simplify_math.cuh
+ * writes it; `/` and sqrt are IEEE.  Positions stay float64 between rounds and are rounded to float32 once, at output.  No
+ * floating-point atomics: reruns give the same bits.  Constants (pm_simplify_math.cuh): W = 1, kDetRel = 1e-9, kFarEdges = 1,
+ * kFlatRel = 1e-9, kMaxValence = 32.
+ * Input.  xyz float32 [nv,3], rgb uint8 [nv,3] or NULL (then colours are 0), faces int32 [nf,3]; nv < 2^31 - 1, nf < 2^29.
+ * Faces with an index outside 0..nv-1 or a repeated index are dropped.  Vertices are not welded; zero-area faces with
+ * distinct indices are kept.
+ * Components (min_component_faces F > 0).  Faces joined through shared vertices; a component's label is its smallest vertex
+ * index (min-label propagation with hooking and pointer jumping, one host read per pass); faces of components with fewer
+ * than F faces are removed, the others keep their order.
+ * Topology of a round, from the current faces: the undirected edges (a < b) sorted by (a, b), each with its face count; a
+ * border edge has 1 face, a non-manifold edge more than 2; a border vertex lies on a border edge; a vertex is locked when it
+ * lies on a non-manifold edge or has more than kMaxValence incident faces.
+ * Quadrics, once, after component removal: 10 float64 entries per vertex (xx xy xz xd yy yz yd zz zd dd of p p^T).  A face
+ * X0 X1 X2 with n = (X1 - X0) x (X2 - X0) (components (a1 b2 - a2 b1, a2 b0 - a0 b2, a0 b1 - a1 b0), dot products
+ * ((x0 y0 + x1 y1) + x2 y2)) adds A (p_i p_j), A = |n| / 2, p = (n / |n|, -(n / |n|) . X0); a border edge (a, b) with its face
+ * adds W |e|^2 (p_i p_j) with e = Xb - Xa, m = e x n, p = (m / |m|, -(m / |m|) . Xa).  A plane with |n| or |m| = 0 adds
+ * nothing.  Per vertex the sum runs over the incident faces by ascending index, then its border edges by ascending key.
+ * Candidate (a, b).  Valid when neither endpoint is locked; it is not an interior edge (2 faces) with two border endpoints;
+ * every common neighbour of a and b is an opposite vertex of the edge, and no face a-x-y has a twin b-x-y (the link
+ * condition of Dey et al.); and, with v placed, no face of the star of a without b (of b without a) whose normal is non-zero
+ * gets new . old <= 0 when a (b) moves to v.
+ * Placement.  Q = Q_a + Q_b, A its 3x3 part, g = A Xa + (xd, yd, zd).  When |det A| > kDetRel s^3 (s the largest |diagonal|,
+ * det by cofactors ((q0 c00 + q1 c01) + q2 c02)) and |e| > 0, w = Xa - adj(A) g / det; w is taken when its distance to the
+ * segment is at most kFarEdges |e|.  Otherwise v = Xa + t e with t = clamp(-(e.g) / (e.A e), 0, 1), or t = 1/2 when
+ * e.A e <= kFlatRel trace(A) |e|^2.  Colour: rint(c_a + t' (c_b - c_a)) (half to even), t' = clamp(((v - Xa).e) / |e|^2, 0, 1).
+ * Cost vT Q v (>= 0); key = float32_bits(cost) << 32 | edge index in this round's sorted edge list.
+ * Selection.  m(v) = min key over the valid edges at v (64-bit atomicMin), M(v) = min of m over v and its neighbours; (a, b)
+ * is selected when key = M(a) = M(b).  Two selected edges (a, b) and (c, d) have no adjacent endpoints: if c were a
+ * neighbour of a, M(c) <= m(a) = key_ab and M(a) <= m(c) = key_cd would force key_ab = key_cd, the same edge.  So their stars
+ * share no face, neither collapse reads a position, quadric or adjacency the other writes, and applying them together
+ * equals applying them one after another in any order.  The globally cheapest valid edge is always selected.
+ * Target.  An interior collapse removes 2 faces, a border collapse 1.  When collapsing every selected edge would leave fewer
+ * than target_faces faces, only the shortest prefix in ascending key order that reaches nf <= target_faces is applied.  The
+ * rounds stop when nf <= target_faces or when no edge is valid (the face count reached is reported; not an error).
+ * Apply.  The lower index a survives with v, its colour and Q_a + Q_b; references to b become a; faces with both go; the
+ * others keep their relative order.
+ * Output.  The vertices some face references, in ascending original index; faces remapped.
+ *
+ * pmb200_simplify_mesh: the whole simplification into the workspace (pmb200_simplify_mesh_workspace_bytes(nv, nf) bytes,
+ *   about 157 bytes per vertex and 205 per face); counts_host (HOST) receives the vertex and face counts of the result and
+ *   the number of rounds.  Host synchronisations: one after the input filter, one per component pass, and one per round
+ *   (the selected count and the faces it removes; a second in the round where the target bites), one for the vertex count.
+ * pmb200_simplify_mesh_write: with the same workspace and sizes, after that call: xyz_out float32 [nv',3], rgb_out uint8
+ *   [nv',3] (may be NULL), faces_out int32 [nf',3].  Enqueue only.
+ * PMB200_EINVAL, nothing launched, for a null pointer, sizes out of range, target_faces or min_component_faces < 0, or a
+ * workspace smaller than the query. */
+int64_t pmb200_simplify_mesh_workspace_bytes(int64_t n_vertices, int64_t n_faces);
+int pmb200_simplify_mesh(const float *xyz, const unsigned char *rgb, int64_t n_vertices, const int *faces, int64_t n_faces,
+                         int64_t target_faces, int64_t min_component_faces, int64_t *counts_host, void *workspace,
+                         int64_t workspace_bytes, void *stream);
+int pmb200_simplify_mesh_write(int64_t n_vertices, int64_t n_faces, int64_t n_faces_out, float *xyz_out, unsigned char *rgb_out,
+                               int *faces_out, void *workspace, int64_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------
  * Rendering of point clouds and triangle meshes (beyond the reference, whose only viewer is an Open3D window; INTEGRATION.md
  * "Rendering (beyond the reference)").  This project's own definition, float32 throughout, every product, sum and
  * difference rounded on its own (no fused multiply-add); `/` and sqrt are IEEE.  Reruns give the same bits.

@@ -246,7 +246,8 @@ def save_ply(path: str, body, faces=None) -> None:
     little endian, one `vertex` element with float x, y, z and uchar red, green, blue) from vertex records produced by
     ops.fuse_points: uint8 [n,15] tensor(s) (a list concatenates the per-reference-view clouds, eval.py:283-284).
     Oriented records, uint8 [n,27] (ops.fuse_points with normals), write float nx, ny, nz between z and red, the property
-    order of COLMAP's fused.ply; every part of one file has the same record size.
+    order of COLMAP's fused.ply; every part of one file has the same record size.  Records of uint8 [n,12] (ops.simplify_mesh
+    without colours) hold float x, y, z alone.
     With `faces`, int32 [nf,3] vertex indices (ops.tsdf_mesh), a `face` element (property list uchar int vertex_indices)
     follows the vertices; without it the file is the vertex element alone."""
     import torch
@@ -255,8 +256,8 @@ def save_ply(path: str, body, faces=None) -> None:
     parts = [b.detach().cpu().contiguous() for b in parts]
     width = int(parts[0].shape[1]) if parts and parts[0].dim() == 2 else 15
     for b in parts:
-        if b.dtype != torch.uint8 or b.dim() != 2 or b.shape[1] not in (15, 27) or b.shape[1] != width:
-            raise ValueError("save_ply: vertex records must be uint8 [n,15] or [n,27] tensors of one size (ops.fuse_points)")
+        if b.dtype != torch.uint8 or b.dim() != 2 or b.shape[1] not in (12, 15, 27) or b.shape[1] != width:
+            raise ValueError("save_ply: vertex records must be uint8 [n,15], [n,27] or [n,12] tensors of one size (ops.fuse_points)")
     n = sum(int(b.shape[0]) for b in parts)
     normals = "property float nx\nproperty float ny\nproperty float nz\n" if width == 27 else ""
     face_rows = None
@@ -270,8 +271,9 @@ def save_ply(path: str, body, faces=None) -> None:
         face_rows["n"] = 3
         face_rows["v"] = fc.numpy()
     face_header = "element face %d\nproperty list uchar int vertex_indices\n" % face_rows.shape[0] if face_rows is not None else ""
+    colours = "" if width == 12 else "property uchar red\nproperty uchar green\nproperty uchar blue\n"
     header = ("ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\nproperty float z\n"
-              "%sproperty uchar red\nproperty uchar green\nproperty uchar blue\n%send_header\n" % (n, normals, face_header))
+              "%s%s%send_header\n" % (n, normals, colours, face_header))
     with open(path, "wb") as f:
         f.write(header.encode("ascii"))
         for b in parts:

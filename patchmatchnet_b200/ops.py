@@ -1198,6 +1198,79 @@ def tsdf_mesh(points: Tensor, depths: Sequence[Tensor], images: Sequence[Tensor]
     return tsdf_extract(keys, tsdf, weight, colour, voxel_size, min_weight)
 
 
+def simplify_mesh_bytes(n_vertices: int, n_faces: int) -> int:
+    """Device memory ops.simplify_mesh needs beyond its inputs: the workspace (pmb200_simplify_mesh_workspace_bytes: about
+    157 bytes per vertex for positions, quadrics, per-round vertex state and the selection, and 205 per face for two face
+    lists, the edge and vertex-face keys and the radix sort's alternate key buffer) plus at most 15 bytes per vertex and 12
+    per face of output.  Needs a CUDA device (the size of the CUB passes' storage)."""
+    lib = _native.lib()
+    ws = lib.pmb200_simplify_mesh_workspace_bytes(n_vertices, n_faces)
+    if ws < 0:
+        _native.check(int(ws), "simplify_mesh_workspace_bytes")
+    return int(ws) + 15 * n_vertices + 12 * n_faces
+
+
+def simplify_mesh(xyz: Tensor, rgb: Optional[Tensor], faces: Tensor, target_faces: int, min_component_faces: int = 0
+                  ) -> Tuple[Tensor, Tensor, int]:
+    """Quadric edge-collapse simplification to at most target_faces faces, in rounds of independent collapses, after removing
+    components with fewer than min_component_faces faces (0: none removed).  Definition in include/patchmatch_b200.h.
+    xyz CUDA float32 [nv,3]; rgb uint8 [nv,3] or None; faces int32 [nf,3].  -> (vertex records uint8 [n,15], the layout of
+    mesh.ply, or [n,12] (x, y, z only) when rgb is None; faces int32 [nf',3]; the number of rounds) on the device.  When no
+    collapse is valid any more the result has more than target_faces faces.  Reruns give the same bits.
+
+    ValueError before any launch on bad arguments (a face index outside 0..nv-1 included), and before allocating when
+    simplify_mesh_bytes(nv, nf) exceeds the device's free memory.  One host read per round."""
+    import ctypes
+
+    what = "simplify_mesh"
+    pts = _render_xyz(xyz, what)
+    nv = pts.shape[0]
+    if not isinstance(faces, Tensor) or not _on_device(faces) or faces.dtype != torch.int32 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError(f"{what}: faces must be a CUDA int32 [nf,3] tensor")
+    if faces.device != pts.device:
+        raise ValueError(f"{what}: faces must be on the vertices' device")
+    for name, v in (("target_faces", target_faces), ("min_component_faces", min_component_faces)):
+        if isinstance(v, bool) or not isinstance(v, int) or v < 0:
+            raise ValueError(f"{what}: {name} must be an int >= 0, got {v!r}")
+    fc = faces.contiguous()
+    nf = fc.shape[0]
+    if nv >= 2 ** 31 - 1 or nf >= 2 ** 29:
+        raise ValueError(f"{what}: at most 2^31 - 2 vertices and 2^29 - 1 faces, got {nv} and {nf}")
+    col = _render_attr(rgb, nv, torch.uint8, pts.device, "rgb", what)
+    if nf:
+        lo, hi = (int(v) for v in torch.aminmax(fc))
+        if lo < 0 or hi >= nv:
+            raise ValueError(f"{what}: a face refers to a vertex outside 0..{nv - 1}")
+    width = 12 if col is None else 15
+    if nv == 0 or nf == 0:
+        return torch.empty((0, width), dtype=torch.uint8, device=pts.device), torch.empty((0, 3), dtype=torch.int32, device=pts.device), 0
+    lib = _native.lib()
+    need = simplify_mesh_bytes(nv, nf)
+    with _device_guard(pts):
+        free = torch.cuda.mem_get_info(pts.device)[0] + torch.cuda.memory_reserved(pts.device) - torch.cuda.memory_allocated(pts.device)
+    if need > free:
+        raise ValueError(f"{what}: {nv} vertices and {nf} faces need {need / 2 ** 30:.2f} GiB ({free / 2 ** 30:.2f} GiB free)")
+    ws_bytes = lib.pmb200_simplify_mesh_workspace_bytes(nv, nf)
+    ws = _workspace(ws_bytes, "simplify_mesh_workspace_bytes", pts.device)
+    counts = (ctypes.c_int64 * 3)()
+    with _device_guard(pts):
+        rc = lib.pmb200_simplify_mesh(pts.data_ptr(), None if col is None else col.data_ptr(), nv, fc.data_ptr(), nf, target_faces,
+                                      min_component_faces, counts, ws.data_ptr(), int(ws_bytes), _stream(pts))
+    _native.check(rc, what)
+    nv_out, nf_out, rounds = (int(c) for c in counts)
+    out_xyz = torch.empty((nv_out, 3), dtype=torch.float32, device=pts.device)
+    out_rgb = None if col is None else torch.empty((nv_out, 3), dtype=torch.uint8, device=pts.device)
+    out_faces = torch.empty((nf_out, 3), dtype=torch.int32, device=pts.device)
+    if nf_out == 0:
+        return torch.empty((0, width), dtype=torch.uint8, device=pts.device), out_faces, rounds
+    with _device_guard(pts):
+        rc = lib.pmb200_simplify_mesh_write(nv, nf, nf_out, out_xyz.data_ptr(), None if out_rgb is None else out_rgb.data_ptr(),
+                                            out_faces.data_ptr(), ws.data_ptr(), int(ws_bytes), _stream(pts))
+    _native.check(rc, what + "_write")
+    parts = [out_xyz.view(torch.uint8).view(nv_out, 12)] + ([] if out_rgb is None else [out_rgb])
+    return torch.cat(parts, 1), out_faces, rounds
+
+
 def render_camera_arrays(P):
     """A 3 x 4 float64 camera K [R | t] -> (P rounded to float32, row-major [12]; camera centre -M^-1 p4 computed in float64
     and rounded to float32 [3]), the HOST values pmb200_render_points / _mesh take.  ValueError for a camera that is not

@@ -48,6 +48,9 @@ surface (ops.tsdf_mesh; definition in include/patchmatch_b200.h).  --mesh-voxel-
 reference views of (median valid depth / fx), a heuristic; --mesh-trunc (voxels, 1..4) and --mesh-min-weight (views) set
 the truncation and the observations a voxel needs.  The volume needs blocks * 512 * 12 bytes besides the kept maps
 (n_ref * H * W * 4 bytes).  dtu_eval scores the mesh's vertices with --ply-template "{outputs}/scan{scan}/mesh.ply".
+With --mesh-target-faces N the mesh is also simplified on the GPU (ops.simplify_mesh: quadric edge collapse in rounds of
+independent collapses) to at most N faces and written to <scan>/mesh_simplified.ply; --mesh-min-component-faces F first
+drops connected pieces of fewer than F faces.  mesh.ply is the same with or without these options.
 tnt_eval scores a Tanks and Temples training scene's fused.ply (or its mesh.ply) by precision, recall and F-score.
 
 Device memory held besides the engines, for a scan of n_img images of H x W and n_ref reference views:
@@ -121,14 +124,20 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--mesh-trunc", type=int, default=argparse.SUPPRESS, help="TSDF truncation in voxels, 1..4 (default 3)")
     ap.add_argument("--mesh-min-weight", type=int, default=argparse.SUPPRESS,
                     help="views that must observe a voxel for it to be meshed (default 1)")
+    ap.add_argument("--mesh-target-faces", type=int, default=argparse.SUPPRESS,
+                    help="with --mesh, also write mesh_simplified.ply: quadric edge collapse to at most this many faces, on the GPU")
+    ap.add_argument("--mesh-min-component-faces", type=int, default=argparse.SUPPRESS,
+                    help="with --mesh-target-faces, first remove connected pieces with fewer faces than this (default 0: none)")
     return ap
 
 
-MESH_DEFAULTS = {"mesh": False, "mesh_voxel_size": None, "mesh_trunc": 3, "mesh_min_weight": 1}
+MESH_DEFAULTS = {"mesh": False, "mesh_voxel_size": None, "mesh_trunc": 3, "mesh_min_weight": 1, "mesh_target_faces": None,
+                 "mesh_min_component_faces": None}
 
 
 def mesh_options(args: argparse.Namespace) -> argparse.Namespace:
-    """--mesh, --mesh-voxel-size, --mesh-trunc and --mesh-min-weight of `args`, with their defaults where not given."""
+    """--mesh, --mesh-voxel-size, --mesh-trunc, --mesh-min-weight, --mesh-target-faces and --mesh-min-component-faces of
+    `args`, with their defaults where not given."""
     return argparse.Namespace(**{k: getattr(args, k, v) for k, v in MESH_DEFAULTS.items()})
 
 
@@ -153,6 +162,10 @@ def check_args(args: argparse.Namespace) -> List[str]:
     if args.checkpoint_path is None or not os.path.isfile(args.checkpoint_path):
         raise Exception("Invalid checkpoint file: {}".format(args.checkpoint_path))
     m = mesh_options(args)
+    if m.mesh_target_faces is not None and (not m.mesh or m.mesh_target_faces < 0):
+        raise ValueError(f"--mesh-target-faces needs --mesh and a value >= 0, got {m.mesh_target_faces}")
+    if m.mesh_min_component_faces is not None and (m.mesh_target_faces is None or m.mesh_min_component_faces < 0):
+        raise ValueError(f"--mesh-min-component-faces needs --mesh-target-faces and a value >= 0, got {m.mesh_min_component_faces}")
     if m.mesh:
         if m.mesh_voxel_size is not None and not (0 < m.mesh_voxel_size < float("inf")):
             raise ValueError(f"--mesh-voxel-size must be positive and finite, got {m.mesh_voxel_size}")
@@ -389,7 +402,16 @@ def mesh_scan(args: argparse.Namespace, bank: SceneBank, refs: Sequence[int], de
     verts, faces = ops.tsdf_mesh(seeds, depths, [bank.images[r] for r in refs], Ks, [bank.extrinsics[r] for r in refs], s,
                                  trunc=m.mesh_trunc, min_weight=m.mesh_min_weight)
     data_io.save_ply(path, verts, faces)
-    return {"mesh_vertices": int(verts.shape[0]), "mesh_faces": int(faces.shape[0]), "mesh_seconds": time.perf_counter() - t0}
+    out = {"mesh_vertices": int(verts.shape[0]), "mesh_faces": int(faces.shape[0]), "mesh_seconds": time.perf_counter() - t0}
+    if m.mesh_target_faces is not None:
+        t0 = time.perf_counter()
+        xyz = verts[:, :12].contiguous().view(torch.float32)
+        body, sfaces, rounds = ops.simplify_mesh(xyz, verts[:, 12:].contiguous(), faces, m.mesh_target_faces,
+                                                 m.mesh_min_component_faces or 0)
+        data_io.save_ply(os.path.join(os.path.dirname(path), "mesh_simplified.ply"), body, sfaces)
+        out.update({"simplified_vertices": int(body.shape[0]), "simplified_faces": int(sfaces.shape[0]), "simplify_rounds": rounds,
+                    "simplify_seconds": time.perf_counter() - t0})
+    return out
 
 
 def fuse_scan(args: argparse.Namespace, scan: str, bank: SceneBank, pairs: Sequence[Tuple[int, List[int]]], maps,
@@ -451,6 +473,8 @@ def reconstruct(args: argparse.Namespace, *, device: str = "cuda:0", n_slots: in
              "depth_maps": 0, "points": 0}
     if mesh_options(args).mesh:
         stats.update({"mesh_vertices": 0, "mesh_faces": 0, "mesh_seconds": 0.0})
+    if mesh_options(args).mesh_target_faces is not None:
+        stats.update({"simplified_vertices": 0, "simplified_faces": 0, "simplify_rounds": 0, "simplify_seconds": 0.0})
     t_start = time.perf_counter()
     with precision(args.tf32), torch.cuda.device(dev), torch.no_grad():
         stage = DepthStage(load_network(args).to(dev), dev, n_slots=n_slots, seed=args.seed) if do_depth else None
