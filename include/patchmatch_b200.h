@@ -446,6 +446,83 @@ int pmb200_render_mesh(const float *xyz, const unsigned char *rgb, int64_t n_ver
                        const unsigned char *background_host, unsigned char *out_rgb, float *out_depth, void *workspace,
                        int64_t workspace_bytes, void *stream);
 
+/* pmb200_render_mesh_textured: pmb200_render_mesh with a texture in place of vertex colours.  uv float32 [nf,3,2] (per face
+ * corner, OBJ's bottom-left convention), page int32 [nf], pages uint8 [n_pages,S,S,3].  The colour of a pixel is the texel
+ * (floor(s S), floor((1 - t) S)) of page[f], clamped to 0..S-1, with (s, t) = ((w0 uv0 + w1 uv1) + w2 uv2) the perspective-
+ * correct interpolation; shade applies as before.  A face whose page is outside 0..n_pages-1 is grey (160).  Same workspace
+ * as pmb200_render_mesh; the z-buffer is the same, only the resolve differs. */
+int pmb200_render_mesh_textured(const float *xyz, int64_t n_vertices, const int *faces, int64_t n_faces, const float *uv,
+                                const int *page, const unsigned char *pages, int n_pages, int side, const float *P_host,
+                                const float *centre_host, int width, int height, float near_z, int shade,
+                                const unsigned char *background_host, unsigned char *out_rgb, float *out_depth, void *workspace,
+                                int64_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------
+ * Mesh texturing: per-face view selection with occlusion, charts packed into texture pages, texture coordinates (beyond
+ * the reference; INTEGRATION.md "Textured meshes (beyond the reference)").  Definition, reproduced bit for bit by
+ * oracle/texture_oracle.py; float64 arithmetic (pm_texture_math.cuh) with each operation rounded on its own, no
+ * floating-point atomics, reruns give the same bits:
+ *
+ * Views.  Per view P (K [R | t] in float64, row-major 3 x 4), its centre C = -R^T t (float64), near_z and W x H.  The
+ * z-buffer uses the renderer's camera (P and C rounded to float32, near_z to float32), coverage rule and key.
+ * 1. Visibility of face f in view v: visible(f, v) = pixels whose z-buffer winner is f; covered(f, v) = pixels f covers by
+ *    the coverage rule, whatever their depth.
+ * 2. v is a candidate for f when visible >= 1 and 10 visible >= 9 covered; each corner's float64 projection (u, v, z)
+ *    (u' = ((P00 x + P01 y) + P02 z) + P03, u = u' / z) has z > near_z, 0 <= u <= W - 1 and 0 <= v <= H - 1; and
+ *    n . (C - ((X0 + X1) + X2) / 3) > 0 with n = (X1 - X0) x (X2 - X0).  D(f, v) = visible(f, v).  Entries (f, v, D) are
+ *    kept per view, then in rows by face, in view order (CSR); no faces x views matrix is allocated.
+ * 3. Labels.  l0(f) = argmax D over the candidates (ties: the lower view).  Then kRounds = 3 Jacobi rounds:
+ *    l(f) = argmax over candidates v of D(f, v) / max D(f, .) + kLambda (= 0.5) * #{(g, e): e an edge of f, g != f another
+ *    face on e, l_prev(g) = v}, ties to the lower view.  Edges are unordered vertex pairs (a != b).  No candidate: l = -1,
+ *    the face is untextured.
+ * 4. Charts: connected components of the textured faces over edges whose two faces share a label; a chart's id is its
+ *    smallest face.  Its rectangle in its view's pixels is x0 = min floor(u) - 2 .. x1 = max ceil(u) + 2 (likewise v) over
+ *    its faces' corners; a texel (x, y) of it copies the image pixel (clamp(x, 0, W - 1), clamp(y, 0, H - 1)) as
+ *    clamp(rint(255 image), 0, 255) (float32 product, half to even).
+ * 5. Atlas.  Side S = the smallest power of two >= max(4096, the largest rectangle side), at most 16384.  The charts, by
+ *    (height desc, width desc, chart id), then one 4 x 4 cell per untextured face in face order, are placed on shelves: a
+ *    rectangle goes right of the previous one, on a new shelf (below the tallest of the current shelf) when it would cross
+ *    x = S, and on a new page when it would cross y = S.  A cell holds rint(((c0 + c1 + c2) / 3)) of its vertex colours
+ *    (160 without colours).  Texels outside every rectangle are 0.
+ * 6. Coordinates.  A corner (u, v) of a chart at rectangle origin (x0, y0) placed at (ox, oy): a = u - x0 + ox,
+ *    b = v - y0 + oy, uv = (float32((a + 0.5) / S), float32(1 - (b + 0.5) / S)).  An untextured face's corners get its
+ *    cell's centre, (float32((ox + 2) / S), float32(1 - (oy + 2) / S)).
+ *
+ * pmb200_texture_mesh: visibility, labels and charts.  xyz float32 [nv,3], faces int32 [nf,3]; nv < 2^31, nf < 2^29;
+ *   views_host (HOST) n_views records; label_out int32 [nf] (-1 untextured); slot_out int32 [nf] (the face's chart's row in
+ *   charts_out, or n_charts + its rank among the untextured faces); charts_out int32 [nf,6] (first n_charts rows: chart id,
+ *   view, x0, y0, width, height, by ascending id).  counts_host (HOST) <- entries, charts, untextured faces.  Host reads:
+ *   one per view (its entry count), one per chart pass, and the counts.  Workspace of
+ *   pmb200_texture_mesh_workspace_bytes bytes: about 170 bytes per face, 16 per vertex, 8 per pixel of the largest view
+ *   and 16 per entry, entries <= sum over views of min(nf, W H).  Needs a CUDA device to size its CUB passes.
+ * pmb200_texture_pack (host only): sizes_host [n_charts,2] (width, height) of the chart rows -> places_host
+ *   [n_charts + n_cells,3] (page, x, y), the side S and the page count.
+ * pmb200_texture_write: view >= 0 writes that view's charts into pages [n_pages,S,S,3] (zeroed by the caller): image
+ *   float32 [3,H,W] (device), rows int32 [n_rows] (device) the chart rows of the view, prefix int64 [n_rows+1] (device) the
+ *   exclusive sums of their width x height; one thread per texel, each texel written once.  view == -1 writes uv_out
+ *   float32 [nf,3,2], page_out int32 [nf] and the untextured faces' cells, with rgb uint8 [nv,3] or NULL; workspace of
+ *   pmb200_texture_write_workspace_bytes(n_views) bytes.
+ * PMB200_EINVAL, nothing launched, for a null pointer, sizes out of range, a view with a size outside 1..16384, a camera
+ * that is not finite or near_z <= 0, a rectangle side > 16384, or a workspace smaller than the query. */
+typedef struct {
+    double P[12];       /* K [R | t], float64, row-major 3 x 4 */
+    double centre[3];   /* -R^T t */
+    double near_z;      /* > 0 */
+    int32_t width, height;
+} pmb200_texture_view;
+
+int64_t pmb200_texture_mesh_workspace_bytes(int64_t n_vertices, int64_t n_faces, const pmb200_texture_view *views_host, int n_views);
+int pmb200_texture_mesh(const float *xyz, int64_t n_vertices, const int *faces, int64_t n_faces, const pmb200_texture_view *views_host,
+                        int n_views, int *label_out, int *slot_out, int *charts_out, int64_t *counts_host, void *workspace,
+                        int64_t workspace_bytes, void *stream);
+int pmb200_texture_pack(const int *sizes_host, int64_t n_charts, int64_t n_cells, int *places_host, int *side_out, int *pages_out);
+int64_t pmb200_texture_write_workspace_bytes(int n_views);
+int pmb200_texture_write(int view, const float *image, int width, int height, const int *rows, const int64_t *prefix, int n_rows,
+                         const float *xyz, const unsigned char *rgb, int64_t n_vertices, const int *faces, int64_t n_faces,
+                         const pmb200_texture_view *views_host, int n_views, const int *label, const int *slot, const int *charts,
+                         const int *places, int side, int n_pages, float *uv_out, int *page_out, unsigned char *pages,
+                         void *workspace, int64_t workspace_bytes, void *stream);
+
 /* ------------------------------------------------------------------------------------
  * DTU point-cloud evaluation (reference evaluations/dtu/*.m; INTEGRATION.md "DTU evaluation"), float64 throughout.
  * Both calls sort the cloud into a fine / coarse cell hash held in a caller-owned device workspace of

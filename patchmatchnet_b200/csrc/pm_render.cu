@@ -8,52 +8,33 @@
 //
 // Points: one thread per point splats its s x s square.  Meshes: vertices are projected once; one thread per triangle
 // rasterises the triangles whose clipped box is at most kSmallBox pixels on a side, larger ones are appended to a list (atomic
-// counter) that a grid of CTAs rasterises, one triangle per CTA at a time, striding over its box.  Both call cover().
+// counter) that a grid of CTAs rasterises, one triangle per CTA at a time, striding over its box.  Both call cover()
+// (pm_raster.cuh, shared with the texturer's visibility pass).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <cmath>
 
 #include "../../include/patchmatch_b200.h"
+#include "pm_raster.cuh"
 
 extern "C" int pmb200_internal_fail(int code, const char *msg);
 extern "C" int pmb200_internal_launch_status(const char *what);
 
 namespace {
 
+using namespace pmraster;
+
 constexpr int kBlock = 256;
-constexpr int kSmallBox = 16;       // a triangle whose clipped box is at most 16 x 16 pixels is rasterised by one thread
 constexpr int kLargeCtas = 1056;    // CTAs of the large-triangle pass (8 per SM of an H100 SXM)
 constexpr int kMaxSide = 16384;     // width and height
-constexpr float kMaxCoord = 4194304.0f;  // 2^22: a triangle vertex farther out in u or v is not rasterised
 constexpr float kGrey = 160.0f;     // colour of a PLY without colours
-constexpr unsigned long long kEmpty = ~0ull;
 
 __host__ __device__ inline size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
-
-struct Camera {
-    float P[12];   // K [R | t], row-major 3 x 4
-    float C[3];    // camera centre
-    int W, H;
-    float near_z;
-    int shade;
-    float bg[3];
-};
 
 inline int grid_blocks(long long n) {
     const long long b = (n + kBlock - 1) / kBlock;
     return (int)(b < 1 ? 1 : (b > 65535 * 8 ? 65535 * 8 : b));
-}
-
-// ((r0 x + r1 y) + r2 z) + r3
-__device__ inline float row(const float *r, float x, float y, float z) {
-    return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(r[0], x), __fmul_rn(r[1], y)), __fmul_rn(r[2], z)), r[3]);
-}
-
-// (u, v, z) of a world point; u = u' / z and v = v' / z, IEEE division
-__device__ inline float3 project(const Camera &c, float x, float y, float z) {
-    const float zz = row(c.P + 8, x, y, z);
-    return make_float3(row(c.P, x, y, z) / zz, row(c.P + 4, x, y, z) / zz, zz);
 }
 
 // 0.25 + 0.75 |n . l| with l = d / |d| (d = camera centre - surface point); 1 where that is undefined
@@ -125,82 +106,6 @@ __global__ void __launch_bounds__(kBlock) project_kernel(const Camera c, const f
     }
 }
 
-struct Tri {
-    float x[3], y[3], z[3];
-    int v[3];      // mesh vertex of each slot (slots 1 and 2 swapped when the signed area is negative)
-    float area;    // > 0
-    bool tl[3];    // the edge opposite slot i is a top or left edge
-    int x0, x1, y0, y1;  // clipped box, inclusive
-};
-
-__device__ inline bool top_left(float ax, float ay, float bx, float by) {
-    const float dx = __fsub_rn(bx, ax), dy = __fsub_rn(by, ay);
-    return dy < 0.0f || (dy == 0.0f && dx > 0.0f);
-}
-
-// the edge function of a -> b at p, evaluated from the edge's lower endpoint (smaller v, then smaller u) and negated when
-// that is b, so the two faces of a shared edge get the same magnitude with opposite signs
-__device__ inline float edge_at(float ax, float ay, float bx, float by, float px, float py) {
-    const bool flip = by < ay || (by == ay && bx < ax);
-    const float sx = flip ? bx : ax, sy = flip ? by : ay, ex = flip ? ax : bx, ey = flip ? ay : by;
-    const float e = __fsub_rn(__fmul_rn(__fsub_rn(ex, sx), __fsub_rn(py, sy)), __fmul_rn(__fsub_rn(ey, sy), __fsub_rn(px, sx)));
-    return flip ? -e : e;
-}
-
-// false for a triangle that is not rasterised (a vertex index out of range, a vertex skipped by the projection, zero area,
-// or an empty clipped box)
-__device__ inline bool setup(const Camera &c, const float4 *proj, const int *faces, long long f, long long nv, Tri &t) {
-    for (int k = 0; k < 3; ++k) {
-        const int v = faces[3 * f + k];
-        if (v < 0 || v >= nv) return false;
-        const float4 q = proj[v];
-        if (q.w == 0.0f) return false;
-        t.x[k] = q.x; t.y[k] = q.y; t.z[k] = q.z; t.v[k] = v;
-    }
-    float a = __fsub_rn(__fmul_rn(__fsub_rn(t.x[1], t.x[0]), __fsub_rn(t.y[2], t.y[0])),
-                        __fmul_rn(__fsub_rn(t.y[1], t.y[0]), __fsub_rn(t.x[2], t.x[0])));
-    if (a == 0.0f) return false;
-    if (a < 0.0f) {
-        float s;
-        s = t.x[1]; t.x[1] = t.x[2]; t.x[2] = s;
-        s = t.y[1]; t.y[1] = t.y[2]; t.y[2] = s;
-        s = t.z[1]; t.z[1] = t.z[2]; t.z[2] = s;
-        const int w = t.v[1]; t.v[1] = t.v[2]; t.v[2] = w;
-        a = -a;
-    }
-    t.area = a;
-    t.tl[0] = top_left(t.x[1], t.y[1], t.x[2], t.y[2]);
-    t.tl[1] = top_left(t.x[2], t.y[2], t.x[0], t.y[0]);
-    t.tl[2] = top_left(t.x[0], t.y[0], t.x[1], t.y[1]);
-    const float umin = fminf(fminf(t.x[0], t.x[1]), t.x[2]), umax = fmaxf(fmaxf(t.x[0], t.x[1]), t.x[2]);
-    const float vmin = fminf(fminf(t.y[0], t.y[1]), t.y[2]), vmax = fmaxf(fmaxf(t.y[0], t.y[1]), t.y[2]);
-    t.x0 = (int)fmaxf(ceilf(umin), 0.0f); t.x1 = (int)fminf(floorf(umax), (float)(c.W - 1));
-    t.y0 = (int)fmaxf(ceilf(vmin), 0.0f); t.y1 = (int)fminf(floorf(vmax), (float)(c.H - 1));
-    return t.x0 <= t.x1 && t.y0 <= t.y1;
-}
-
-// pixel (px, py) inside the triangle: its barycentrics b and depth z (0 < z < inf), else false
-__device__ inline bool cover(const Tri &t, int px, int py, float b[3], float &z) {
-    const float fx = (float)px, fy = (float)py;
-    const float e0 = edge_at(t.x[1], t.y[1], t.x[2], t.y[2], fx, fy);
-    const float e1 = edge_at(t.x[2], t.y[2], t.x[0], t.y[0], fx, fy);
-    const float e2 = edge_at(t.x[0], t.y[0], t.x[1], t.y[1], fx, fy);
-    if (!(e0 > 0.0f || (e0 == 0.0f && t.tl[0])) || !(e1 > 0.0f || (e1 == 0.0f && t.tl[1])) ||
-        !(e2 > 0.0f || (e2 == 0.0f && t.tl[2])))
-        return false;
-    b[0] = e0 / t.area; b[1] = e1 / t.area; b[2] = e2 / t.area;
-    const float s = __fadd_rn(__fadd_rn(b[0] / t.z[0], b[1] / t.z[1]), b[2] / t.z[2]);
-    if (!(s > 0.0f)) return false;
-    z = 1.0f / s;
-    return z < INFINITY;
-}
-
-__device__ inline void raster_pixel(const Camera &c, const Tri &t, int px, int py, uint32_t f, unsigned long long *zbuf) {
-    float b[3], z;
-    if (cover(t, px, py, b, z))
-        atomicMin(zbuf + (size_t)py * c.W + px, ((unsigned long long)__float_as_uint(z) << 32) | (unsigned long long)f);
-}
-
 __global__ void __launch_bounds__(kBlock) raster_small_kernel(const Camera c, const float4 *proj, const int *faces, long long nf,
                                                               long long nv, unsigned long long *zbuf, int *large, int *n_large) {
     for (long long f = blockIdx.x * (long long)kBlock + threadIdx.x; f < nf; f += (long long)gridDim.x * kBlock) {
@@ -269,6 +174,58 @@ __global__ void __launch_bounds__(kBlock) resolve_mesh_kernel(const Camera c, co
                                 __fmul_rn(w[2], (float)rgb[3 * (size_t)t.v[2] + k]));
             out_rgb[3 * p + k] = channel(col, f_shade);
         }
+        out_depth[p] = __uint_as_float((uint32_t)(key >> 32));
+    }
+}
+
+// a textured face's colour: the nearest texel of the perspective-correct texture coordinate (the PLY path above is untouched)
+__global__ void __launch_bounds__(kBlock) resolve_textured_kernel(const Camera c, const float *xyz, const float4 *proj, const int *faces,
+                                                                  long long nv, const float *uv, const int *page,
+                                                                  const unsigned char *pages, int n_pages, int S,
+                                                                  const unsigned long long *zbuf, unsigned char *out_rgb,
+                                                                  float *out_depth) {
+    const size_t npix = (size_t)c.W * c.H;
+    for (size_t p = blockIdx.x * (size_t)kBlock + threadIdx.x; p < npix; p += (size_t)gridDim.x * kBlock) {
+        const unsigned long long key = zbuf[p];
+        if (key == kEmpty) {
+            write_background(c, p, out_rgb, out_depth);
+            continue;
+        }
+        const long long f = (uint32_t)key;
+        Tri t;
+        float b[3], z;
+        setup(c, proj, faces, f, nv, t);
+        cover(t, (int)(p % c.W), (int)(p / c.W), b, z);
+        float w[3];
+        for (int k = 0; k < 3; ++k) w[k] = __fmul_rn(b[k] / t.z[k], z);
+        const bool swapped = t.v[1] != faces[3 * f + 1];  // setup swapped corners 1 and 2 (a rasterised face has distinct corners)
+        const int corner[3] = {0, swapped ? 2 : 1, swapped ? 1 : 2};
+        float st[2];
+        for (int a = 0; a < 2; ++a)
+            st[a] = __fadd_rn(__fadd_rn(__fmul_rn(w[0], uv[6 * f + 2 * corner[0] + a]), __fmul_rn(w[1], uv[6 * f + 2 * corner[1] + a])),
+                              __fmul_rn(w[2], uv[6 * f + 2 * corner[2] + a]));
+        float f_shade = 1.0f;
+        if (c.shade) {
+            float X[3], e1[3], e2[3];
+            const int v0 = faces[3 * f], v1 = faces[3 * f + 1], v2 = faces[3 * f + 2];
+            for (int a = 0; a < 3; ++a) {
+                X[a] = __fadd_rn(__fadd_rn(__fmul_rn(w[0], xyz[3 * (size_t)t.v[0] + a]), __fmul_rn(w[1], xyz[3 * (size_t)t.v[1] + a])),
+                                 __fmul_rn(w[2], xyz[3 * (size_t)t.v[2] + a]));
+                e1[a] = __fsub_rn(xyz[3 * (size_t)v1 + a], xyz[3 * (size_t)v0 + a]);
+                e2[a] = __fsub_rn(xyz[3 * (size_t)v2 + a], xyz[3 * (size_t)v0 + a]);
+            }
+            f_shade = shade_factor(__fsub_rn(__fmul_rn(e1[1], e2[2]), __fmul_rn(e1[2], e2[1])),
+                                   __fsub_rn(__fmul_rn(e1[2], e2[0]), __fmul_rn(e1[0], e2[2])),
+                                   __fsub_rn(__fmul_rn(e1[0], e2[1]), __fmul_rn(e1[1], e2[0])), __fsub_rn(c.C[0], X[0]),
+                                   __fsub_rn(c.C[1], X[1]), __fsub_rn(c.C[2], X[2]));
+        }
+        const int pg = page[f];
+        const float fs = (float)S;
+        const int tx = (int)fminf(fmaxf(floorf(__fmul_rn(st[0], fs)), 0.0f), fs - 1.0f);
+        const int ty = (int)fminf(fmaxf(floorf(__fmul_rn(__fsub_rn(1.0f, st[1]), fs)), 0.0f), fs - 1.0f);
+        const unsigned char *texel = pages + 3 * (((size_t)pg * S + ty) * S + tx);
+        for (int k = 0; k < 3; ++k)
+            out_rgb[3 * p + k] = channel(pg >= 0 && pg < n_pages ? (float)texel[k] : kGrey, f_shade);
         out_depth[p] = __uint_as_float((uint32_t)(key >> 32));
     }
 }
@@ -375,4 +332,36 @@ extern "C" int pmb200_render_mesh(const float *xyz, const unsigned char *rgb, in
     resolve_mesh_kernel<<<grid_blocks((long long)npix), kBlock, 0, st>>>(c, xyz, rgb, w.proj, faces, n_vertices, w.zbuf, out_rgb,
                                                                          out_depth);
     return pmb200_internal_launch_status("render_mesh");
+}
+
+extern "C" int pmb200_render_mesh_textured(const float *xyz, int64_t n_vertices, const int *faces, int64_t n_faces, const float *uv,
+                                          const int *page, const unsigned char *pages, int n_pages, int side, const float *P_host,
+                                          const float *centre_host, int width, int height, float near_z, int shade,
+                                          const unsigned char *background_host, unsigned char *out_rgb, float *out_depth,
+                                          void *workspace, int64_t workspace_bytes, void *stream) {
+    if ((!xyz && n_vertices > 0) || (!faces && n_faces > 0) || ((!uv || !page) && n_faces > 0) || (!pages && n_pages > 0) || !out_rgb ||
+        !out_depth || !workspace)
+        return pmb200_internal_fail(PMB200_EINVAL, "render_mesh_textured: null pointer");
+    if (n_vertices < 0 || n_vertices >= (1ll << 31) || n_faces < 0 || n_faces >= (1ll << 31) || n_pages < 0 || side < 1 || side > kMaxSide)
+        return pmb200_internal_fail(PMB200_EINVAL, "render_mesh_textured: 0 <= n_vertices, n_faces < 2^31, n_pages >= 0, 1 <= side <= 16384");
+    Camera c;
+    if (check_camera("render_mesh_textured: null camera, a size outside 1..16384, a non-finite camera or near not finite and > 0", P_host,
+                     centre_host, width, height, near_z, background_host, shade, c))
+        return PMB200_EINVAL;
+    MeshLayout w;
+    const long long need = mesh_layout(static_cast<char *>(workspace), width, height, n_vertices, n_faces, w);
+    if (workspace_bytes < need)
+        return pmb200_internal_fail(PMB200_EINVAL, "render_mesh_textured: workspace smaller than render_mesh_workspace_bytes(...)");
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const size_t npix = (size_t)width * height;
+    cudaMemsetAsync(w.zbuf, 0xff, npix * 8, st);
+    cudaMemsetAsync(w.n_large, 0, sizeof(int), st);
+    if (n_vertices > 0) project_kernel<<<grid_blocks(n_vertices), kBlock, 0, st>>>(c, xyz, n_vertices, w.proj);
+    if (n_faces > 0) {
+        raster_small_kernel<<<grid_blocks(n_faces), kBlock, 0, st>>>(c, w.proj, faces, n_faces, n_vertices, w.zbuf, w.large, w.n_large);
+        raster_large_kernel<<<kLargeCtas, kBlock, 0, st>>>(c, w.proj, faces, n_vertices, w.large, w.n_large, w.zbuf);
+    }
+    resolve_textured_kernel<<<grid_blocks((long long)npix), kBlock, 0, st>>>(c, xyz, w.proj, faces, n_vertices, uv, page, pages, n_pages,
+                                                                             side, w.zbuf, out_rgb, out_depth);
+    return pmb200_internal_launch_status("render_mesh_textured");
 }

@@ -487,3 +487,112 @@ def _ply_triangles(f, ascii_rows, count_t: str, item_t: str, count: int, path: s
                 raise ValueError(f"{path}: face {i} is not a triangle ({' '.join(words) or 'missing'})")
             v[i] = [int(w) for w in words[1:]]
     return v
+
+
+def save_obj(stem: str, xyz, faces, uv, page, pages) -> None:
+    """Write a textured mesh (ops.texture_mesh's output) as Wavefront OBJ: `<stem>.obj` (mtllib; v per vertex; three vt per
+    face, in face order; the faces grouped by page under `usemtl page_NN`, in their original order within a page, as
+    `f a/ta b/tb c/tc`), `<stem>.mtl` (one material per page, map_Kd `<stem>_NN.png`) and the pages as PNG.  xyz float32
+    [nv,3], faces int32 [nf,3], uv float32 [nf,3,2], page int32 [nf], pages uint8 [P,S,S,3]; tensors or arrays, any device.
+    Coordinates are written with 9 significant digits, which reads back to the same float32."""
+    from PIL import Image
+
+    arr = lambda t: t.detach().cpu().numpy() if isinstance(t, torch.Tensor) else np.asarray(t)
+    xyz, faces, uv, page, pages = arr(xyz).astype(np.float32), arr(faces).astype(np.int64), arr(uv).astype(np.float32), arr(page), arr(pages)
+    nf = faces.shape[0]
+    if xyz.ndim != 2 or xyz.shape[1] != 3 or faces.shape != (nf, 3) or uv.shape != (nf, 3, 2) or page.shape != (nf,):
+        raise ValueError("save_obj: xyz [nv,3], faces [nf,3], uv [nf,3,2] and page [nf]")
+    if pages.dtype != np.uint8 or pages.ndim != 4 or pages.shape[3] != 3:
+        raise ValueError("save_obj: pages must be uint8 [P,S,S,3]")
+    if nf and (faces.min() < 0 or faces.max() >= len(xyz) or page.min() < 0 or page.max() >= len(pages)):
+        raise ValueError("save_obj: a face refers to a vertex or page that does not exist")
+    base = os.path.basename(stem)
+    with open(stem + ".mtl", "w") as f:
+        for p in range(len(pages)):
+            f.write(f"newmtl page_{p:02d}\nKa 1 1 1\nKd 1 1 1\nKs 0 0 0\nillum 1\nmap_Kd {base}_{p:02d}.png\n")
+    lines = [f"mtllib {base}.mtl\n"]
+    lines += ["v %.9g %.9g %.9g\n" % tuple(r) for r in xyz.tolist()]
+    lines += ["vt %.9g %.9g\n" % tuple(r) for r in uv.reshape(-1, 2).tolist()]
+    for p in range(len(pages)):
+        sel = np.flatnonzero(page == p)
+        if sel.size == 0:
+            continue
+        lines.append(f"usemtl page_{p:02d}\n")
+        v = faces[sel] + 1
+        t = 3 * sel[:, None] + np.arange(1, 4)[None, :]
+        lines += ["f %d/%d %d/%d %d/%d\n" % (a, ta, b, tb, c, tc) for (a, b, c), (ta, tb, tc) in zip(v.tolist(), t.tolist())]
+    with open(stem + ".obj", "w") as f:
+        f.writelines(lines)
+    for p in range(len(pages)):
+        Image.fromarray(pages[p]).save(f"{stem}_{p:02d}.png")
+
+
+def read_obj(path: str):
+    """The OBJ subset save_obj writes -> (xyz float32 [nv,3], faces int32 [nf,3], uv float32 [nf,3,2], page int32 [nf],
+    pages uint8 [P,S,S,3]), faces in file order.  Reads v, vt, triangles `f a/ta b/tb c/tc` (1-based), usemtl, mtllib and
+    the materials' map_Kd (square RGB pages of one size), blank lines and comments; ValueError on anything else."""
+    from PIL import Image
+
+    folder = os.path.dirname(os.path.abspath(path))
+    vs, vts, fs, pgs = [], [], [], []
+    materials: Dict[str, str] = {}
+    current = -1
+    names: List[str] = []
+    with open(path) as f:
+        for n, line in enumerate(f, 1):
+            tok = line.split()
+            if not tok or tok[0].startswith("#"):
+                continue
+            try:
+                if tok[0] == "v" and len(tok) == 4:
+                    vs.append([float(t) for t in tok[1:]])
+                elif tok[0] == "vt" and len(tok) == 3:
+                    vts.append([float(t) for t in tok[1:]])
+                elif tok[0] == "f" and len(tok) == 4 and all(t.count("/") == 1 for t in tok[1:]):
+                    pairs = [t.split("/") for t in tok[1:]]
+                    fs.append([int(a) for a, _ in pairs] + [int(b) for _, b in pairs])
+                    pgs.append(current)
+                elif tok[0] == "usemtl" and len(tok) == 2:
+                    if tok[1] not in names:
+                        names.append(tok[1])
+                    current = names.index(tok[1])
+                elif tok[0] == "mtllib" and len(tok) == 2:
+                    materials.update(_read_mtl(os.path.join(folder, tok[1])))
+                else:
+                    raise ValueError
+            except ValueError:
+                raise ValueError(f"{path}:{n}: not part of the OBJ subset read_obj reads: {line.strip()!r}") from None
+    xyz = np.asarray(vs, np.float32).reshape(-1, 3)
+    tex = np.asarray(vts, np.float32).reshape(-1, 2)
+    fa = np.asarray(fs, np.int64).reshape(-1, 6) - 1
+    if fa.size and (fa[:, :3].min() < 0 or fa[:, :3].max() >= len(xyz) or fa[:, 3:].min() < 0 or fa[:, 3:].max() >= len(tex)):
+        raise ValueError(f"{path}: a face refers to a vertex or texture coordinate that does not exist")
+    if any(p < 0 for p in pgs):
+        raise ValueError(f"{path}: a face comes before any usemtl")
+    images = []
+    for name in names:
+        if name not in materials:
+            raise ValueError(f"{path}: material {name!r} has no map_Kd")
+        img = np.asarray(Image.open(materials[name]).convert("RGB"), np.uint8)
+        if img.shape[0] != img.shape[1] or (images and img.shape != images[0].shape):
+            raise ValueError(f"{path}: the pages must be square and of one size")
+        images.append(img)
+    pages = np.stack(images) if images else np.zeros((0, 1, 1, 3), np.uint8)
+    return xyz, fa[:, :3].astype(np.int32), tex[fa[:, 3:]], np.asarray(pgs, np.int32), pages
+
+
+def _read_mtl(path: str) -> Dict[str, str]:
+    out: Dict[str, str] = {}
+    name = None
+    with open(path) as f:
+        for n, line in enumerate(f, 1):
+            tok = line.split()
+            if not tok or tok[0].startswith("#") or tok[0] in ("Ka", "Kd", "Ks", "illum", "Ns", "d"):
+                continue
+            if tok[0] == "newmtl" and len(tok) == 2:
+                name = tok[1]
+            elif tok[0] == "map_Kd" and len(tok) == 2 and name is not None:
+                out[name] = os.path.join(os.path.dirname(os.path.abspath(path)), tok[1])
+            else:
+                raise ValueError(f"{path}:{n}: not part of the MTL subset read_obj reads: {line.strip()!r}")
+    return out

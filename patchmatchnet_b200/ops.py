@@ -1970,3 +1970,265 @@ def depth_metrics(maps: Sequence[Tensor], depth_gt: Tensor, mask: Tensor, thresh
                                                 _stream(gt))
     _native.check(rc, "depth_metrics")
     return out
+
+
+# ---- mesh texturing -------------------------------------------------------------------------------------------------------
+
+
+def mesh_box_centre(xyz: Tensor):
+    """Centre of the per-axis 1st-99th percentile box of the vertices (the k-th and (n-1-k)-th smallest coordinates,
+    k = floor(0.01 (n - 1))), float64 [3]; render frames the same box."""
+    import numpy as np
+
+    n = xyz.shape[0]
+    if n == 0:
+        return np.zeros(3)
+    k = int(0.01 * (n - 1))
+    s = torch.sort(xyz, dim=0).values
+    lo, hi = s[k].double().cpu().numpy(), s[n - 1 - k].double().cpu().numpy()
+    return (lo + hi) / 2.0
+
+
+def texture_view_table(Ks, Es, sizes, box_centre):
+    """ctypes array of pmb200_texture_view: P = K [R | t] composed in float64, centre -M^-1 p4, near = 1e-3 x the distance
+    from the centre to box_centre (render's default near, so render --views sees the same front faces) and (H, W) per view."""
+    import numpy as np
+
+    V = len(sizes)
+    table = (_native.TextureView * V)()
+    for v in range(V):
+        K = np.asarray(Ks[v].detach().cpu().numpy() if isinstance(Ks[v], Tensor) else Ks[v], np.float64)
+        E = np.asarray(Es[v].detach().cpu().numpy() if isinstance(Es[v], Tensor) else Es[v], np.float64)
+        if K.shape != (3, 3) or E.shape != (4, 4) or not np.isfinite(K).all() or not np.isfinite(E).all():
+            raise ValueError(f"texture_mesh: view {v}: K must be a finite [3,3] and E a finite [4,4]")
+        P = K @ E[:3, :4]
+        try:
+            centre = -np.linalg.solve(P[:, :3], P[:, 3])
+        except np.linalg.LinAlgError:
+            raise ValueError(f"texture_mesh: view {v}: the camera's left 3 x 3 is singular") from None
+        table[v].P[:] = P.ravel().tolist()
+        table[v].centre[:] = centre.tolist()
+        table[v].near_z = 1e-3 * max(float(np.linalg.norm(centre - box_centre)), 1e-30)
+        table[v].height, table[v].width = int(sizes[v][0]), int(sizes[v][1])
+    return table
+
+
+def _texture_images(images, xyz: Tensor, what: str):
+    if len(images) < 1:
+        raise ValueError(f"{what}: at least one view")
+    for v, img in enumerate(images):
+        if (not isinstance(img, Tensor) or not _on_device(img) or img.dtype != torch.float32 or img.dim() != 3 or img.shape[0] != 3
+                or not 1 <= img.shape[1] <= 16384 or not 1 <= img.shape[2] <= 16384):
+            raise ValueError(f"{what}: view {v}: the image must be a CUDA float32 [3,H,W] tensor, 1 <= H, W <= 16384")
+        if img.device != xyz.device:
+            raise ValueError(f"{what}: view {v}: the image must be on the vertices' device")
+    return [tuple(img.shape[1:]) for img in images]
+
+
+TEXTURE_OUTPUT_BYTES_PER_FACE = 4 + 4 + 24 + 24 + 4  # label, slot, chart rows, uv, page
+
+
+def texture_mesh_bytes(n_vertices: int, n_faces: int, sizes) -> int:
+    """Estimate of the device memory ops.texture_mesh needs beyond its inputs: the workspace of pmb200_texture_mesh (about
+    170 bytes per face, 16 per vertex, 8 per pixel of the largest view and 16 per visibility entry, at most min(nf, H W)
+    entries per view), 60 bytes per face of outputs and one 4096 x 4096 page.  `sizes` the views' (H, W).  More pages add
+    48 MiB each (at side 4096) and are checked again before they are allocated.  Needs a CUDA device."""
+    table = texture_view_table([[[1, 0, 0], [0, 1, 0], [0, 0, 1]]] * len(sizes), [[[1, 0, 0, 0], [0, 1, 0, 0], [0, 0, 1, 0], [0, 0, 0, 1]]]
+                               * len(sizes), sizes, [0.0, 0.0, -1.0])
+    ws = _native.lib().pmb200_texture_mesh_workspace_bytes(n_vertices, n_faces, _addr(table), len(sizes))
+    if ws < 0:
+        _native.check(int(ws), "texture_mesh_workspace_bytes")
+    return int(ws) + TEXTURE_OUTPUT_BYTES_PER_FACE * n_faces + 4096 * 4096 * 3
+
+
+def _addr(obj) -> int:
+    import ctypes
+
+    return ctypes.addressof(obj)
+
+
+def _free_bytes(device) -> int:
+    with torch.cuda.device(device):
+        return torch.cuda.mem_get_info(device)[0] + torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device)
+
+
+def texture_mesh(xyz: Tensor, rgb: Optional[Tensor], faces: Tensor, images: Sequence[Tensor], Ks, Es):
+    """Texture a triangle mesh from views: per face the view that sees it best among those that see at least 90 % of it
+    unoccluded, smoothed over edge neighbours; charts of neighbouring faces with one view cut from that view's image and
+    shelf-packed into square pages (definition in include/patchmatch_b200.h).  xyz CUDA float32 [nv,3]; rgb uint8 [nv,3] or
+    None (an untextured face's cell takes its vertices' mean colour, or grey); faces int32 [nf,3]; per view the image
+    float32 [3,H,W] in [0,1] (views may differ in size), K [3,3] scaled to that size and E [4,4] world -> camera.
+    -> (uv float32 [nf,3,2] per face corner, OBJ's bottom-left convention; page int32 [nf]; pages uint8 [P,S,S,3]; stats
+    dict) on the device, in the original face order.  Reruns give the same bits.
+
+    ValueError before any launch on bad arguments (a face index outside 0..nv-1 included), and before allocating when
+    texture_mesh_bytes exceeds the device's free memory.  Host reads: one per view, one per chart pass, a few counts."""
+    import numpy as np
+
+    what = "texture_mesh"
+    pts = _render_xyz(xyz, what)
+    nv = pts.shape[0]
+    if not isinstance(faces, Tensor) or not _on_device(faces) or faces.dtype != torch.int32 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError(f"{what}: faces must be a CUDA int32 [nf,3] tensor")
+    if faces.device != pts.device:
+        raise ValueError(f"{what}: faces must be on the vertices' device")
+    fc = faces.contiguous()
+    nf = fc.shape[0]
+    if nv >= 2 ** 31 or nf >= 2 ** 29:
+        raise ValueError(f"{what}: at most 2^31 - 1 vertices and 2^29 - 1 faces, got {nv} and {nf}")
+    col = _render_attr(rgb, nv, torch.uint8, pts.device, "rgb", what)
+    sizes = _texture_images(images, pts, what)
+    if len(Ks) != len(images) or len(Es) != len(images):
+        raise ValueError(f"{what}: one K and one E per image, got {len(Ks)} and {len(Es)} for {len(images)} images")
+    if len(images) > 65535:
+        raise ValueError(f"{what}: at most 65535 views")
+    if nf:
+        lo, hi = (int(v) for v in torch.aminmax(fc))
+        if lo < 0 or hi >= nv:
+            raise ValueError(f"{what}: a face refers to a vertex outside 0..{nv - 1}")
+    table = texture_view_table(Ks, Es, sizes, mesh_box_centre(pts))
+    dev = pts.device
+    stats = {"textured_faces": 0, "untextured_faces": 0, "charts": 0, "pages": 0, "page_side": 0, "atlas_fill": 0.0}
+    if nf == 0:
+        return (torch.empty((0, 3, 2), dtype=torch.float32, device=dev), torch.empty(0, dtype=torch.int32, device=dev),
+                torch.empty((0, 4096, 4096, 3), dtype=torch.uint8, device=dev), stats)
+    lib = _native.lib()
+    V = len(images)
+    ws_bytes = lib.pmb200_texture_mesh_workspace_bytes(nv, nf, _addr(table), V)
+    if ws_bytes < 0:
+        _native.check(int(ws_bytes), "texture_mesh_workspace_bytes")
+    need = texture_mesh_bytes(nv, nf, sizes)
+    free = _free_bytes(dev)
+    if need > free:
+        raise ValueError(f"{what}: {nv} vertices, {nf} faces and {V} views need {need / 2 ** 30:.2f} GiB ({free / 2 ** 30:.2f} GiB free)")
+    import ctypes
+
+    ws = _workspace(ws_bytes, "texture_mesh_workspace_bytes", dev)
+    label = torch.empty(nf, dtype=torch.int32, device=dev)
+    slot = torch.empty(nf, dtype=torch.int32, device=dev)
+    charts = torch.empty((nf, 6), dtype=torch.int32, device=dev)
+    counts = (ctypes.c_int64 * 3)()
+    with _device_guard(pts):
+        rc = lib.pmb200_texture_mesh(pts.data_ptr(), nv, fc.data_ptr(), nf, _addr(table), V, label.data_ptr(), slot.data_ptr(),
+                                     charts.data_ptr(), counts, ws.data_ptr(), int(ws_bytes), _stream(pts))
+    _native.check(rc, what)
+    del ws
+    n_entries, n_charts, n_cells = (int(c) for c in counts)
+    table_h = np.ascontiguousarray(charts[:n_charts].cpu().numpy())
+    sizes_h = np.ascontiguousarray(table_h[:, 4:6])
+    places_h = np.zeros((n_charts + n_cells, 3), np.int32)
+    side, n_pages = ctypes.c_int(0), ctypes.c_int(0)
+    rc = lib.pmb200_texture_pack(sizes_h.ctypes.data, n_charts, n_cells, places_h.ctypes.data, ctypes.byref(side), ctypes.byref(n_pages))
+    _native.check(rc, "texture_pack")
+    S, P = side.value, n_pages.value
+    page_bytes = P * S * S * 3
+    free = _free_bytes(dev)
+    if page_bytes + 24 * nf > free:
+        raise ValueError(f"{what}: {P} pages of {S} x {S} texels need {page_bytes / 2 ** 30:.2f} GiB ({free / 2 ** 30:.2f} GiB free)")
+    pages = torch.zeros((P, S, S, 3), dtype=torch.uint8, device=dev)
+    places = torch.from_numpy(places_h).to(dev)
+    uv = torch.empty((nf, 3, 2), dtype=torch.float32, device=dev)
+    page = torch.empty(nf, dtype=torch.int32, device=dev)
+    wws = _workspace(lib.pmb200_texture_write_workspace_bytes(V), "texture_write_workspace_bytes", dev)
+    texels = table_h[:, 4].astype(np.int64) * table_h[:, 5]
+    for v in range(V):
+        rows = np.flatnonzero(table_h[:, 1] == v).astype(np.int32)
+        if rows.size == 0:
+            continue
+        prefix = np.zeros(rows.size + 1, np.int64)
+        np.cumsum(texels[rows], out=prefix[1:])
+        rows_d, prefix_d = torch.from_numpy(rows).to(dev), torch.from_numpy(prefix).to(dev)
+        img = images[v].contiguous()
+        with _device_guard(pts):
+            rc = lib.pmb200_texture_write(v, img.data_ptr(), sizes[v][1], sizes[v][0], rows_d.data_ptr(), prefix_d.data_ptr(), rows.size,
+                                          None, None, 0, None, 0, None, 0, None, None, charts.data_ptr(), places.data_ptr(), S, P,
+                                          None, None, pages.data_ptr(), wws.data_ptr(), wws.numel(), _stream(pts))
+        _native.check(rc, what + "_write")
+    with _device_guard(pts):
+        rc = lib.pmb200_texture_write(-1, None, 0, 0, None, None, 0, pts.data_ptr(), None if col is None else col.data_ptr(), nv,
+                                      fc.data_ptr(), nf, _addr(table), V, label.data_ptr(), slot.data_ptr(), charts.data_ptr(),
+                                      places.data_ptr(), S, P, uv.data_ptr(), page.data_ptr(), pages.data_ptr(), wws.data_ptr(),
+                                      wws.numel(), _stream(pts))
+    _native.check(rc, what + "_write")
+    stats.update({"textured_faces": nf - n_cells, "untextured_faces": n_cells, "charts": n_charts, "pages": P, "page_side": S,
+                  "atlas_fill": float(texels.sum()) / float(P * S * S) if P else 0.0, "entries": n_entries})
+    return uv, page, pages, stats
+
+
+def texture_labels(xyz: Tensor, faces: Tensor, images: Sequence[Tensor], Ks, Es):
+    """The selection alone (pmb200_texture_mesh): -> (label int32 [nf], -1 untextured; chart table int32 [n_charts,6]:
+    chart id, view, x0, y0, width, height; slot int32 [nf]; counts (entries, charts, untextured)) on the device."""
+    import ctypes
+
+    pts = _render_xyz(xyz, "texture_labels")
+    fc = faces.contiguous()
+    nv, nf = pts.shape[0], fc.shape[0]
+    sizes = _texture_images(images, pts, "texture_labels")
+    table = texture_view_table(Ks, Es, sizes, mesh_box_centre(pts))
+    lib = _native.lib()
+    ws_bytes = lib.pmb200_texture_mesh_workspace_bytes(nv, nf, _addr(table), len(images))
+    _native.check(min(int(ws_bytes), 0), "texture_mesh_workspace_bytes")
+    ws = _workspace(ws_bytes, "texture_mesh_workspace_bytes", pts.device)
+    label = torch.empty(nf, dtype=torch.int32, device=pts.device)
+    slot = torch.empty(nf, dtype=torch.int32, device=pts.device)
+    charts = torch.empty((max(nf, 1), 6), dtype=torch.int32, device=pts.device)
+    counts = (ctypes.c_int64 * 3)()
+    with _device_guard(pts):
+        rc = lib.pmb200_texture_mesh(pts.data_ptr(), nv, fc.data_ptr(), nf, _addr(table), len(images), label.data_ptr(),
+                                     slot.data_ptr(), charts.data_ptr(), counts, ws.data_ptr(), int(ws_bytes), _stream(pts))
+    _native.check(rc, "texture_mesh")
+    return label, charts[: int(counts[1])], slot, tuple(int(c) for c in counts)
+
+
+def texture_pack(sizes, n_cells: int):
+    """Host shelf packing (pmb200_texture_pack): sizes int [n,2] (width, height) -> (places int32 [n + n_cells,3] (page, x, y),
+    side, pages)."""
+    import ctypes
+
+    import numpy as np
+
+    sz = np.ascontiguousarray(np.asarray(sizes, np.int32).reshape(-1, 2))
+    places = np.zeros((sz.shape[0] + n_cells, 3), np.int32)
+    side, n_pages = ctypes.c_int(0), ctypes.c_int(0)
+    rc = _native.lib().pmb200_texture_pack(sz.ctypes.data, sz.shape[0], n_cells, places.ctypes.data, ctypes.byref(side), ctypes.byref(n_pages))
+    if rc == -1:
+        raise ValueError(_native.lib().pmb200_last_error().decode("utf-8", "replace"))
+    _native.check(rc, "texture_pack")
+    return places, side.value, n_pages.value
+
+
+def render_mesh_textured(xyz: Tensor, faces: Tensor, uv: Tensor, page: Tensor, pages: Tensor, P, width: int, height: int, near: float,
+                         shade: bool = False, background=(255, 255, 255)) -> Tuple[Tensor, Tensor]:
+    """render_mesh with a texture (pmb200_render_mesh_textured): each pixel takes the nearest texel of its perspective-correct
+    texture coordinate.  uv float32 [nf,3,2], page int32 [nf], pages uint8 [P,S,S,3] on the vertices' device."""
+    what = "render_mesh_textured"
+    pts = _render_xyz(xyz, what)
+    nv = pts.shape[0]
+    if not isinstance(faces, Tensor) or not _on_device(faces) or faces.dtype != torch.int32 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError(f"{what}: faces must be a CUDA int32 [nf,3] tensor")
+    fc = faces.contiguous()
+    nf = fc.shape[0]
+    if tuple(uv.shape) != (nf, 3, 2) or uv.dtype != torch.float32 or tuple(page.shape) != (nf,) or page.dtype != torch.int32:
+        raise ValueError(f"{what}: uv must be float32 [nf,3,2] and page int32 [nf]")
+    if pages.dtype != torch.uint8 or pages.dim() != 4 or pages.shape[1] != pages.shape[2] or pages.shape[3] != 3:
+        raise ValueError(f"{what}: pages must be uint8 [P,S,S,3]")
+    for t in (fc, uv, page, pages):
+        if not _on_device(t) or t.device != pts.device:
+            raise ValueError(f"{what}: every tensor must be on the vertices' CUDA device")
+    if nf:
+        lo, hi = (int(v) for v in torch.aminmax(fc))
+        if lo < 0 or hi >= nv:
+            raise ValueError(f"{what}: a face refers to a vertex outside 0..{nv - 1}")
+    p_host, c_host, bg = _render_args(P, width, height, near, background, what)
+    lib = _native.lib()
+    ws = _workspace(lib.pmb200_render_mesh_workspace_bytes(width, height, nv, nf), "render_mesh_workspace_bytes", pts.device)
+    out_rgb = torch.empty((height, width, 3), dtype=torch.uint8, device=pts.device)
+    out_depth = torch.empty((height, width), dtype=torch.float32, device=pts.device)
+    uvc, pgc, pagesc = uv.contiguous(), page.contiguous(), pages.contiguous()
+    with _device_guard(pts):
+        rc = lib.pmb200_render_mesh_textured(pts.data_ptr(), nv, fc.data_ptr(), nf, uvc.data_ptr(), pgc.data_ptr(), pagesc.data_ptr(),
+                                             pagesc.shape[0], max(int(pagesc.shape[1]), 1), p_host, c_host, width, height, float(near),
+                                             1 if shade else 0, bg, out_rgb.data_ptr(), out_depth.data_ptr(), ws.data_ptr(), ws.numel(),
+                                             _stream(pts))
+    _native.check(rc, what)
+    return out_rgb, out_depth

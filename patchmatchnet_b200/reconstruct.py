@@ -51,6 +51,8 @@ the truncation and the observations a voxel needs.  The volume needs blocks * 51
 With --mesh-target-faces N the mesh is also simplified on the GPU (ops.simplify_mesh: quadric edge collapse in rounds of
 independent collapses) to at most N faces and written to <scan>/mesh_simplified.ply; --mesh-min-component-faces F first
 drops connected pieces of fewer than F faces.  mesh.ply is the same with or without these options.
+With --mesh-texture the simplified mesh (the mesh without --mesh-target-faces) is also textured from the scan's reference
+views (ops.texture_mesh) and written as <scan>/mesh_textured.obj, .mtl and mesh_textured_NN.png.
 tnt_eval scores a Tanks and Temples training scene's fused.ply (or its mesh.ply) by precision, recall and F-score.
 
 Device memory held besides the engines, for a scan of n_img images of H x W and n_ref reference views:
@@ -128,16 +130,19 @@ def build_parser() -> argparse.ArgumentParser:
                     help="with --mesh, also write mesh_simplified.ply: quadric edge collapse to at most this many faces, on the GPU")
     ap.add_argument("--mesh-min-component-faces", type=int, default=argparse.SUPPRESS,
                     help="with --mesh-target-faces, first remove connected pieces with fewer faces than this (default 0: none)")
+    ap.add_argument("--mesh-texture", action="store_true", default=argparse.SUPPRESS,
+                    help="with --mesh, also write mesh_textured.obj (.mtl, _NN.png): the simplified mesh (or the mesh) textured "
+                         "from the reference views, on the GPU")
     return ap
 
 
 MESH_DEFAULTS = {"mesh": False, "mesh_voxel_size": None, "mesh_trunc": 3, "mesh_min_weight": 1, "mesh_target_faces": None,
-                 "mesh_min_component_faces": None}
+                 "mesh_min_component_faces": None, "mesh_texture": False}
 
 
 def mesh_options(args: argparse.Namespace) -> argparse.Namespace:
-    """--mesh, --mesh-voxel-size, --mesh-trunc, --mesh-min-weight, --mesh-target-faces and --mesh-min-component-faces of
-    `args`, with their defaults where not given."""
+    """--mesh, --mesh-voxel-size, --mesh-trunc, --mesh-min-weight, --mesh-target-faces, --mesh-min-component-faces and
+    --mesh-texture of `args`, with their defaults where not given."""
     return argparse.Namespace(**{k: getattr(args, k, v) for k, v in MESH_DEFAULTS.items()})
 
 
@@ -166,6 +171,8 @@ def check_args(args: argparse.Namespace) -> List[str]:
         raise ValueError(f"--mesh-target-faces needs --mesh and a value >= 0, got {m.mesh_target_faces}")
     if m.mesh_min_component_faces is not None and (m.mesh_target_faces is None or m.mesh_min_component_faces < 0):
         raise ValueError(f"--mesh-min-component-faces needs --mesh-target-faces and a value >= 0, got {m.mesh_min_component_faces}")
+    if m.mesh_texture and not m.mesh:
+        raise ValueError("--mesh-texture needs --mesh")
     if m.mesh:
         if m.mesh_voxel_size is not None and not (0 < m.mesh_voxel_size < float("inf")):
             raise ValueError(f"--mesh-voxel-size must be positive and finite, got {m.mesh_voxel_size}")
@@ -411,7 +418,19 @@ def mesh_scan(args: argparse.Namespace, bank: SceneBank, refs: Sequence[int], de
         data_io.save_ply(os.path.join(os.path.dirname(path), "mesh_simplified.ply"), body, sfaces)
         out.update({"simplified_vertices": int(body.shape[0]), "simplified_faces": int(sfaces.shape[0]), "simplify_rounds": rounds,
                     "simplify_seconds": time.perf_counter() - t0})
+    if m.mesh_texture:
+        from .texture import texture_and_save
+
+        tb, tf = (body, sfaces) if m.mesh_target_faces is not None else (verts, faces)
+        xyz = tb[:, :12].contiguous().view(torch.float32)
+        rgb = tb[:, 12:15].contiguous() if tb.shape[1] >= 15 else None
+        st = texture_and_save(xyz, rgb, tf, [bank.images[r] for r in refs], Ks, [bank.extrinsics[r] for r in refs],
+                              os.path.join(os.path.dirname(path), "mesh_textured"))
+        out.update({k: st[k] for k in TEXTURE_STATS})
     return out
+
+
+TEXTURE_STATS = ("texture_charts", "texture_pages", "texture_untextured_faces", "texture_seconds", "texture_write_seconds")
 
 
 def fuse_scan(args: argparse.Namespace, scan: str, bank: SceneBank, pairs: Sequence[Tuple[int, List[int]]], maps,
@@ -475,6 +494,8 @@ def reconstruct(args: argparse.Namespace, *, device: str = "cuda:0", n_slots: in
         stats.update({"mesh_vertices": 0, "mesh_faces": 0, "mesh_seconds": 0.0})
     if mesh_options(args).mesh_target_faces is not None:
         stats.update({"simplified_vertices": 0, "simplified_faces": 0, "simplify_rounds": 0, "simplify_seconds": 0.0})
+    if mesh_options(args).mesh_texture:
+        stats.update(dict.fromkeys(TEXTURE_STATS, 0))
     t_start = time.perf_counter()
     with precision(args.tf32), torch.cuda.device(dev), torch.no_grad():
         stage = DepthStage(load_network(args).to(dev), dev, n_slots=n_slots, seed=args.seed) if do_depth else None

@@ -6,7 +6,8 @@ visualize_ply.py, which opens an Open3D window and so needs a display.
     python -m patchmatchnet_b200.render --ply results/fused.ply --viewpoint viewpoint.json --point-size 3 --output-folder renders
 
 The PLY is read once (data_io.read_ply) and uploaded once; a file with faces renders as a mesh (ops.render_mesh), any other
-as points (ops.render_points).  Cameras, which may be combined:
+as points (ops.render_points).  A textured OBJ (data_io.save_obj's, e.g. from the texture command) renders with its
+texture (ops.render_mesh_textured: the nearest texel of the perspective-correct texture coordinate).  Cameras, which may be combined:
   --views ID ...     the views' cams/%08d_cam.txt under --input-folder, intrinsics scaled to the image size as reconstruct
                      scales them (with --image-max-dim); image sizes come from the image headers.  -> view_%08d.png
   --orbit N          N frames on a circle around the centre of the per-axis 1st-99th percentile box of the vertices, at
@@ -40,7 +41,7 @@ DEFAULT_UP = (0.0, -1.0, 0.0)
 
 def build_parser() -> argparse.ArgumentParser:
     ap = argparse.ArgumentParser(prog="python -m patchmatchnet_b200.render", description="Render a PLY cloud or mesh to PNG images")
-    ap.add_argument("--ply", type=str, required=True, help="PLY point cloud or triangle mesh")
+    ap.add_argument("--ply", type=str, required=True, help="PLY point cloud or triangle mesh, or a textured .obj")
     ap.add_argument("--output-folder", type=str, default="renders", help="where the images go")
     ap.add_argument("--input-folder", type=str, default="", help="scene folder (cams/, images/) for --views and the default up")
     ap.add_argument("--views", nargs="+", type=int, default=[], help="render from these scene views")
@@ -234,7 +235,12 @@ def render(args: argparse.Namespace, *, device: str = "cuda:0", log=print) -> Di
     dev = torch.device(device)
     stats = {"read_seconds": 0.0, "upload_seconds": 0.0, "render_seconds": 0.0, "write_seconds": 0.0}
     t_start = time.perf_counter()
-    xyz, rgb, normals, faces = data_io.read_ply(args.ply)
+    textured = args.ply.lower().endswith(".obj")
+    if textured:
+        xyz, faces, uv, page, pages = data_io.read_obj(args.ply)
+        rgb = normals = None
+    else:
+        xyz, rgb, normals, faces = data_io.read_ply(args.ply)
     t0 = time.perf_counter()
     stats["read_seconds"] = t0 - t_start
     with torch.cuda.device(dev):
@@ -242,6 +248,8 @@ def render(args: argparse.Namespace, *, device: str = "cuda:0", log=print) -> Di
         d_rgb = torch.from_numpy(rgb).to(dev) if rgb is not None else None
         d_nrm = torch.from_numpy(normals).to(dev) if normals is not None else None
         d_faces = torch.from_numpy(faces).to(dev) if faces is not None else None
+        if textured:
+            d_uv, d_page, d_pages = torch.from_numpy(uv).to(dev), torch.from_numpy(page).to(dev), torch.from_numpy(pages).to(dev)
         torch.cuda.synchronize(dev)
         t1 = time.perf_counter()
         stats["upload_seconds"] = t1 - t0
@@ -252,7 +260,10 @@ def render(args: argparse.Namespace, *, device: str = "cuda:0", log=print) -> Di
         for stem, P, w, h in todo:
             t1 = time.perf_counter()
             near = args.near if args.near is not None else 1e-3 * max(float(np.linalg.norm(camera_centre(P) - centre)), 1e-30)
-            if d_faces is not None:
+            if textured:
+                img, depth = ops.render_mesh_textured(d_xyz, d_faces, d_uv, d_page, d_pages, P, w, h, near, shade=args.shade,
+                                                      background=args.background)
+            elif d_faces is not None:
                 img, depth = ops.render_mesh(d_xyz, d_rgb, d_faces, P, w, h, near, shade=args.shade, background=args.background,
                                              check_faces=False)  # read_ply checked the indices
             else:
