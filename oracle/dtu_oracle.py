@@ -5,6 +5,8 @@ MATLAB scripts step by step, in float64:
 
     thin              reducePts_haa.m: the literal sequential loop over the visiting order -- a point still in the set
                       removes every point within distance <= dst of it, then puts itself back
+    thin_violations   a vectorised check of a keep mask against `thin` for clouds too big for its Python loop
+    thin_sync_rounds  the rounds a synchronous parallel thinning needs, and its keep mask
     max_dist_cp       MaxDistCP.m: the literal loop over the max_dist blocks of BB, a nearest-neighbour search per block into
                       the "to" points of the block widened by max_dist, max_dist where that set is empty or the point is in
                       no block (values above max_dist are kept, as the script keeps them)
@@ -46,6 +48,90 @@ def thin(points: np.ndarray, order: np.ndarray, dst: float) -> np.ndarray:
             keep[c[_dist(points[c], points[i]) <= dst]] = False
             keep[i] = True
     return keep
+
+
+# thin's result is the one set in which a point is kept iff no kept point u != v with dist(u, v) <= dst comes before it in the
+# visiting order: the loop's result has that property, and by induction over the order no other set does.  So a mask equals
+# thin's iff every point passes that local test, which needs only the kept points' neighbourhoods.
+
+def rank_of(order: np.ndarray) -> np.ndarray:
+    """Visiting order (point indices, first visited first) -> rank[i], the position at which point i is visited."""
+    order = np.asarray(order, dtype=np.int64)
+    rank = np.empty(order.size, dtype=np.int64)
+    rank[order] = np.arange(order.size, dtype=np.int64)
+    return rank
+
+
+def _exact_within(points: np.ndarray, a: np.ndarray, b: np.ndarray, dst: float) -> np.ndarray:
+    """_dist's expression on index pairs (any matching shapes): dist(points[a], points[b]) <= dst."""
+    d = points[a] - points[b]
+    return np.sqrt((d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]) + d[..., 2] * d[..., 2]) <= dst
+
+
+THIN_CHECK_K = 24     # kept points are pairwise more than dst apart: at most 13 fit in a ball of radius dst (12 + centre)
+THIN_CHECK_CHUNK = 1 << 20
+
+
+def thin_violations(points: np.ndarray, rank: np.ndarray, keep: np.ndarray, dst: float) -> np.ndarray:
+    """Indices v where keep[v] differs from "no kept u != v within dst has rank[u] < rank[v]" (rank[i]: visiting position of
+    point i).  Empty iff keep == thin(points, order, dst) for the order whose ranks these are."""
+    points = np.asarray(points, dtype=np.float64)
+    rank = np.asarray(rank, dtype=np.int64)
+    keep = np.asarray(keep, dtype=bool)
+    n = points.shape[0]
+    kept = np.nonzero(keep)[0]
+    if kept.size == 0:
+        return np.arange(n) if n else np.zeros(0, dtype=np.int64)
+    tree = cKDTree(points[kept])
+    bad = []
+    for a in range(0, n, THIN_CHECK_CHUNK):
+        v = np.arange(a, min(n, a + THIN_CHECK_CHUNK))
+        d, j = tree.query(points[v], k=THIN_CHECK_K, distance_upper_bound=dst * (1 + 1e-9), workers=-1)
+        # a saturated query could hide a neighbour; only a mask keeping points within dst of each other saturates
+        if np.isfinite(d[:, -1]).any():
+            raise AssertionError(f"thin_violations: more than {THIN_CHECK_K - 1} kept points within dst of one point")
+        u = kept[np.where(np.isfinite(d), j, 0)]
+        nb = np.isfinite(d) & (u != v[:, None]) & _exact_within(points, u, v[:, None], dst)
+        earlier = (nb & (rank[u] < rank[v][:, None])).any(axis=1)
+        bad.append(v[keep[v] == earlier])
+    return np.concatenate(bad)
+
+
+def thin_pairs(points: np.ndarray, dst: float) -> np.ndarray:
+    """Every unordered pair [i, j] (i < j) with dist <= dst in _dist's expression -> int64 [m, 2]."""
+    points = np.asarray(points, dtype=np.float64)
+    if points.shape[0] < 2:
+        return np.zeros((0, 2), dtype=np.int64)
+    pairs = cKDTree(points).query_pairs(dst * (1 + 1e-9), output_type="ndarray").astype(np.int64)
+    return pairs[_exact_within(points, pairs[:, 0], pairs[:, 1], dst)]
+
+
+def thin_sync_rounds(points: np.ndarray, rank: np.ndarray, dst: float):
+    """The thinning as synchronous rounds: in each, an undecided point is rejected if an earlier neighbour is accepted and
+    accepted if every earlier neighbour is decided, all reading the state the round started with.  -> (rounds, keep).
+    keep equals thin's.  A parallel thinning whose points also read decisions made earlier in the same round, decisions
+    being final, needs at most `rounds` rounds."""
+    points = np.asarray(points, dtype=np.float64)
+    rank = np.asarray(rank, dtype=np.int64)
+    n = points.shape[0]
+    pairs = thin_pairs(points, dst)
+    first = rank[pairs[:, 0]] < rank[pairs[:, 1]]
+    early = np.where(first, pairs[:, 0], pairs[:, 1])
+    late = np.where(first, pairs[:, 1], pairs[:, 0])
+    undecided, accepted, rejected = 0, 1, 2
+    state = np.full(n, undecided, dtype=np.int8)
+    rounds = 0
+    while (state == undecided).any():
+        rounds += 1
+        s = state[early]
+        blocked = np.zeros(n, dtype=bool)
+        blocked[late[s == undecided]] = True
+        hit = np.zeros(n, dtype=bool)
+        hit[late[s == accepted]] = True
+        open_ = state == undecided
+        state[open_ & hit] = rejected
+        state[open_ & ~hit & ~blocked] = accepted
+    return rounds, state == accepted
 
 
 def max_dist_cp(q_to: np.ndarray, q_from: np.ndarray, bb: np.ndarray, max_dist: float) -> np.ndarray:

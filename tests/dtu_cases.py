@@ -32,10 +32,16 @@ def make_scan(seed: int, n_stl: int = 20000, n_data: int = 40000, side: float = 
     hi = stl.max(axis=0) + 40.0
     data[:n_out] = rng.uniform(lo - 40.0, hi + 40.0, (n_out, 3))  # some fall outside BB and its blocks on purpose
     data = data[rng.permutation(n_data)].astype(np.float32).astype(np.float64)
+    return {"data": data, "stl": stl, **scan_truth(stl, lo, hi, res)}
+
+
+def scan_truth(stl: np.ndarray, lo: np.ndarray, hi: np.ndarray, res: float):
+    """bb = [lo, hi], the observation mask (voxels of `res` within 10 mm of an STL point, per axis) and the plane near the
+    base of the STL cloud -> {"obs_mask", "bb", "res", "plane"}."""
     bb = np.stack([lo, hi]).astype(np.float64)
     dims = np.ceil((hi - lo) / res).astype(int) + 1
     mask = np.zeros(dims, dtype=bool)
-    vox = np.floor((stl - lo) / res).astype(int)
+    vox = np.unique(np.floor((stl - lo) / res).astype(int), axis=0)
     r = int(np.ceil(10.0 / res))
     for dx in range(-r, r + 1):
         for dy in range(-r, r + 1):
@@ -44,7 +50,7 @@ def make_scan(seed: int, n_stl: int = 20000, n_data: int = 40000, side: float = 
                 mask[v[:, 0], v[:, 1], v[:, 2]] = True
     z0 = float(np.percentile(stl[:, 2], 10))
     plane = np.array([0.05, 0.0, 1.0, -z0], dtype=np.float64)  # above: 0.05 x + z > z0
-    return {"data": data, "stl": stl, "obs_mask": mask, "bb": bb, "res": float(res), "plane": plane}
+    return {"obs_mask": mask, "bb": bb, "res": float(res), "plane": plane}
 
 
 def ply_bytes(points: np.ndarray, colours: bool = True) -> bytes:

@@ -15,7 +15,7 @@ import torch
 
 from oracle import dtu_oracle as do
 from patchmatchnet_b200 import _native, data_io, dtu_eval
-from tests import dtu_cases
+from tests import dtu_cases, dtu_scale_cases
 
 
 # ---- thinning ---------------------------------------------------------------------------------------------------------------
@@ -39,6 +39,110 @@ def test_thin_duplicates():
     # the first visited copy survives, the other copies are at distance 0; the point 0.3 away is beyond dst = 0.25
     assert do.thin(pts, [2, 0, 1, 3], 0.25).tolist() == [False, False, True, True]
     assert do.thin(pts, [3, 1, 0, 2], 0.25).tolist() == [False, True, False, True]
+
+
+def _clouds():
+    """The thinning cases of tests/test_gpu_dtu_eval.py."""
+    rng = np.random.RandomState(11)
+    uniform = rng.uniform(0.0, 10.0, (50000, 3))
+    # 220k samples of a 60 x 60 mm surface: ~60 points per mm^2, about 7 neighbours within 0.2 mm
+    x, y = rng.uniform(0, 60, 220000), rng.uniform(0, 60, 220000)
+    clustered = np.stack([x, y, 3.0 * np.sin(x / 5.0) + 0.01 * x * y], axis=1).astype(np.float32).astype(np.float64)
+    base = rng.uniform(0.0, 5.0, (6000, 3)).astype(np.float32).astype(np.float64)
+    duplicates = np.concatenate([base, base[:3000], base[:1000]])
+    g = np.arange(20) * 0.25  # exact lattice: every neighbour exactly dst = 0.25 apart
+    lattice = np.stack(np.meshgrid(g, g, g, indexing="ij"), axis=-1).reshape(-1, 3) + 1000.0
+    return [("uniform", uniform, 0.2), ("clustered", clustered, 0.2), ("duplicates", duplicates, 0.2), ("lattice", lattice, 0.25)]
+
+
+# ---- the checker and the round count of thinning at scan sizes (tests/dtu_scale_cases.py) ------------------------------------
+
+def _thin_rows():
+    rows = [(name, {"points": p, "dst": dst, "order": dtu_eval.visiting_order(p.shape[0], 7 + i)})
+            for i, (name, p, dst) in enumerate(_clouds())]
+    return rows + [("literal", dtu_scale_cases.literal(0))]
+
+
+def test_thin_violations_accepts_the_sequential_oracle():
+    for name, r in _thin_rows():
+        keep = do.thin(r["points"], r["order"], r["dst"])
+        assert do.thin_violations(r["points"], do.rank_of(r["order"]), keep, r["dst"]).size == 0, name
+        assert 0 < keep.sum() < keep.size, name
+
+
+def test_thin_violations_reports_planted_errors():
+    r = dtu_scale_cases.literal(0)
+    pts, dst, order = r["points"], r["dst"], r["order"]
+    rank = do.rank_of(order)
+    keep = do.thin(pts, order, dst)
+    removed, kept = np.nonzero(~keep)[0][0], np.nonzero(keep)[0][0]
+    flipped = keep.copy()
+    flipped[removed] = True
+    assert removed in do.thin_violations(pts, rank, flipped, dst)
+    flipped = keep.copy()
+    flipped[kept] = False
+    assert kept in do.thin_violations(pts, rank, flipped, dst)
+    # a kept point a and a point b that only a removed trade places in the visiting order: b is kept and a removed in that
+    # order's mask, which is wrong for this one
+    pairs = do.thin_pairs(pts, dst)
+    pairs = np.concatenate([pairs, pairs[:, ::-1]])
+    kept_nbrs = np.bincount(pairs[keep[pairs[:, 0]], 1], minlength=keep.size)
+    a, b = pairs[keep[pairs[:, 0]] & ~keep[pairs[:, 1]] & (kept_nbrs[pairs[:, 1]] == 1)][0]
+    swapped = np.asarray(order).copy()
+    swapped[rank[a]], swapped[rank[b]] = b, a
+    other = do.thin(pts, swapped, dst)
+    assert other[b] and not other[a]
+    assert do.thin_violations(pts, rank, other, dst).size > 0
+    assert do.thin_violations(pts, do.rank_of(swapped), other, dst).size == 0
+
+
+def test_thin_sync_rounds_hand_case():
+    # 0 accepted; 1 rejected while 2 waits for it; 2 accepted; 3 rejected; 4 accepted
+    rounds, keep = do.thin_sync_rounds(_line([0.0, 0.25, 0.5, 0.75, 1.0]), np.arange(5), 0.25)
+    assert rounds == 5 and keep.tolist() == [True, False, True, False, True]
+    rounds, keep = do.thin_sync_rounds(_line([0.0, 0.25, 0.5, 0.75, 1.0]), do.rank_of([1, 0, 2, 3, 4]), 0.25)
+    assert rounds == 4 and keep.tolist() == [False, True, False, True, False]
+
+
+@pytest.mark.parametrize("row", ["literal", "stack"])
+def test_thin_sync_rounds_is_the_oracle_far_below_the_native_round_bound(row):
+    """Random visiting orders at DTU densities settle in a few rounds: 12 and 14 here against the bound of 256.  `stack` at
+    50k points has the neighbour counts of the 200k row the GPU tests run, at a cost the sequential oracle can pay."""
+    r = dtu_scale_cases.literal(0) if row == "literal" else dtu_scale_cases.stack(0, n=50_000)
+    rounds, keep = do.thin_sync_rounds(r["points"], do.rank_of(r["order"]), r["dst"])
+    assert (keep == do.thin(r["points"], r["order"], r["dst"])).all()
+    assert rounds <= 32
+
+
+@pytest.mark.parametrize("decreasing", [False, True])
+def test_chain_needs_more_rounds_than_the_native_bound(decreasing):
+    r = dtu_scale_cases.chain(decreasing)
+    rounds, keep = do.thin_sync_rounds(r["points"], do.rank_of(r["order"]), r["dst"])
+    assert rounds > dtu_scale_cases.THIN_ROUND_BOUND
+    assert (keep == do.thin(r["points"], r["order"], r["dst"])).all()
+    first = r["order"][0]
+    assert keep[first] and (keep[::2] != keep[1::2]).all()  # every other point along the chain, from the first visited
+
+
+def test_scale_rows_are_pinned():
+    sc = dtu_scale_cases
+    s = sc.sheets(0)
+    assert s["data"].shape[0] > 2 ** 24 and s["stl"].shape[0] == sc.N_STL
+    assert (s["data"].astype(np.float32).astype(np.float64) == s["data"]).all()
+    rng = np.floor((s["bb"][1] - s["bb"][0]) / 60.0) + 1
+    assert rng.tolist() == [6.0, 6.0, 3.0]  # MaxDistCP blocks per axis
+    for pts in (s["data"], sc.literal(0)["points"]):  # about 23 neighbours within dst, at most about 50
+        counts = sc.neighbour_counts(pts, sc.DST, [-2.5, -2.5, -np.inf], [2.5, 2.5, np.inf])
+        assert 18 < counts.mean() < 28 and counts.size > 7000
+    st = sc.stack(0)["points"]
+    assert st.shape[0] == 200_000 and np.unique(st, axis=0).shape[0] < 0.92 * st.shape[0]
+    counts = sc.neighbour_counts(st, sc.DST, [-0.5, -0.5, -np.inf], [0.5, 0.5, np.inf])
+    assert 400 < counts.mean() < 1000
+    lat = sc.lattice(0)
+    inner = sc.neighbour_counts(lat["points"], lat["dst"], [1000.2] * 3, [1024.6] * 3)
+    assert lat["points"].shape[0] == 10 ** 6 and (inner == 6).all()  # exactly dst apart along the axes, nothing closer
+    ch = sc.chain()
+    assert (sc.neighbour_counts(ch["points"], sc.DST, [-np.inf] * 3, [np.inf] * 3) == [1] + [2] * 2998 + [1]).all()
 
 
 # ---- MaxDistCP ----------------------------------------------------------------------------------------------------------------

@@ -16,7 +16,7 @@ import torch
 from oracle import dtu_oracle as do
 from patchmatchnet_b200 import dtu_eval, ops
 from tests import dtu_cases
-from tests.test_dtu_eval import BLOCK_BB, BLOCK_FROM, BLOCK_TO
+from tests.test_dtu_eval import BLOCK_BB, BLOCK_FROM, BLOCK_TO, _clouds
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -28,19 +28,6 @@ def _gpu_thin(points, order, dst):
     rank[np.asarray(order, dtype=np.int64)] = np.arange(len(order), dtype=np.int32)
     keep = ops.thin_points(torch.as_tensor(points, device=DEV), torch.as_tensor(rank, device=DEV), dst)
     return keep.cpu().numpy()
-
-
-def _clouds():
-    rng = np.random.RandomState(11)
-    uniform = rng.uniform(0.0, 10.0, (50000, 3))
-    # 220k samples of a 60 x 60 mm surface: ~60 points per mm^2, about 7 neighbours within 0.2 mm
-    x, y = rng.uniform(0, 60, 220000), rng.uniform(0, 60, 220000)
-    clustered = np.stack([x, y, 3.0 * np.sin(x / 5.0) + 0.01 * x * y], axis=1).astype(np.float32).astype(np.float64)
-    base = rng.uniform(0.0, 5.0, (6000, 3)).astype(np.float32).astype(np.float64)
-    duplicates = np.concatenate([base, base[:3000], base[:1000]])
-    g = np.arange(20) * 0.25  # exact lattice: every neighbour exactly dst = 0.25 apart
-    lattice = np.stack(np.meshgrid(g, g, g, indexing="ij"), axis=-1).reshape(-1, 3) + 1000.0
-    return [("uniform", uniform, 0.2), ("clustered", clustered, 0.2), ("duplicates", duplicates, 0.2), ("lattice", lattice, 0.25)]
 
 
 @pytest.mark.parametrize("idx", range(4), ids=["uniform", "clustered", "duplicates", "lattice"])
