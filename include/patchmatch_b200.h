@@ -339,6 +339,83 @@ int pmb200_tsdf_mesh_write(const uint64_t *block_keys, int64_t n_blocks, double 
                            int *faces_out, void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------
+ * Poisson surface reconstruction of oriented points (beyond the reference, which has no mesher; INTEGRATION.md "Poisson
+ * surface reconstruction (beyond the reference)").  Definition:
+ *
+ * Input.  xyz float32 [n,3], normals float32 [n,3], optionally rgb uint8 [n,3]; n < 2^28.  A point is kept when its xyz is
+ * finite and its normal is finite with a float64 length > 0; the kept normal is divided by that length in float64.
+ *
+ * Grid.  depth d in 5..10, N = 2^d.  The box runs per axis from the q quantile to the 1 - q quantile of the kept points'
+ * coordinates (q = bbox_quantile in [0, 0.5); q = 0 is the exact bounding box).  The q quantile of m sorted values v is
+ * v[g] + t (v[g+1] - v[g]) with pos = q (m - 1), g = floor(pos), t = pos - g (v[g+1] = v[g] at the end).  E is the box's largest
+ * extent and c its centre (float64), h = scale E / N (scale >= 1), I0 = floor(c / h) - N / 2 per axis.  Node i, i in 0..N
+ * per axis, is TSDF voxel I0 + i: it sits at (I0 + i + 0.5) h, so the grid is a box of the TSDF mesher's lattice with voxel
+ * size h.  Grid coordinates: u = p / h - 0.5 - I0 (float64, in that order), node i at u = i.  A kept point stays when
+ * 0 <= u <= N on every axis (always with q = 0, since scale >= 1); the others are dropped.  Boundary nodes (an index 0 or N)
+ * have chi = 0; the interior nodes are the unknowns.
+ *
+ * Density and weights.  A point's cell is floor(u) (N - 1 at u = N), f = u - cell, and the hat of node i is
+ * phi_i(u) = prod_a max(0, 1 - |u_a - i_a|), its gradient taken inside the point's cell.  rho_i = sum_p phi_i(u_p),
+ * rho(p) = sum_i phi_i(u_p) rho_i (the 8 corners of the cell, x fastest), w_p = 1 / rho(p).
+ *
+ * System.  Trilinear finite elements in grid units: A_ij = integral grad phi_i . grad phi_j, the 27-point stencil with 8/3
+ * at the centre, 0 at the 6 face, -1/6 at the 12 edge and -1/12 at the 8 corner neighbours (K(x)M(x)M + M(x)K(x)M +
+ * M(x)M(x)K with K = [-1, 2, -1], M = [1, 4, 1] / 6), and b_i = sum_p w_p n_p . grad phi_i(u_p), rounded to float32.  Solve
+ * A chi = b over the interior nodes with V(2,2) multigrid cycles in float32 (Jacobi smoothing; level l uses the stencil
+ * times 2^l, since P^T A_h P = 2 A_2h for trilinear prolongation P; the coarsest level, N = 2, is solved exactly) until
+ * ||b - A chi||_2 / ||b||_2 <= tol or max_cycles cycles.  Normals point outward, so chi is 0 outside and about -1 inside.
+ * iso = sum_p w_p chi(u_p) / sum_p w_p with trilinear chi.  b = 0 gives chi = 0, iso = 0 and an empty mesh.
+ *
+ * Extraction.  pmb200_tsdf_alloc of the points that stay, with voxel size h and trunc = band (1..4); every allocated voxel
+ * that is an interior node gets tsdf = float32(chi - iso) and weight 1, every other voxel weight 0; pmb200_tsdf_mesh_count
+ * and _write with min_weight 1.  tsdf is positive on the normals' side, so faces are wound towards the cameras.  Each vertex
+ * takes the colour of the nearest point that stays, by float64 Euclidean distance, ties to the smaller point index.
+ *
+ * Determinism.  rho and b are sums of 64-bit fixed-point atomics (units of 2^-32); the norms and the iso-value are float64
+ * sums over a fixed grid of CTAs reduced in a fixed order.  Reruns are bit-identical.
+ *
+ * Calls (device pointers unless marked HOST; *_workspace_bytes returns bytes or a negative PMB200_E*):
+ *   pmb200_poisson_setup: the keep test, the box, the grid and the compaction of the points that stay into the workspace;
+ *       grid_out (HOST) receives the grid and the counts; two host synchronisations.  h = 0 in grid_out when no point is
+ *       kept or E = 0.  PMB200_EINVAL for a null pointer, n outside 0..2^28-1, depth outside 5..10, scale < 1 or not finite,
+ *       bbox_quantile outside [0, 0.5), or a workspace smaller than pmb200_poisson_workspace_bytes(depth, n).
+ *   pmb200_poisson_density: rho and w.  Optional outputs: rho_out double [(N+1)^3] (x fastest), w_out double [n_inside].
+ *   pmb200_poisson_rhs: b.  Optional output: b_out float32 [(N+1)^3].
+ *   pmb200_poisson_solve: the multigrid and the iso-value; result_out (HOST).  One host read per cycle.  Optional output:
+ *       chi_out float32 [(N+1)^3].
+ *   pmb200_poisson_band: tsdf_out, weight_out float32 [n_blocks * 512] over the blocks pmb200_tsdf_alloc returned.
+ *   pmb200_poisson_colours: overwrites red, green, blue of the vertex records [nv,15] pmb200_tsdf_mesh_write wrote; needs rgb
+ *       at setup.
+ * Each later call takes the grid setup returned and the same workspace, in this order; all but setup and solve only enqueue. */
+typedef struct pmb200_poisson_grid {
+    int32_t depth, N;
+    double h;
+    int64_t I0[3];
+    double lo[3], hi[3];                      /* the box */
+    int64_t n_points, n_kept, n_inside;       /* input points, kept points, kept points inside the node box */
+    int64_t points_offset;                    /* bytes from the workspace's start: float32 [n_inside,3], the points that stay */
+    int32_t has_rgb, reserved;
+} pmb200_poisson_grid;
+
+typedef struct pmb200_poisson_result {
+    int32_t cycles, converged;
+    double residual, iso;                     /* final ||b - A chi|| / ||b|| (0 when b = 0), the iso-value */
+} pmb200_poisson_result;
+
+int64_t pmb200_poisson_workspace_bytes(int depth, int64_t n_points);
+int pmb200_poisson_setup(const float *xyz, const float *normals, const unsigned char *rgb, int64_t n_points, int depth, double scale,
+                         double bbox_quantile, pmb200_poisson_grid *grid_out, void *workspace, int64_t workspace_bytes, void *stream);
+int pmb200_poisson_density(const pmb200_poisson_grid *grid, double *rho_out, double *w_out, void *workspace, int64_t workspace_bytes,
+                           void *stream);
+int pmb200_poisson_rhs(const pmb200_poisson_grid *grid, float *b_out, void *workspace, int64_t workspace_bytes, void *stream);
+int pmb200_poisson_solve(const pmb200_poisson_grid *grid, double tol, int max_cycles, pmb200_poisson_result *result_out, float *chi_out,
+                         void *workspace, int64_t workspace_bytes, void *stream);
+int pmb200_poisson_band(const pmb200_poisson_grid *grid, double iso, const uint64_t *block_keys, int64_t n_blocks, float *tsdf_out,
+                        float *weight_out, void *workspace, int64_t workspace_bytes, void *stream);
+int pmb200_poisson_colours(const pmb200_poisson_grid *grid, unsigned char *vertices, int64_t n_vertices, void *workspace,
+                           int64_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------
  * Mesh simplification: Garland-Heckbert quadric edge collapse in rounds of independent collapses, with removal of small
  * components (beyond the reference; INTEGRATION.md "Mesh simplification (beyond the reference)").  Definition:
  *

@@ -17,12 +17,13 @@ from typing import Optional
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 _REPO_DIR = os.path.dirname(_PKG_DIR)
 LIB_PATH = os.path.join(_PKG_DIR, "libpmb200.so")
-SOURCES = [os.path.join(_PKG_DIR, "csrc", f) for f in ("pm_kernels.cu", "pm_backward.cu", "pm_conv.cu", "pm_conv5.cu", "pm_stem.cu", "pm_refine.cu", "pm_geo.cu", "pm_cloud.cu", "pm_scan.cu", "pm_colmap.cu", "pm_undistort.cu", "pm_mesh.cu", "pm_simplify.cu", "pm_render.cu", "pm_texture.cu", "pm_train.cu", "pm_mapio.cpp")]
+SOURCES = [os.path.join(_PKG_DIR, "csrc", f) for f in ("pm_kernels.cu", "pm_backward.cu", "pm_conv.cu", "pm_conv5.cu", "pm_stem.cu", "pm_refine.cu", "pm_geo.cu", "pm_cloud.cu", "pm_scan.cu", "pm_colmap.cu", "pm_undistort.cu", "pm_mesh.cu", "pm_poisson.cu", "pm_simplify.cu", "pm_render.cu", "pm_texture.cu", "pm_train.cu", "pm_mapio.cpp")]
 HEADERS = [
     os.path.join(_PKG_DIR, "csrc", "pm_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_warpcorr4.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_geo_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_mesh_math.cuh"),
+    os.path.join(_PKG_DIR, "csrc", "pm_poisson_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_simplify_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_camera_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_raster.cuh"),
@@ -130,6 +131,23 @@ class TsdfView(ctypes.Structure):
                 ("height", c_int), ("width", c_int)]
 
 
+class PoissonGrid(ctypes.Structure):
+    """pmb200_poisson_grid (include/patchmatch_b200.h): the grid and counts pmb200_poisson_setup returns."""
+
+    _fields_ = [("depth", c_int), ("N", c_int), ("h", c_double), ("I0", c_int64 * 3), ("lo", c_double * 3), ("hi", c_double * 3),
+                ("n_points", c_int64), ("n_kept", c_int64), ("n_inside", c_int64), ("points_offset", c_int64), ("has_rgb", c_int),
+                ("reserved", c_int)]
+
+
+class PoissonResult(ctypes.Structure):
+    """pmb200_poisson_result (include/patchmatch_b200.h): cycles, convergence, final relative residual and iso-value."""
+
+    _fields_ = [("cycles", c_int), ("converged", c_int), ("residual", c_double), ("iso", c_double)]
+
+
+_PGRID = POINTER(PoissonGrid)
+
+
 class CameraStruct(ctypes.Structure):
     """pmb200_camera (include/patchmatch_b200.h): one COLMAP camera of the undistortion."""
 
@@ -169,6 +187,13 @@ _SIGNATURES = {
     "pmb200_tsdf_mesh_workspace_bytes": (c_int64, [c_int64]),
     "pmb200_tsdf_mesh_count": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
     "pmb200_tsdf_mesh_write": (c_int, [c_void_p, c_int64, c_double] + [c_void_p] * 3 + [c_int] + [c_void_p] * 3 + [c_int64, c_void_p]),
+    "pmb200_poisson_workspace_bytes": (c_int64, [c_int, c_int64]),
+    "pmb200_poisson_setup": (c_int, [c_void_p] * 3 + [c_int64, c_int, c_double, c_double, _PGRID, c_void_p, c_int64, c_void_p]),
+    "pmb200_poisson_density": (c_int, [_PGRID, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pmb200_poisson_rhs": (c_int, [_PGRID, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pmb200_poisson_solve": (c_int, [_PGRID, c_double, c_int, POINTER(PoissonResult), c_void_p, c_void_p, c_int64, c_void_p]),
+    "pmb200_poisson_band": (c_int, [_PGRID, c_double, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pmb200_poisson_colours": (c_int, [_PGRID, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
     "pmb200_simplify_mesh_workspace_bytes": (c_int64, [c_int64, c_int64]),
     "pmb200_simplify_mesh": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, POINTER(c_int64), c_void_p,
                                      c_int64, c_void_p]),

@@ -1198,6 +1198,174 @@ def tsdf_mesh(points: Tensor, depths: Sequence[Tensor], images: Sequence[Tensor]
     return tsdf_extract(keys, tsdf, weight, colour, voxel_size, min_weight)
 
 
+def _poisson_args(depth, scale, band, bbox_quantile, tol, max_cycles, what: str) -> None:
+    import math
+
+    def real(v):
+        return not isinstance(v, bool) and isinstance(v, (int, float)) and math.isfinite(v)
+
+    if isinstance(depth, bool) or not isinstance(depth, int) or not 5 <= depth <= 10:
+        raise ValueError(f"{what}: depth must be an int in 5..10, got {depth!r}")
+    if not real(scale) or scale < 1:
+        raise ValueError(f"{what}: scale must be a finite number >= 1, got {scale!r}")
+    if isinstance(band, bool) or not isinstance(band, int) or not 1 <= band <= 4:
+        raise ValueError(f"{what}: band must be an int in 1..4 (voxels), got {band!r}")
+    if not real(bbox_quantile) or not 0 <= bbox_quantile < 0.5:
+        raise ValueError(f"{what}: bbox_quantile must be in [0, 0.5), got {bbox_quantile!r}")
+    if not real(tol) or tol < 0:
+        raise ValueError(f"{what}: tol must be a finite number >= 0, got {tol!r}")
+    if isinstance(max_cycles, bool) or not isinstance(max_cycles, int) or max_cycles < 0:
+        raise ValueError(f"{what}: max_cycles must be an int >= 0, got {max_cycles!r}")
+
+
+def poisson_mesh_bytes(depth: int, n_points: int) -> int:
+    """Device memory ops.poisson_mesh needs besides its inputs and the band volume: the workspace of
+    pmb200_poisson_workspace_bytes, about 12 bytes per node of the (2^depth + 1)^3 grid (chi and the residual, which alias
+    the fixed-point sums of rho and b, and b) plus 12 / 7 for the coarser levels, and about 64 bytes per point.  ValueError
+    on bad arguments; needs a CUDA device (the size of the CUB passes' storage)."""
+    _poisson_args(depth, 1.1, 2, 0.0, 1e-5, 50, "poisson_mesh_bytes")
+    if isinstance(n_points, bool) or not isinstance(n_points, int) or not 0 <= n_points < 2 ** 28:
+        raise ValueError(f"poisson_mesh_bytes: n_points must be an int in 0..2^28-1, got {n_points!r}")
+    ws = _native.lib().pmb200_poisson_workspace_bytes(depth, n_points)
+    if ws < 0:
+        raise ValueError("poisson_mesh_bytes: " + _native.lib().pmb200_last_error().decode("utf-8", "replace"))
+    return int(ws)
+
+
+def _poisson_inputs(xyz: Tensor, normals: Tensor, rgb: Optional[Tensor], what: str):
+    for name, t, dt in (("xyz", xyz, torch.float32), ("normals", normals, torch.float32)):
+        if not isinstance(t, Tensor) or not _on_device(t) or t.dtype != dt or t.dim() != 2 or t.shape[1] != 3:
+            raise ValueError(f"{what}: {name} must be a CUDA float32 [n,3] tensor")
+    if normals.shape[0] != xyz.shape[0] or normals.device != xyz.device:
+        raise ValueError(f"{what}: normals must match xyz in length and device")
+    if rgb is not None:
+        if not isinstance(rgb, Tensor) or rgb.dtype != torch.uint8 or tuple(rgb.shape) != tuple(xyz.shape) or rgb.device != xyz.device:
+            raise ValueError(f"{what}: rgb must be a uint8 [n,3] tensor on the points' device, or None")
+        rgb = rgb.contiguous()
+    if xyz.shape[0] >= 2 ** 28:
+        raise ValueError(f"{what}: at most 2^28 - 1 points, got {xyz.shape[0]}")
+    return xyz.contiguous(), normals.contiguous(), rgb
+
+
+class _PoissonRun:
+    """One cloud's setup and solve: the grid, the workspace it lives in and, when asked, the intermediate fields."""
+
+    def __init__(self, xyz, normals, rgb, depth, scale, bbox_quantile, tol, max_cycles, fields: bool, what: str):
+        import ctypes
+
+        pts, nrm, col = _poisson_inputs(xyz, normals, rgb, what)
+        n = pts.shape[0]
+        N = 2 ** depth
+        need = poisson_mesh_bytes(depth, n)
+        free = _free_bytes(pts.device)
+        if need > free:
+            raise ValueError(f"{what}: depth {depth} has {(N + 1) ** 3} grid nodes and needs {need / 2 ** 30:.2f} GiB "
+                             f"({free / 2 ** 30:.2f} GiB free); use a smaller depth")
+        lib = _native.lib()
+        self.lib, self.device = lib, pts.device
+        self.ws = torch.empty(max(need, 1), dtype=torch.uint8, device=pts.device)
+        self.grid = _native.PoissonGrid()
+        st = _stream(pts)
+        with _device_guard(pts):
+            rc = lib.pmb200_poisson_setup(pts.data_ptr(), nrm.data_ptr(), None if col is None else col.data_ptr(), n, depth, float(scale),
+                                          float(bbox_quantile), ctypes.byref(self.grid), self.ws.data_ptr(), need, st)
+        _native.check(rc, "poisson_setup")
+        g = self.grid
+        if g.n_kept == 0:
+            raise ValueError(f"{what}: no point is kept (every xyz or normal is non-finite or the normal is zero)")
+        if g.h == 0:
+            raise ValueError(f"{what}: the box of the kept points has zero extent")
+        if g.n_inside == 0:
+            raise ValueError(f"{what}: no kept point lies inside the grid's node box")
+        self.fields = {}
+        M = (N + 1) ** 3
+        rho = torch.empty(M, dtype=torch.float64, device=pts.device) if fields else None
+        w = torch.empty(g.n_inside, dtype=torch.float64, device=pts.device) if fields else None
+        b = torch.empty(M, dtype=torch.float32, device=pts.device) if fields else None
+        chi = torch.empty(M, dtype=torch.float32, device=pts.device) if fields else None
+        ptr = lambda t: None if t is None else t.data_ptr()
+        self.result = _native.PoissonResult()
+        with _device_guard(pts):
+            _native.check(lib.pmb200_poisson_density(ctypes.byref(g), ptr(rho), ptr(w), self.ws.data_ptr(), need, st), "poisson_density")
+            _native.check(lib.pmb200_poisson_rhs(ctypes.byref(g), ptr(b), self.ws.data_ptr(), need, st), "poisson_rhs")
+            _native.check(lib.pmb200_poisson_solve(ctypes.byref(g), float(tol), max_cycles, ctypes.byref(self.result), ptr(chi),
+                                                   self.ws.data_ptr(), need, st), "poisson_solve")
+        if fields:
+            shape = (N + 1,) * 3  # [z, y, x]
+            self.fields = {"rho": rho.view(shape), "w": w, "b": b.view(shape), "chi": chi.view(shape)}
+        self.stats = {"points": n, "kept": int(g.n_inside), "dropped": n - int(g.n_inside), "N": N, "h": float(g.h),
+                      "I0": tuple(int(v) for v in g.I0), "iso": float(self.result.iso), "cycles": int(self.result.cycles),
+                      "residual": float(self.result.residual), "converged": bool(self.result.converged)}
+
+    def points(self) -> Tensor:
+        """The points that stay, float32 [n_inside,3], in input order (a view of the workspace)."""
+        off, m = int(self.grid.points_offset), int(self.grid.n_inside)
+        return self.ws[off : off + 12 * m].view(torch.float32).view(m, 3)
+
+    def band(self, keys: Tensor) -> Tuple[Tensor, Tensor]:
+        import ctypes
+
+        nb = keys.shape[0]
+        tsdf = torch.empty(nb * 512, dtype=torch.float32, device=self.device)
+        weight = torch.empty_like(tsdf)
+        with _device_guard(keys):
+            rc = self.lib.pmb200_poisson_band(ctypes.byref(self.grid), self.result.iso, keys.data_ptr(), nb, tsdf.data_ptr(),
+                                              weight.data_ptr(), self.ws.data_ptr(), self.ws.numel(), _stream(keys))
+        _native.check(rc, "poisson_band")
+        return tsdf, weight
+
+    def colours(self, verts: Tensor) -> None:
+        import ctypes
+
+        with _device_guard(verts):
+            rc = self.lib.pmb200_poisson_colours(ctypes.byref(self.grid), verts.data_ptr(), verts.shape[0], self.ws.data_ptr(),
+                                                 self.ws.numel(), _stream(verts))
+        _native.check(rc, "poisson_colours")
+
+
+def poisson_fields(xyz: Tensor, normals: Tensor, depth: int = 9, scale: float = 1.1, bbox_quantile: float = 0.0, tol: float = 1e-5,
+                   max_cycles: int = 50) -> Tuple[dict, dict]:
+    """The intermediate fields of ops.poisson_mesh, for inspection: ({"rho": float64, "b", "chi": float32, each [N+1]^3 as
+    [z, y, x], "w": float64 [kept]}, stats).  Arguments as poisson_mesh."""
+    _poisson_args(depth, scale, 2, bbox_quantile, tol, max_cycles, "poisson_fields")
+    run = _PoissonRun(xyz, normals, None, depth, scale, bbox_quantile, tol, max_cycles, True, "poisson_fields")
+    return run.fields, run.stats
+
+
+def poisson_mesh(xyz: Tensor, normals: Tensor, rgb: Optional[Tensor] = None, depth: int = 9, scale: float = 1.1, band: int = 2,
+                 bbox_quantile: float = 0.0, tol: float = 1e-5, max_cycles: int = 50) -> Tuple[Tensor, Tensor, dict]:
+    """A triangle mesh of oriented points by Poisson surface reconstruction on a (2^depth + 1)^3 grid, trimmed to a band of
+    `band` voxels around the points (this project's own definition, include/patchmatch_b200.h).  xyz, normals CUDA float32
+    [n,3] (normals pointing out of the surface, towards the cameras); rgb uint8 [n,3] or None.  -> (vertex records uint8
+    [nv,15] (x, y, z, red, green, blue: each vertex has the colour of the nearest kept point) or [nv,12] without rgb; faces
+    int32 [nf,3]; stats: points, kept, dropped, N, h, I0, iso, cycles, residual, converged) on the device.  When the
+    multigrid does not reach tol in max_cycles cycles the mesh is still extracted and one warning line is printed.
+
+    ValueError before any launch on bad arguments, when the grid would need more than the device's free memory (use a
+    smaller depth), and when no point is kept or the kept points' box has zero extent."""
+    what = "poisson_mesh"
+    _poisson_args(depth, scale, band, bbox_quantile, tol, max_cycles, what)
+    run = _PoissonRun(xyz, normals, rgb, depth, scale, bbox_quantile, tol, max_cycles, False, what)
+    st = run.stats
+    if not st["converged"]:
+        print(f"{what}: warning: the multigrid stopped at relative residual {st['residual']:.3g} after {st['cycles']} cycles "
+              f"(tol {tol:g})")
+    h = st["h"]
+    keys =tsdf_allocate(run.points(), h, band)
+    nb = keys.shape[0]
+    if nb >= 2 ** 22 or tsdf_mesh_bytes(nb) > _free_bytes(keys.device):
+        raise ValueError(f"{what}: the band has {nb} blocks of 8^3 voxels and needs {tsdf_mesh_bytes(nb) / 2 ** 30:.2f} GiB; use a "
+                         "smaller depth")
+    tsdf, weight = run.band(keys)
+    colour = torch.zeros((nb * 512, 4), dtype=torch.uint8, device=keys.device)
+    verts, faces = tsdf_extract(keys, tsdf, weight, colour, h, 1)
+    if rgb is not None:
+        run.colours(verts)
+    else:
+        verts = verts[:, :12].contiguous()
+    return verts, faces, st
+
+
 def simplify_mesh_bytes(n_vertices: int, n_faces: int) -> int:
     """Device memory ops.simplify_mesh needs beyond its inputs: the workspace (pmb200_simplify_mesh_workspace_bytes: about
     157 bytes per vertex for positions, quadrics, per-round vertex state and the selection, and 205 per face for two face

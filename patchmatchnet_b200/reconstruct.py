@@ -36,6 +36,7 @@ reconstruction takes as is.  For COLMAP's own fusion and meshers, export the res
 
     python -m patchmatchnet_b200.reconstruct --input-folder scene --output-folder outputs --checkpoint-path model.pt --normals
     PoissonRecon --in outputs/fused.ply --out mesh.ply            # or Open3D, or colmap poisson_mesher on this file
+    python -m patchmatchnet_b200.poisson --ply outputs/fused.ply --output mesh_poisson.ply   # or on the GPU, here
     python -m patchmatchnet_b200.colmap_output --input-folder scene --results-folder outputs --output-folder ws --normals
     colmap stereo_fusion --workspace_path ws --input_type geometric --output_path ws/fused.ply
     colmap poisson_mesher --input_path ws/fused.ply --output_path ws/meshed-poisson.ply
@@ -53,6 +54,10 @@ independent collapses) to at most N faces and written to <scan>/mesh_simplified.
 drops connected pieces of fewer than F faces.  mesh.ply is the same with or without these options.
 With --mesh-texture the simplified mesh (the mesh without --mesh-target-faces) is also textured from the scan's reference
 views (ops.texture_mesh) and written as <scan>/mesh_textured.obj, .mtl and mesh_textured_NN.png.
+With --poisson (needs --normals and the fusion stage; off by default, it changes no other output) the oriented fused
+points are also meshed on the GPU by Poisson surface reconstruction (ops.poisson_mesh: a multigrid solve on a
+(2^depth + 1)^3 grid, marching cubes trimmed to 2 voxels around the points) and written to <scan>/mesh_poisson.ply, the same
+bytes as python -m patchmatchnet_b200.poisson on that fused.ply; --poisson-depth (5..10, default 9) sets the grid.
 tnt_eval scores a Tanks and Temples training scene's fused.ply (or its mesh.ply) by precision, recall and F-score.
 
 Device memory held besides the engines, for a scan of n_img images of H x W and n_ref reference views:
@@ -133,7 +138,20 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--mesh-texture", action="store_true", default=argparse.SUPPRESS,
                     help="with --mesh, also write mesh_textured.obj (.mtl, _NN.png): the simplified mesh (or the mesh) textured "
                          "from the reference views, on the GPU")
+    ap.add_argument("--poisson", action="store_true", default=argparse.SUPPRESS,
+                    help="with --normals, also write mesh_poisson.ply: Poisson surface reconstruction of the oriented fused "
+                         "points, on the GPU")
+    ap.add_argument("--poisson-depth", type=int, default=argparse.SUPPRESS,
+                    help="with --poisson, a grid of 2^depth cells per axis, 5..10 (default 9)")
     return ap
+
+
+POISSON_DEFAULTS = {"poisson": False, "poisson_depth": 9}
+
+
+def poisson_options(args: argparse.Namespace) -> argparse.Namespace:
+    """--poisson and --poisson-depth of `args`, with their defaults where not given."""
+    return argparse.Namespace(**{k: getattr(args, k, v) for k, v in POISSON_DEFAULTS.items()})
 
 
 MESH_DEFAULTS = {"mesh": False, "mesh_voxel_size": None, "mesh_trunc": 3, "mesh_min_weight": 1, "mesh_target_faces": None,
@@ -182,6 +200,16 @@ def check_args(args: argparse.Namespace) -> List[str]:
             raise ValueError(f"--mesh-min-weight must be >= 1, got {m.mesh_min_weight}")
         if args.output_type == "depth":
             raise ValueError("--mesh needs the fusion stage (--output-type fusion or both)")
+    p = poisson_options(args)
+    if hasattr(args, "poisson_depth") and not p.poisson:
+        raise ValueError("--poisson-depth needs --poisson")
+    if p.poisson:
+        if not args.normals:
+            raise ValueError("--poisson needs --normals (an oriented fused.ply)")
+        if args.output_type == "depth":
+            raise ValueError("--poisson needs the fusion stage (--output-type fusion or both)")
+        if not 5 <= p.poisson_depth <= 10:
+            raise ValueError(f"--poisson-depth must be 5..10, got {p.poisson_depth}")
     scans = list_scans(args.scan_list)
     if not args.output_folder:
         args.output_folder = args.input_folder
@@ -468,9 +496,19 @@ def fuse_scan(args: argparse.Namespace, scan: str, bank: SceneBank, pairs: Seque
     data_io.save_ply(ply, bodies)
     log("saving the final model to", ply)
     mesh = {}
+    if poisson_options(args).poisson:
+        from .poisson import mesh_cloud
+
+        path = os.path.join(out_dir, "mesh_poisson.ply")
+        rec = torch.cat(bodies)
+        st = mesh_cloud(rec[:, :12].contiguous().view(torch.float32), rec[:, 12:24].contiguous().view(torch.float32),
+                        rec[:, 24:27].contiguous(), path, depth=poisson_options(args).poisson_depth)
+        mesh.update({"poisson_vertices": st["vertices"], "poisson_faces": st["faces"], "poisson_seconds": st["seconds"],
+                     "poisson_cycles": st["cycles"]})
+        log("saving the Poisson mesh to", path, "({} vertices, {} faces)".format(st["vertices"], st["faces"]))
     if mesh_options(args).mesh:
         path = os.path.join(out_dir, "mesh.ply")
-        mesh = mesh_scan(args, bank, [ref for ref, _ in pairs], mesh_depths, bodies, path)
+        mesh.update(mesh_scan(args, bank, [ref for ref, _ in pairs], mesh_depths, bodies, path))
         log("saving the mesh to", path, "({} vertices, {} faces)".format(mesh["mesh_vertices"], mesh["mesh_faces"]))
     return sum(int(b.shape[0]) for b in bodies), mesh
 
@@ -496,6 +534,8 @@ def reconstruct(args: argparse.Namespace, *, device: str = "cuda:0", n_slots: in
         stats.update({"simplified_vertices": 0, "simplified_faces": 0, "simplify_rounds": 0, "simplify_seconds": 0.0})
     if mesh_options(args).mesh_texture:
         stats.update(dict.fromkeys(TEXTURE_STATS, 0))
+    if poisson_options(args).poisson:
+        stats.update({"poisson_vertices": 0, "poisson_faces": 0, "poisson_seconds": 0.0, "poisson_cycles": 0})
     t_start = time.perf_counter()
     with precision(args.tf32), torch.cuda.device(dev), torch.no_grad():
         stage = DepthStage(load_network(args).to(dev), dev, n_slots=n_slots, seed=args.seed) if do_depth else None
