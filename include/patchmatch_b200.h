@@ -474,6 +474,48 @@ int pmb200_simplify_mesh_write(int64_t n_vertices, int64_t n_faces, int64_t n_fa
                                int *faces_out, void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------
+ * Surface sampling of triangle meshes: a regular barycentric lattice on every face, so that the point-cloud evaluations can
+ * score a mesh as a surface (beyond the reference; INTEGRATION.md "Surface sampling of meshes (beyond the reference)").
+ * Definition:
+ *
+ * Input.  xyz float32 [nv,3], rgb uint8 [nv,3] or NULL, faces int32 [nf,3], spacing s (float64, finite, > 0); nv, nf < 2^31 - 1.
+ * Arithmetic.  float64, every product, sum and quotient rounded on its own (no fused multiply-add), in the order
+ * csrc/pm_sample_math.cuh writes it; `/` and sqrt are IEEE.  No atomic touches a float: reruns give the same bits.
+ * Faces.  A face with an index outside 0..nv-1 emits nothing here (ops.sample_mesh rejects it with ValueError).  A face with
+ * a non-finite corner emits nothing.  A face with repeated indices is sampled like any other: it is a segment or a point.
+ * Lattice size.  A, B, C are the float32 corners widened; an edge length is sqrt((dx dx + dy dy) + dz dz), over B - A, C - B
+ * and A - C; L is the largest and n = max(1, ceil(L / s)).  A face with n >= 2^31 is reported (see the count call).
+ * Vertex samples.  Every finite vertex that at least one face references, in vertex-index order, with its coordinates (widened)
+ * and colour as they are.  They come first.
+ * Face samples.  Per face, in face order, the closed lattice without the three corners: i from 0 to n and, within each i, j
+ * from 0 to n - i, skipping (0,0), (n,0) and (0,n): (n+1)(n+2)/2 - 3 points, none for n = 1.  Weights a = (n-i-j)/n, b = i/n,
+ * c = j/n; P = (a A + b B) + c C per axis; colour = round-half-even((a rA + b rB) + c rC) clamped to 0..255 (0 without rgb).
+ * Guarantees.  Every point of every sampled face lies within s of some sample: the sub-triangles' edges are at most
+ * L / n <= s and their corners are all emitted.  A mesh whose longest edge is <= s samples to exactly its referenced finite
+ * vertices, in order.
+ * Duplicates.  Points on an edge shared by two faces with n >= 2 appear once per face; the two copies may differ in the last
+ * bit, because the two faces sum the corners in a different order.  They are not merged.
+ *
+ * Calls (device pointers unless marked HOST; the size query returns bytes or a negative PMB200_E*, and needs a CUDA device to
+ * size the CUB scans):
+ *   pmb200_mesh_sample_workspace_bytes(nv, nf): 8 bytes per face (the int64 counts, then offsets), 9 per vertex (the flags and
+ *       their int64 offsets) and the CUB scans' storage.
+ *   pmb200_mesh_sample_count: the count pass into the workspace; one host synchronisation.  counts_host (HOST, 4 int64):
+ *       [0] vertex samples, [1] face samples, [2] the lowest face index with n >= 2^31 or -1 (such faces count 0), [3] 1 when
+ *       the face samples may reach 2^62 (the counts are then not exact), else 0.
+ *   pmb200_mesh_sample: with the same inputs and workspace, after the count pass and with its counts [0] and [1]: xyz_out
+ *       float64 [n0 + n1, 3] and rgb_out uint8 [n0 + n1, 3] (may be NULL).  Enqueue only.  One thread per face sample; the
+ *       grid is capped and strides, so no launch exceeds the grid limits.
+ * PMB200_EINVAL, nothing launched, for a null pointer, sizes out of range, a spacing that is not finite and > 0, or a
+ * workspace smaller than the query. */
+int64_t pmb200_mesh_sample_workspace_bytes(int64_t n_vertices, int64_t n_faces);
+int pmb200_mesh_sample_count(const float *xyz, int64_t n_vertices, const int *faces, int64_t n_faces, double spacing,
+                             int64_t *counts_host, void *workspace, int64_t workspace_bytes, void *stream);
+int pmb200_mesh_sample(const float *xyz, const unsigned char *rgb, int64_t n_vertices, const int *faces, int64_t n_faces,
+                       int64_t n_vertex_samples, int64_t n_face_samples, double *xyz_out, unsigned char *rgb_out, void *workspace,
+                       int64_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------
  * Rendering of point clouds and triangle meshes (beyond the reference, whose only viewer is an Open3D window; INTEGRATION.md
  * "Rendering (beyond the reference)").  This project's own definition, float32 throughout, every product, sum and
  * difference rounded on its own (no fused multiply-add); `/` and sqrt are IEEE.  Reruns give the same bits.

@@ -17,7 +17,7 @@ from typing import Optional
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 _REPO_DIR = os.path.dirname(_PKG_DIR)
 LIB_PATH = os.path.join(_PKG_DIR, "libpmb200.so")
-SOURCES = [os.path.join(_PKG_DIR, "csrc", f) for f in ("pm_kernels.cu", "pm_backward.cu", "pm_conv.cu", "pm_conv5.cu", "pm_stem.cu", "pm_refine.cu", "pm_geo.cu", "pm_cloud.cu", "pm_scan.cu", "pm_colmap.cu", "pm_undistort.cu", "pm_mesh.cu", "pm_poisson.cu", "pm_simplify.cu", "pm_render.cu", "pm_texture.cu", "pm_train.cu", "pm_mapio.cpp")]
+SOURCES = [os.path.join(_PKG_DIR, "csrc", f) for f in ("pm_kernels.cu", "pm_backward.cu", "pm_conv.cu", "pm_conv5.cu", "pm_stem.cu", "pm_refine.cu", "pm_geo.cu", "pm_cloud.cu", "pm_scan.cu", "pm_colmap.cu", "pm_undistort.cu", "pm_mesh.cu", "pm_poisson.cu", "pm_simplify.cu", "pm_sample.cu", "pm_render.cu", "pm_texture.cu", "pm_train.cu", "pm_mapio.cpp")]
 HEADERS = [
     os.path.join(_PKG_DIR, "csrc", "pm_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_warpcorr4.cuh"),
@@ -25,6 +25,7 @@ HEADERS = [
     os.path.join(_PKG_DIR, "csrc", "pm_mesh_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_poisson_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_simplify_math.cuh"),
+    os.path.join(_PKG_DIR, "csrc", "pm_sample_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_camera_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_raster.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_texture_math.cuh"),
@@ -198,7 +199,11 @@ _SIGNATURES = {
     "pmb200_simplify_mesh": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, POINTER(c_int64), c_void_p,
                                      c_int64, c_void_p]),
     "pmb200_simplify_mesh_write": (c_int, [c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
-    "pmb200_render_points_workspace_bytes": (c_int64, [c_int, c_int]),
+    "pmb200_mesh_sample_workspace_bytes": (c_int64, [c_int64, c_int64]),
+    "pmb200_mesh_sample_count": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_double, POINTER(c_int64), c_void_p, c_int64, c_void_p]),
+    "pmb200_mesh_sample": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64,
+                                   c_void_p]),
+    "pmb200_render_points_workspace_bytes":(c_int64, [c_int, c_int]),
     "pmb200_render_points": (c_int, [c_void_p] * 3 + [c_int64, _PF, _PF, c_int, c_int, c_int, c_float, c_int, POINTER(ctypes.c_ubyte)]
                              + [c_void_p] * 3 + [c_int64, c_void_p]),
     "pmb200_render_mesh_workspace_bytes": (c_int64, [c_int, c_int, c_int64, c_int64]),

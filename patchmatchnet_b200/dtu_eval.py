@@ -15,6 +15,10 @@ Two documented differences from a MATLAB run (INTEGRATION.md, "DTU evaluation"):
 
 Command line:
     python -m patchmatchnet_b200.dtu_eval --data-path "SampleSet/MVS Data" --outputs outputs --json dtu.json
+
+With --surface the reconstruction is a triangle mesh scored as a surface: its samples (ops.sample_mesh, every point of the
+surface within --surface-spacing of one, default the thinning distance 0.2 mm) go through the unchanged thinning, instead of
+its vertices (INTEGRATION.md, "Surface sampling of meshes (beyond the reference)").
 """
 from __future__ import annotations
 
@@ -29,11 +33,12 @@ from typing import Dict, Sequence
 import numpy as np
 import torch
 
-from . import data_io, ops
+from . import data_io, ops, sample
 
 # BaseEvalMain_web.m:23
 DTU_EVAL_SCANS = (1, 4, 9, 10, 11, 12, 13, 15, 23, 24, 29, 32, 33, 34, 48, 49, 62, 75, 77, 110, 114, 118)
 MASK_MARGIN = 10  # PointCompareMain.m: ObsMask{scan}_10.mat
+THIN_DST = 0.2  # BaseEvalMain_web.m: dst, the thinning distance (mm); also the default --surface-spacing
 
 
 def visiting_order(n: int, seed: int) -> np.ndarray:
@@ -76,7 +81,7 @@ def side_stats(d: torch.Tensor) -> Dict[str, float]:
     return {"count": n, "mean": float(mean), "median": float(med), "var": float(var)}
 
 
-def evaluate_scan(data_points, stl_points, obs_mask, bb, res, plane, *, dst: float = 0.2, search_dist: float = 60.0,
+def evaluate_scan(data_points, stl_points, obs_mask, bb, res, plane, *, dst: float = THIN_DST, search_dist: float = 60.0,
                   outlier_dist: float = 20.0, seed: int = 0, device="cuda") -> Dict[str, float]:
     """One scan (PointCompareMain.m + the per-scan statistics of BaseEvalMain_web.m / ComputeStat_web.m).
 
@@ -142,17 +147,34 @@ def main(argv=None) -> int:
     ap.add_argument("--seed", type=int, default=0, help="seed of the thinning's visiting order")
     ap.add_argument("--json", default=None, help="write the per-scan and final results to this file")
     ap.add_argument("--device", default="cuda")
+    ap.add_argument("--surface", action="store_true",
+                    help="score the mesh at --ply-template as a surface: its samples instead of its vertices")
+    ap.add_argument("--surface-spacing", type=float, default=None,
+                    help=f"sample spacing of --surface in mm (default {THIN_DST:g}, the thinning distance)")
     args = ap.parse_args(argv)
+    if args.surface_spacing is not None and not args.surface:
+        raise ValueError("--surface-spacing needs --surface")
+    sample.check_spacing(args.surface_spacing, "--surface-spacing")
+    spacing = THIN_DST if args.surface_spacing is None else args.surface_spacing
 
     per_scan = []
     for scan in args.scans:
         t0 = time.perf_counter()
         truth = load_scan_truth(args.data_path, scan)
-        data = data_io.read_ply_points(args.ply_template.format(outputs=args.outputs, scan=scan))
+        path = args.ply_template.format(outputs=args.outputs, scan=scan)
+        surface = None
+        if args.surface:
+            pts, surface = sample.mesh_samples(path, spacing, args.device)
+            data = pts.cpu().numpy()
+            del pts
+        else:
+            data = data_io.read_ply_points(path)
         r = evaluate_scan(data, truth["stl_points"], truth["obs_mask"], truth["bb"], truth["res"], truth["plane"],
                           seed=args.seed, device=args.device)
         r["scan"] = scan
         r["seconds"] = time.perf_counter() - t0
+        if surface is not None:
+            r["surface"] = surface
         per_scan.append(r)
         print(f"scan{scan}: acc. mean/median {r['acc_mean']:.6f}/{r['acc_median']:.6f}  comp. mean/median "
               f"{r['comp_mean']:.6f}/{r['comp_median']:.6f}  ({r['n_data']} -> {r['n_thinned']} points, {r['seconds']:.1f} s)",

@@ -20,6 +20,10 @@ the scene frame.
 
 Command line:
     python -m patchmatchnet_b200.eth3d_eval --gt-path eth3d_gt --outputs outputs --scenes courtyard pipes --json eth3d.json
+
+With --surface the reconstruction is a triangle mesh scored as a surface: its samples (ops.sample_mesh, every point of the
+surface within --surface-spacing of one, default half the smallest tolerance) instead of its vertices; the memory check
+counts the samples.
 """
 from __future__ import annotations
 
@@ -35,7 +39,7 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 import torch
 
-from . import _native, data_io, ops
+from . import _native, data_io, ops, sample
 
 MLP = os.path.join("dslr_scan_eval", "scan_alignment.mlp")
 TOLERANCES = (0.01, 0.02, 0.05, 0.1, 0.2, 0.5)
@@ -237,6 +241,10 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--cloud-tolerance", type=float, default=CLOUD_TOLERANCE)
     ap.add_argument("--json", default=None, help="write the results to this file")
     ap.add_argument("--device", default="cuda")
+    ap.add_argument("--surface", action="store_true",
+                    help="score the mesh at --ply-template as a surface: its samples instead of its vertices")
+    ap.add_argument("--surface-spacing", type=float, default=None,
+                    help="sample spacing of --surface in metres (default half the smallest tolerance)")
     return ap
 
 
@@ -250,6 +258,9 @@ def check_args(args: argparse.Namespace) -> List[str]:
         raise ValueError(f"--beam-divergence-halfangle-deg must be in [0, 90), got {args.beam_divergence_halfangle_deg}")
     if not (args.cloud_tolerance > 0 and math.isfinite(args.cloud_tolerance)):
         raise ValueError(f"--cloud-tolerance must be positive and finite, got {args.cloud_tolerance}")
+    if args.surface_spacing is not None and not args.surface:
+        raise ValueError("--surface-spacing needs --surface")
+    sample.check_spacing(args.surface_spacing, "--surface-spacing")
     scenes = args.scenes if args.scenes else find_scenes(args.gt_path)
     if not scenes:
         raise ValueError(f"no scene under {args.gt_path!r} has {MLP}")
@@ -269,7 +280,15 @@ def main(argv=None) -> int:
     for scene in scenes:
         t0 = time.perf_counter()
         truth = load_scene_truth(args.gt_path, scene)
-        rec = data_io.read_ply_points(args.ply_template.format(outputs=args.outputs, scene=scene))
+        path = args.ply_template.format(outputs=args.outputs, scene=scene)
+        surface = None
+        if args.surface:
+            spacing = min(args.tolerances) / 2 if args.surface_spacing is None else args.surface_spacing
+            pts, surface = sample.mesh_samples(path, spacing, args.device)
+            rec = pts.cpu().numpy()
+            del pts
+        else:
+            rec = data_io.read_ply_points(path)
         r, state = _evaluate(rec, truth["scans"], args.tolerances, args.beam_start_radius, args.beam_divergence_halfangle_deg,
                              args.device, args.cloud_tolerance if clouds else None)
         if clouds:
@@ -283,6 +302,8 @@ def main(argv=None) -> int:
         del state
         r["scene"] = scene
         r["seconds"] = time.perf_counter() - t0
+        if surface is not None:
+            r["surface"] = surface
         results.append(r)
     mean = [{"tolerance": tau, **{k: float(np.mean([r["tolerances"][i][k] for r in results]))
                                   for k in ("accuracy", "completeness", "f1")}}

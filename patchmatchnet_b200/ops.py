@@ -1439,6 +1439,98 @@ def simplify_mesh(xyz: Tensor, rgb: Optional[Tensor], faces: Tensor, target_face
     return torch.cat(parts, 1), out_faces, rounds
 
 
+def sample_mesh_bytes(n_vertices: int, n_faces: int, n_samples: int, rgb: bool = True) -> int:
+    """Device memory ops.sample_mesh needs beyond its inputs: the workspace (pmb200_mesh_sample_workspace_bytes: 8 bytes per
+    face, 9 per vertex and the CUB scans' storage) plus 24 bytes per sample of float64 xyz and 3 more with colours.  Needs a
+    CUDA device (the size of the CUB scans' storage)."""
+    ws = _native.lib().pmb200_mesh_sample_workspace_bytes(n_vertices, n_faces)
+    if ws < 0:
+        _native.check(int(ws), "mesh_sample_workspace_bytes")
+    return int(ws) + (27 if rgb else 24) * int(n_samples)
+
+
+class _SampleCount:
+    """The count pass of ops.sample_mesh: checked inputs, the workspace it filled and the two totals."""
+
+    def __init__(self, xyz, faces, spacing, what):
+        import ctypes
+        import math
+
+        self.xyz = _render_xyz(xyz, what)
+        nv = self.xyz.shape[0]
+        if not isinstance(faces, Tensor) or not _on_device(faces) or faces.dtype != torch.int32 or faces.dim() != 2 or faces.shape[1] != 3:
+            raise ValueError(f"{what}: faces must be a CUDA int32 [nf,3] tensor")
+        if faces.device != self.xyz.device:
+            raise ValueError(f"{what}: faces must be on the vertices' device")
+        if isinstance(spacing, bool) or not isinstance(spacing, (int, float)) or not math.isfinite(spacing) or spacing <= 0:
+            raise ValueError(f"{what}: spacing must be a finite number > 0, got {spacing!r}")
+        self.faces = faces.contiguous()
+        nf = self.faces.shape[0]
+        if nv >= 2 ** 31 - 1 or nf >= 2 ** 31 - 1:
+            raise ValueError(f"{what}: at most 2^31 - 2 vertices and faces, got {nv} and {nf}")
+        if nf:
+            lo, hi = (int(v) for v in torch.aminmax(self.faces))
+            if lo < 0 or hi >= nv:
+                raise ValueError(f"{what}: a face refers to a vertex outside 0..{nv - 1}")
+        self.nv, self.nf, self.spacing = nv, nf, float(spacing)
+        lib = _native.lib()
+        self.ws_bytes = int(lib.pmb200_mesh_sample_workspace_bytes(nv, nf))
+        if self.ws_bytes > _free_bytes(self.xyz.device):
+            raise ValueError(f"{what}: {nv} vertices and {nf} faces need a workspace of {self.ws_bytes / 2 ** 30:.2f} GiB, more than "
+                             "the device has free")
+        self.ws = _workspace(self.ws_bytes, "mesh_sample_workspace_bytes", self.xyz.device)
+        counts = (ctypes.c_int64 * 4)()
+        with _device_guard(self.xyz):
+            rc = lib.pmb200_mesh_sample_count(self.xyz.data_ptr(), nv, self.faces.data_ptr(), nf, self.spacing, counts,
+                                              self.ws.data_ptr(), self.ws_bytes, _stream(self.xyz))
+        _native.check(rc, what)
+        if counts[2] >= 0:
+            raise ValueError(f"{what}: face {counts[2]} needs a lattice of 2^31 or more points per edge at spacing {spacing:g}; use a "
+                             "larger spacing")
+        if counts[3]:
+            raise ValueError(f"{what}: the faces would give 2^62 or more samples at spacing {spacing:g}; use a larger spacing")
+        self.n_vertex, self.n_face = int(counts[0]), int(counts[1])
+        self.total = self.n_vertex + self.n_face
+
+
+def sample_mesh_count(xyz: Tensor, faces: Tensor, spacing: float) -> int:
+    """The exact number of samples ops.sample_mesh(xyz, faces, spacing) returns: the count pass alone, with no emit and no
+    output allocation.  Same arguments and ValueErrors as ops.sample_mesh, except the memory check of the output."""
+    return _SampleCount(xyz, faces, spacing, "sample_mesh_count").total
+
+
+def sample_mesh(xyz: Tensor, faces: Tensor, spacing: float, rgb: Optional[Tensor] = None) -> Tuple[Tensor, Optional[Tensor]]:
+    """Samples of a triangle mesh's surface on a regular barycentric lattice per face, at most `spacing` apart along every
+    lattice edge: the referenced finite vertices first, in index order, then each face's lattice points without its corners,
+    in face order.  Every point of the surface lies within `spacing` of a sample.  Definition in include/patchmatch_b200.h.
+    xyz CUDA float32 [nv,3]; faces int32 [nf,3]; spacing a finite float > 0; rgb uint8 [nv,3] or None.  -> (float64 [n,3],
+    uint8 [n,3] or None) on the device.  Reruns give the same bits.
+
+    ValueError before any launch on bad arguments (a face index outside 0..nv-1 included), when a face would need a lattice
+    of 2^31 or more points per edge, and, before the output is allocated, when sample_mesh_bytes exceeds the device's free
+    memory: each names the sample count and suggests a larger spacing.  One host read (the count)."""
+    what = "sample_mesh"
+    run = _SampleCount(xyz, faces, spacing, what)
+    col = _render_attr(rgb, run.nv, torch.uint8, run.xyz.device, "rgb", what)
+    col = None if col is None else col.contiguous()
+    dev, n = run.xyz.device, run.total
+    need = (27 if col is not None else 24) * n
+    free = _free_bytes(dev)
+    if need > free:
+        raise ValueError(f"{what}: {n} samples at spacing {spacing:g} need {need / 2 ** 30:.2f} GiB of output ({free / 2 ** 30:.2f} GiB "
+                         "free); use a larger spacing")
+    out = torch.empty((n, 3), dtype=torch.float64, device=dev)
+    out_rgb = None if col is None else torch.empty((n, 3), dtype=torch.uint8, device=dev)
+    if n:
+        with _device_guard(run.xyz):
+            rc = _native.lib().pmb200_mesh_sample(run.xyz.data_ptr(), None if col is None else col.data_ptr(), run.nv,
+                                                  run.faces.data_ptr(), run.nf, run.n_vertex, run.n_face, out.data_ptr(),
+                                                  None if out_rgb is None else out_rgb.data_ptr(), run.ws.data_ptr(), run.ws_bytes,
+                                                  _stream(run.xyz))
+        _native.check(rc, what)
+    return out, out_rgb
+
+
 def render_camera_arrays(P):
     """A 3 x 4 float64 camera K [R | t] -> (P rounded to float32, row-major [12]; camera centre -M^-1 p4 computed in float64
     and rounded to float32 [3]), the HOST values pmb200_render_points / _mesh take.  ValueError for a camera that is not

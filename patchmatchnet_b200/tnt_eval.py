@@ -19,6 +19,10 @@ RANSAC over the few hundred camera centres and the 3 x 3 SVD of each ICP update.
 
 Command line:
     python -m patchmatchnet_b200.tnt_eval --gt-path TrainingSet --outputs outputs --scenes Ignatius Barn --json tnt.json
+
+With --surface the reconstruction is a triangle mesh scored as a surface: its samples (ops.sample_mesh) instead of its
+vertices, taken in the reconstruction's frame before the alignment at spacing (tau / 4) / c, c the scale of the initial
+similarity (surface_spacing), so that every point of the surface lies within half the tau / 2 scoring voxel of a sample.
 """
 from __future__ import annotations
 
@@ -35,7 +39,7 @@ from typing import Dict, Optional
 import numpy as np
 import torch
 
-from . import data_io, ops
+from . import data_io, ops, sample
 
 # distance threshold tau of each training scene (T&T toolbox, run.py / setup)
 SCENE_TAU = {"Barn": 0.01, "Caterpillar": 0.005, "Church": 0.025, "Courthouse": 0.025, "Ignatius": 0.003,
@@ -266,6 +270,15 @@ def evaluate_scene(rec_points, gt_points, crop_volume, init_transform, tau: floa
     return out
 
 
+def surface_spacing(tau: float, init: np.ndarray) -> float:
+    """The default --surface spacing in the reconstruction's frame: (tau / 4) / c, c = cbrt(det) of the initial similarity's
+    3 x 3 part (its scale).  ICP's later change of scale is not included; it is small once the initial alignment holds."""
+    det = float(np.linalg.det(np.asarray(init, np.float64)[:3, :3]))
+    if not (det > 0 and math.isfinite(det)):
+        raise ValueError(f"--surface: the initial alignment's 3 x 3 part has determinant {det}; it is not a similarity")
+    return (tau / 4) / (det ** (1.0 / 3.0))
+
+
 def main(argv=None) -> int:
     ap = argparse.ArgumentParser(prog="python -m patchmatchnet_b200.tnt_eval", description=__doc__.split("\n\n")[0])
     ap.add_argument("--gt-path", required=True, help="T&T ground-truth folder holding <Scene>/<Scene>.ply, .json, _trans.txt, .log")
@@ -279,7 +292,14 @@ def main(argv=None) -> int:
     ap.add_argument("--seed", type=int, default=0, help="seed of the trajectory alignment's RANSAC")
     ap.add_argument("--json", default=None, help="write the per-scene results to this file")
     ap.add_argument("--device", default="cuda")
+    ap.add_argument("--surface", action="store_true",
+                    help="score the mesh at --ply-template as a surface: its samples instead of its vertices")
+    ap.add_argument("--surface-spacing", type=float, default=None,
+                    help="sample spacing of --surface in the reconstruction's frame (default (tau / 4) / the initial scale)")
     args = ap.parse_args(argv)
+    if args.surface_spacing is not None and not args.surface:
+        raise ValueError("--surface-spacing needs --surface")
+    sample.check_spacing(args.surface_spacing, "--surface-spacing")
     if not torch.cuda.is_available() or torch.device(args.device).type != "cuda":
         raise RuntimeError("tnt_eval needs a CUDA device; there is no CPU path")
     for scene in args.scenes:
@@ -299,13 +319,23 @@ def main(argv=None) -> int:
             init = align["transformation"]
         else:
             init = truth["trans"]
-        rec = data_io.read_ply_points(args.ply_template.format(outputs=args.outputs, scene=scene))
+        path = args.ply_template.format(outputs=args.outputs, scene=scene)
+        surface = None
+        if args.surface:
+            spacing = surface_spacing(tau, init) if args.surface_spacing is None else args.surface_spacing
+            pts, surface = sample.mesh_samples(path, spacing, args.device)
+            rec = pts.cpu().numpy()
+            del pts
+        else:
+            rec = data_io.read_ply_points(path)
         r = evaluate_scene(rec, truth["points"], truth["crop"], init, tau, device=args.device)
         r["scene"] = scene
         r["init"] = args.init
         if align is not None:
             r["alignment"] = {"inliers": align["inliers"], "rmse": align["rmse"], "best_sample": align["best_sample"]}
         r["seconds"] = time.perf_counter() - t0
+        if surface is not None:
+            r["surface"] = surface
         results.append(r)
         print(f"{scene}: precision {r['precision']:.4f}  recall {r['recall']:.4f}  f-score {r['fscore']:.4f}  tau {tau:g}  "
               f"fitness {r['fitness']:.4f}  ({r['seconds']:.1f} s)", flush=True)
