@@ -656,17 +656,24 @@ int pmb200_texture_write(int view, const float *image, int width, int height, co
  *                  keep_out is 0 and the result must not be used)
  * pmb200_nearest_distance (MaxDistCP.m): for each "from" point, min(exact distance to the nearest "to" point, max_dist) if it
  * lies in one of MaxDistCP's blocks of the box bb_host (BB_lo + k * max_dist <= x < BB_lo + k * max_dist + max_dist,
- * k = 0 .. floor((BB_hi - BB_lo) / max_dist) per axis), else max_dist.
+ * k = 0 .. floor((BB_hi - BB_lo) / max_dist) per axis, each product and sum rounded on its own: no fused multiply-add),
+ * else max_dist.
  *   to_points [n_to,3], from_points [n_from,3], dist_out [n_from]: float64 device;  bb_host: HOST, 6 doubles (lo xyz, hi xyz)
  *   cell: edge of the fine search cells, max_dist / 256 <= cell (speed only: the result does not depend on it); the search
  *         visits at most 5^3 fine cells, then rings of 16^3-cell coarse cells out to max_dist (at most 35^3 coarse cells)
- * Sort + table launches, then the search; no host synchronisation.  Point and output pointers may be NULL for empty clouds. */
+ * Sort + table launches, then the search; no host synchronisation.  Point and output pointers may be NULL for empty clouds.
+ * pmb200_nearest_distance_capped: the same search without blocks, for every "from" point min(exact distance to the nearest
+ *   "to" point, max_dist) (max_dist when n_to = 0), with the workspace of pmb200_nearest_distance_workspace_bytes(n_to).
+ *   The Tanks and Temples scoring uses it: MaxDistCP's adjacent blocks can leave a gap of one rounding step
+ *   (Low_k + max_dist < Low_{k+1}), and a point exactly in such a gap would get max_dist whatever its nearest distance. */
 int64_t pmb200_thin_points_workspace_bytes(int64_t n);
 int pmb200_thin_points(const double *points, const int *rank, int64_t n, double dst, unsigned char *keep_out, int *undecided_out,
                        void *workspace, int64_t workspace_bytes, void *stream);
 int64_t pmb200_nearest_distance_workspace_bytes(int64_t n_to);
 int pmb200_nearest_distance(const double *to_points, int64_t n_to, const double *from_points, int64_t n_from, const double *bb_host,
                             double max_dist, double cell, double *dist_out, void *workspace, int64_t workspace_bytes, void *stream);
+int pmb200_nearest_distance_capped(const double *to_points, int64_t n_to, const double *from_points, int64_t n_from, double max_dist,
+                                   double cell, double *dist_out, void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------
  * Tanks and Temples evaluation (beyond the reference; INTEGRATION.md "Tanks and Temples evaluation"), float64 throughout,

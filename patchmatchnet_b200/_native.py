@@ -222,6 +222,7 @@ _SIGNATURES = {
     "pmb200_thin_points": (c_int, [c_void_p, c_void_p, c_int64, c_double, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
     "pmb200_nearest_distance_workspace_bytes": (c_int64, [c_int64]),
     "pmb200_nearest_distance": (c_int, [c_void_p, c_int64, c_void_p, c_int64, POINTER(c_double), c_double, c_double, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pmb200_nearest_distance_capped": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_double, c_double, c_void_p, c_void_p, c_int64, c_void_p]),
     "pmb200_crop_polygon": (c_int, [c_void_p, c_int64, POINTER(c_double), c_int, c_double, c_double, POINTER(c_double), c_int,
                                     c_void_p, c_void_p, c_void_p]),
     "pmb200_voxel_downsample_workspace_bytes": (c_int64, [c_int64]),

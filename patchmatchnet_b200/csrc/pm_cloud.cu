@@ -262,7 +262,7 @@ __global__ void __launch_bounds__(kBlock) thin_scatter_kernel(const unsigned cha
     }
 }
 
-// ---- nearest distance, capped, with the block membership of MaxDistCP ---------------------------------------------------
+// ---- nearest distance, capped, with or without the block membership of MaxDistCP--------------------------------------------
 
 struct NearestParams {
     const double *from;
@@ -271,6 +271,7 @@ struct NearestParams {
     const double *pts;        // "to" cloud, sorted
     double inv_cell, cell, max_dist;
     double bb_lo[3], range[3];  // range: MaxDistCP's last block index per axis
+    bool blocks;                // false: every query is searched (no block membership)
     double *out;
 };
 
@@ -283,7 +284,7 @@ __device__ inline bool in_some_block(double q, double lo, double range, double m
     if (!(k0 >= -1.0 && k0 <= range + 1.0)) return false;  // far outside (or not finite): also keeps k0 +- 1 exact
     for (double k = k0 - 1.0; k <= k0 + 1.0; k += 1.0) {
         if (k < 0.0 || k > range) continue;
-        const double low = lo + k * m, high = low + m;
+        const double low = __dadd_rn(lo, __dmul_rn(k, m)), high = __dadd_rn(low, m);  // no fused multiply-add
         if (q >= low && q < high) return true;
     }
     return false;
@@ -302,8 +303,8 @@ __global__ void __launch_bounds__(kBlock) nearest_kernel(const NearestParams p) 
     for (int i = blockIdx.x * kBlock + threadIdx.x; i < p.n_from; i += gridDim.x * kBlock) {
         const double x = p.from[3 * (size_t)i], y = p.from[3 * (size_t)i + 1], z = p.from[3 * (size_t)i + 2];
         const double m = p.max_dist, inv_m = 1.0 / p.max_dist;
-        if (!(in_some_block(x, p.bb_lo[0], p.range[0], m, inv_m) && in_some_block(y, p.bb_lo[1], p.range[1], m, inv_m) &&
-              in_some_block(z, p.bb_lo[2], p.range[2], m, inv_m))) {
+        if (p.blocks && !(in_some_block(x, p.bb_lo[0], p.range[0], m, inv_m) && in_some_block(y, p.bb_lo[1], p.range[1], m, inv_m) &&
+                          in_some_block(z, p.bb_lo[2], p.range[2], m, inv_m))) {
             p.out[i] = p.max_dist;
             continue;
         }
@@ -702,10 +703,12 @@ extern "C" int64_t pmb200_nearest_distance_workspace_bytes(int64_t n_to) {
     return b < 0 ? pmb200_internal_fail(PMB200_EINVAL, "nearest_distance_workspace_bytes: no CUDA device to size the CUB sort for") : b;
 }
 
-extern "C" int pmb200_nearest_distance(const double *to_points, int64_t n_to, const double *from_points, int64_t n_from,
-                                       const double *bb_host, double max_dist, double cell, double *dist_out, void *workspace,
-                                       int64_t workspace_bytes, void *stream) {
-    if ((!to_points && n_to > 0) || ((!from_points || !dist_out) && n_from > 0) || !bb_host || !workspace)
+namespace {
+
+// pmb200_nearest_distance (bb_host: MaxDistCP's blocks) and pmb200_nearest_distance_capped (bb_host NULL: no blocks)
+int nearest_distance_call(const double *to_points, int64_t n_to, const double *from_points, int64_t n_from, const double *bb_host,
+                          double max_dist, double cell, double *dist_out, void *workspace, int64_t workspace_bytes, void *stream) {
+    if ((!to_points && n_to > 0) || ((!from_points || !dist_out) && n_from > 0) || !workspace)
         return pmb200_internal_fail(PMB200_EINVAL, "nearest_distance: null pointer");
     if (n_to < 0 || n_to >= (1ll << 31) || n_from < 0 || n_from >= (1ll << 31))
         return pmb200_internal_fail(PMB200_EINVAL, "nearest_distance: 0 <= n_to, n_from < 2^31");
@@ -728,10 +731,29 @@ extern "C" int pmb200_nearest_distance(const double *to_points, int64_t n_to, co
     NearestParams p;
     p.from = from_points; p.n_from = (int)n_from; p.fine = g.fine; p.coarse = g.coarse; p.pts = g.pts;
     p.inv_cell = 1.0 / cell; p.cell = cell; p.max_dist = max_dist;
-    for (int a = 0; a < 3; ++a) { p.bb_lo[a] = bb_host[a]; p.range[a] = floor((bb_host[3 + a] - bb_host[a]) / max_dist); }
+    p.blocks = bb_host != nullptr;
+    for (int a = 0; a < 3; ++a) {
+        p.bb_lo[a] = p.blocks ? bb_host[a] : 0.0;
+        p.range[a] = p.blocks ? floor((bb_host[3 + a] - bb_host[a]) / max_dist) : 0.0;
+    }
     p.out = dist_out;
     nearest_kernel<<<blocks, kBlock, 0, st>>>(p);
     return pmb200_internal_launch_status("nearest_distance");
+}
+
+}  // namespace
+
+extern "C" int pmb200_nearest_distance(const double *to_points, int64_t n_to, const double *from_points, int64_t n_from,
+                                       const double *bb_host, double max_dist, double cell, double *dist_out, void *workspace,
+                                       int64_t workspace_bytes, void *stream) {
+    if (!bb_host) return pmb200_internal_fail(PMB200_EINVAL, "nearest_distance: null pointer");
+    return nearest_distance_call(to_points, n_to, from_points, n_from, bb_host, max_dist, cell, dist_out, workspace, workspace_bytes, stream);
+}
+
+extern "C" int pmb200_nearest_distance_capped(const double *to_points, int64_t n_to, const double *from_points, int64_t n_from,
+                                              double max_dist, double cell, double *dist_out, void *workspace, int64_t workspace_bytes,
+                                              void *stream) {
+    return nearest_distance_call(to_points, n_to, from_points, n_from, nullptr, max_dist, cell, dist_out, workspace, workspace_bytes, stream);
 }
 
 extern "C" int pmb200_crop_polygon(const double *points, int64_t n, const double *transform_host, int orthogonal_axis, double axis_min,

@@ -1694,10 +1694,13 @@ def default_search_cell(n_to: int, bb, max_dist: float) -> float:
     return min(max(cell, max_dist / 256.0), max_dist / 8.0)  # the library requires cell >= max_dist / 256
 
 
-def nearest_distance(to_points: Tensor, from_points: Tensor, bb, max_dist: float = 60.0, cell: Optional[float] = None) -> Tensor:
+def nearest_distance(to_points: Tensor, from_points: Tensor, bb, max_dist: float = 60.0, cell: Optional[float] = None,
+                     blocks: bool = True) -> Tensor:
     """Distance from every `from` point to the nearest `to` point, capped at max_dist, with the block membership of the
     reference's evaluations/dtu/MaxDistCP.m: a point outside its max_dist blocks over the box `bb` ([[x,y,z] lo, [x,y,z] hi])
-    gets max_dist.  Exact float64 distances.  to_points [m,3], from_points [n,3] float64 CUDA -> float64 [n]."""
+    gets max_dist.  blocks=False drops the block membership (pmb200_nearest_distance_capped): every point gets
+    min(nearest distance, max_dist), and `bb` only sizes the default search cell.  Exact float64 distances.
+    to_points [m,3], from_points [n,3] float64 CUDA -> float64 [n]."""
     import ctypes
 
     to = _points_arg(to_points, "nearest_distance (to)")
@@ -1717,8 +1720,12 @@ def nearest_distance(to_points: Tensor, from_points: Tensor, bb, max_dist: float
     ws = torch.empty(max(int(ws_bytes), 1), dtype=torch.uint8, device=frm.device)
     bb_host = (ctypes.c_double * 6)(*box)
     with _device_guard(frm):
-        rc = lib.pmb200_nearest_distance(to.data_ptr(), to.shape[0], frm.data_ptr(), frm.shape[0], bb_host, float(max_dist), float(cell),
-                                         out.data_ptr(), ws.data_ptr(), int(ws_bytes), _stream(frm))
+        if blocks:
+            rc = lib.pmb200_nearest_distance(to.data_ptr(), to.shape[0], frm.data_ptr(), frm.shape[0], bb_host, float(max_dist),
+                                             float(cell), out.data_ptr(), ws.data_ptr(), int(ws_bytes), _stream(frm))
+        else:
+            rc = lib.pmb200_nearest_distance_capped(to.data_ptr(), to.shape[0], frm.data_ptr(), frm.shape[0], float(max_dist),
+                                                    float(cell), out.data_ptr(), ws.data_ptr(), int(ws_bytes), _stream(frm))
     _native.check(rc, "nearest_distance")
     return out
 

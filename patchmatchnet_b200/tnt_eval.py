@@ -11,7 +11,7 @@ Inputs of one scene, ground-truth folder <gt>/<Scene>/: <Scene>.ply (GT points),
     2. refinement          three ICP rounds (point to point, with scaling), each on the cropped and down-sampled clouds:
                            voxel tau / 80 tau, voxel tau/2 / 20 tau, uniform / 2 tau (down-sampling / max distance)
     3. scoring             crop, voxel down-sample at tau/2, nearest distances both ways (ops.nearest_distance capped at
-                           5 tau), precision = mean(d1 < tau), recall = mean(d2 < tau), F = 2PR / (P + R), and the
+                           5 tau, without MaxDistCP's blocks), precision = mean(d1 < tau), recall = mean(d2 < tau), F = 2PR / (P + R), and the
                            cumulative histograms over np.arange(0, 5 tau, tau / 100)
 
 Kernels: ops.crop_points, ops.voxel_downsample, ops.icp and ops.nearest_distance (csrc/pm_cloud.cu).  The host runs the
@@ -239,8 +239,9 @@ def score(rec: torch.Tensor, gt: torch.Tensor, crop_volume, transform: np.ndarra
         box = [(allp.min(0).values - cap).cpu().tolist(), (allp.max(0).values + cap).cpu().tolist()]
     else:
         box = [[0.0] * 3, [1.0] * 3]
-    d1 = ops.nearest_distance(g, s, box, cap)  # reconstruction -> GT
-    d2 = ops.nearest_distance(s, g, box, cap)  # GT -> reconstruction
+    # plain capped distances (compute_point_cloud_distance has no blocks); the box only sizes the search cell
+    d1 = ops.nearest_distance(g, s, box, cap, blocks=False)  # reconstruction -> GT
+    d2 = ops.nearest_distance(s, g, box, cap, blocks=False)  # GT -> reconstruction
     n1, n2 = int(d1.numel()), int(d2.numel())
     c1, c2 = int((d1 < tau).sum()) if n1 else 0, int((d2 < tau).sum()) if n2 else 0
     precision = c1 / n1 if n1 else 0.0
