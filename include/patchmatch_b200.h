@@ -643,6 +643,79 @@ int pmb200_texture_write(int view, const float *image, int width, int height, co
                          void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------
+ * Mesh refinement: vertices moved by multi-view photo-consistency, after Vu et al. (PAMI 2012) and OpenMVS RefineMesh,
+ * without remeshing (beyond the reference; INTEGRATION.md "Mesh refinement (beyond the reference)").  Definition,
+ * reproduced bit for bit by oracle/refine_oracle.py; float64 arithmetic (pm_refine_mesh_math.cuh) with each operation
+ * rounded on its own (no fused multiply-add), no floating-point atomics, reruns give the same bits.  Constants:
+ * kRadius = 2, kMinCount = 13, kMinVariance = 1e-4, kDepthTolerance = 0.01, kMinCosine = 0.3, kGradUnit = 2^20,
+ * kWeightUnit = 2^32, kEnergyUnit = 2^24.
+ *
+ * Views and levels.  Per view K, E = [R | t] (float64), an image float32 [3,H,W] in [0,1]; views may differ in size.  Grey
+ * G = ((0.299 r + 0.587 g) + 0.114 b) in float32.  Level l + 1 has floor(H/2) x floor(W/2) pixels, each ((a + b) + (c + d))
+ * * 0.25 (float32) of its 2 x 2 block, and fx/2, fy/2, skew/2, cx' = (cx + 0.5)/2 - 0.5, cy' likewise.  P = K [R | t]
+ * (float64), C = -R^T t (C_c = -((R0c t0 + R1c t1) + R2c t2)), near_z = 1e-3 |C' - box centre| as the texturer's
+ * (C' its solve of P, the box the 1st-99th percentile box of the input vertices).  Levels run coarse to fine,
+ * `iterations` iterations each.  Pairs (i, j) are the caller's, in its order (the result does not depend on it).
+ * 1. Visibility.  Each iteration starts with a z-buffer of the current mesh in every view at the level's size (the
+ *    renderer's camera, coverage rule and key, pm_raster.cuh).  Pixel q = (x, y) of view i is covered when the z-buffer
+ *    has a winner f.  r_q = R^T (x', y', 1), y' = (y - cy) / fy, x' = ((x - cx) - skew y') / fx, r_c = ((R0c x' + R1c y')
+ *    + R2c); n_f = (X1 - X0) x (X2 - X0) of f's float32 corners in float64, in its own order; the hit needs n_f . r_q < 0
+ *    and t_q = n_f . (X0 - C) / (n_f . r_q) > 0 finite; X_q = C + t_q r_q; beta_k = n_f . ((X_{k+1} - X) x (X_{k+2} - X))
+ *    / (n_f . n_f).  q is valid in pair (i, j) when it has a hit, n_f . (C_j - X0) > 0, neither view sees f at grazing
+ *    incidence (-(n_f . r_q) > 0.3 sqrt((n_f . n_f) (r_q . r_q)) and n_f . d > 0.3 sqrt((n_f . n_f) (d . d)), d = C_j - X_q:
+ *    the images alias the texture there), X_q projects (u' = ((P00 x + P01 y)
+ *    + P02 z) + P03, u = u' / z) into view j with z > near_j and 0 <= u <= W_j - 1, 0 <= v <= H_j - 1, and z <= (1 + 0.01)
+ *    z_j, z_j the float32 depth of j's z-buffer at (rint u, rint v) (an empty pixel fails).
+ * 2. Energy.  At every valid centre p of view i, the window of offsets -2..2 (clipped to the image) in row-major order
+ *    sums, over its valid pixels q, n, Sa, Sb, Saa, Sbb, Sab (a_q = G_i(q) float32, b_q = G_j(u, v) bilinear: x0 = floor u,
+ *    x1 = min(x0 + 1, W - 1), fx = u - x0, top = p + fx (q - p), bot = s + fx (t - s), b = top + fy (bot - top)).  It
+ *    counts when n >= 13 and both variances va = Saa/n - ma ma, vb = Sbb/n - mb mb exceed 1e-4; ZNCC Z = (Sab/n - ma mb)
+ *    / sqrt(va vb), E_p = 1 - Z.  E = sum over pairs and counted windows.
+ * 3. Gradient.  A counted window gives dE_p/db_q = (c1 a_q + c2 b_q) + c0 with c1 = -1/(n sigma), c2 = Z/(n vb),
+ *    c0 = ma/(n sigma) - (Z mb)/(n vb), sigma = sqrt(va vb).  Per valid q, c is summed (row-major) over the counted windows
+ *    around it; with none, q contributes nothing.  dE/dt_q = dE/db_q db/dt_q, db/dt = du (du/dt) + dv (dv/dt),
+ *    du = (q - p) + fy ((t - s) - (q - p)), dv = bot - top, du/dt = ((P0 . r) - u (P2 . r)) / z (likewise v).  Per corner
+ *    k of f, the vertex gets rint(((((g beta_k) / (n_f . r)) n_c) L) 2^20) (gradient, g = dE/dt), rint(beta_k 2^32)
+ *    (weight W) and rint((((beta_k t_q) / fx_i) / L) 2^32) (footprint S), int64, half to even.  L = the diagonal of the
+ *    input vertices' 1st-99th percentile box, sqrt((dx dx + dy dy) + dz dz).
+ * 4. Update.  Per vertex v: n_v = the sum over incident faces in face order of n_f, divided by its length (0 when 0); the
+ *    umbrella U(v) = (sum over distinct edge neighbours w, incident faces in face order and corners in slot order, of
+ *    (x_w - x_v)) / their count (0 without neighbours); U2(v) = the same sum of U(w) - U(v) over the count.  With W > 0:
+ *    w = W / 2^32, s = ((S / 2^32) L) / w, g = (n_v . (G / 2^20 / L)) / w, d = -clamp((alpha s) s g, -s/2, s/2); else
+ *    d = 0.  x_c <- float32((x_c + d n_c) - lambda U2_c).  Normals, umbrellas and the step all read the positions the
+ *    iteration started with.  Faces and their order never change.
+ *
+ * pmb200_refine_mesh_pyramid: grey_out [sum over levels of H_l W_l] float32 (device), level 0 first, from rgb float32
+ *   [3,H,W] (device).
+ * pmb200_refine_mesh: xyz float32 [nv,3] (device, refined in place), faces int32 [nf,3]; nv < 2^31, nf < 2^29; grey the
+ *   caller's pyramids (grey_floats floats); views_host (HOST) levels x n_views records, level-major, each level half the
+ *   previous, `offset` the view's level in grey; pairs_host (HOST) int32 [n_pairs,2] (i != j, both < n_views);
+ *   acc_out int64 [nv,5] (device) or NULL: the last iteration's sums (G xyz, W, S); stats_host (HOST) [levels *
+ *   iterations, 6] per iteration coarse to fine: energy, counted windows, reference pixels over the pairs, seconds of the
+ *   z-buffers, the pixel passes and the update.  Workspace of pmb200_refine_mesh_workspace_bytes bytes (level-0 views):
+ *   8 bytes per pixel of every view, 46 per pixel of the largest, about 112 per vertex and 52 per face.  One host read per
+ *   iteration.
+ * PMB200_EINVAL, nothing launched, for a null pointer, sizes out of range, a non-finite camera or fx, fy = 0, near_z <= 0, a
+ * level that is not half the previous, an image outside grey, a pair naming a view that does not exist (or i == j),
+ * levels outside 1..16, iterations < 0, a negative or non-finite alpha or smoothness, L <= 0, or a workspace smaller than
+ * the query. */
+typedef struct {
+    double P[12];      /* K [R | t] at the level, float64, row-major 3 x 4 */
+    double K[9];       /* the level's intrinsics, row-major */
+    double Rt[12];     /* [R | t], row-major 3 x 4 */
+    double near_z;     /* > 0 */
+    int64_t offset;    /* of the view's level in the grey buffer, floats */
+    int32_t width, height;
+} pmb200_refine_view;
+
+int pmb200_refine_mesh_pyramid(const float *rgb, int width, int height, int levels, float *grey_out, void *stream);
+int64_t pmb200_refine_mesh_workspace_bytes(int64_t n_vertices, int64_t n_faces, const pmb200_refine_view *views_host, int n_views);
+int pmb200_refine_mesh(float *xyz, int64_t n_vertices, const int *faces, int64_t n_faces, const float *grey, int64_t grey_floats,
+                       const pmb200_refine_view *views_host, int n_views, int levels, const int *pairs_host, int64_t n_pairs,
+                       int iterations, double alpha, double smoothness, double unit_length, int64_t *acc_out, double *stats_host,
+                       void *workspace, int64_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------
  * DTU point-cloud evaluation (reference evaluations/dtu/*.m; INTEGRATION.md "DTU evaluation"), float64 throughout.
  * Both calls sort the cloud into a fine / coarse cell hash held in a caller-owned device workspace of
  * *_workspace_bytes(n) bytes (O(n), whatever the extent of the cloud; the size query returns bytes or a negative PMB200_E*).

@@ -17,7 +17,7 @@ from typing import Optional
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 _REPO_DIR = os.path.dirname(_PKG_DIR)
 LIB_PATH = os.path.join(_PKG_DIR, "libpmb200.so")
-SOURCES = [os.path.join(_PKG_DIR, "csrc", f) for f in ("pm_kernels.cu", "pm_backward.cu", "pm_conv.cu", "pm_conv5.cu", "pm_stem.cu", "pm_refine.cu", "pm_geo.cu", "pm_cloud.cu", "pm_scan.cu", "pm_colmap.cu", "pm_undistort.cu", "pm_mesh.cu", "pm_poisson.cu", "pm_simplify.cu", "pm_sample.cu", "pm_render.cu", "pm_texture.cu", "pm_train.cu", "pm_mapio.cpp")]
+SOURCES = [os.path.join(_PKG_DIR, "csrc", f) for f in ("pm_kernels.cu", "pm_backward.cu", "pm_conv.cu", "pm_conv5.cu", "pm_stem.cu", "pm_refine.cu", "pm_geo.cu", "pm_cloud.cu", "pm_scan.cu", "pm_colmap.cu", "pm_undistort.cu", "pm_mesh.cu", "pm_poisson.cu", "pm_simplify.cu", "pm_sample.cu", "pm_render.cu", "pm_texture.cu", "pm_refine_mesh.cu", "pm_train.cu", "pm_mapio.cpp")]
 HEADERS = [
     os.path.join(_PKG_DIR, "csrc", "pm_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_warpcorr4.cuh"),
@@ -29,6 +29,7 @@ HEADERS = [
     os.path.join(_PKG_DIR, "csrc", "pm_camera_math.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_raster.cuh"),
     os.path.join(_PKG_DIR, "csrc", "pm_texture_math.cuh"),
+    os.path.join(_PKG_DIR, "csrc", "pm_refine_mesh_math.cuh"),
     os.path.join(_REPO_DIR, "include", "patchmatch_b200.h"),
 ]
 NVCC_FLAGS = [
@@ -125,6 +126,13 @@ class TextureView(ctypes.Structure):
     _fields_ = [("P", c_double * 12), ("centre", c_double * 3), ("near_z", c_double), ("width", c_int), ("height", c_int)]
 
 
+class RefineView(ctypes.Structure):
+    """pmb200_refine_view (include/patchmatch_b200.h): one view at one level of the mesh refinement."""
+
+    _fields_ = [("P", c_double * 12), ("K", c_double * 9), ("Rt", c_double * 12), ("near_z", c_double), ("offset", c_int64),
+                ("width", c_int), ("height", c_int)]
+
+
 class TsdfView(ctypes.Structure):
     """pmb200_tsdf_view (include/patchmatch_b200.h): one view of the TSDF integration."""
 
@@ -218,6 +226,10 @@ _SIGNATURES = {
     "pmb200_texture_write_workspace_bytes": (c_int64, [c_int]),
     "pmb200_texture_write": (c_int, [c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p,
                                      c_int64, c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_int] + [c_void_p] * 4 + [c_int64, c_void_p]),
+    "pmb200_refine_mesh_pyramid": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "pmb200_refine_mesh_workspace_bytes": (c_int64, [c_int64, c_int64, c_void_p, c_int]),
+    "pmb200_refine_mesh": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_int64,
+                                   c_int, c_double, c_double, c_double, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
     "pmb200_thin_points_workspace_bytes": (c_int64, [c_int64]),
     "pmb200_thin_points": (c_int, [c_void_p, c_void_p, c_int64, c_double, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
     "pmb200_nearest_distance_workspace_bytes": (c_int64, [c_int64]),

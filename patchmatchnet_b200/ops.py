@@ -2499,3 +2499,190 @@ def render_mesh_textured(xyz: Tensor, faces: Tensor, uv: Tensor, page: Tensor, p
                                              _stream(pts))
     _native.check(rc, what)
     return out_rgb, out_depth
+
+
+# ---- mesh refinement ------------------------------------------------------------------------------------------------------
+
+# defaults chosen on the refinement's convergence test (tests/test_gpu_refine_mesh.py): an icosphere with 2.7-pixel edges
+# displaced radially by up to 2 pixel footprints, 14 views of 160 x 120 with a 10-pixel-period albedo, 4 sources each
+REFINE_ITERATIONS = 8
+REFINE_LEVELS = 1
+REFINE_NEIGHBOURS = 4
+REFINE_ALPHA = 0.3
+REFINE_SMOOTHNESS = 0.4
+
+
+def refine_level_sizes(size, levels: int):
+    """[(H, W)] of levels 0 .. levels-1: each floor(half) of the previous."""
+    out = [tuple(int(s) for s in size)]
+    for _ in range(levels - 1):
+        out.append((out[-1][0] // 2, out[-1][1] // 2))
+    return out
+
+
+def refine_level_intrinsics(K, levels: int):
+    """[K_l] float64 [3,3]: fx, skew and fy halved, c' = (c + 0.5) / 2 - 0.5 per level."""
+    import numpy as np
+
+    out = [np.asarray(K.detach().cpu().numpy() if isinstance(K, Tensor) else K, np.float64).copy()]
+    for _ in range(levels - 1):
+        k = out[-1].copy()
+        k[0, 0] = k[0, 0] / 2.0
+        k[0, 1] = k[0, 1] / 2.0
+        k[1, 1] = k[1, 1] / 2.0
+        k[0, 2] = (k[0, 2] + 0.5) / 2.0 - 0.5
+        k[1, 2] = (k[1, 2] + 0.5) / 2.0 - 0.5
+        out.append(k)
+    return out
+
+
+def refine_view_table(Ks, Es, sizes, levels: int, box_centre):
+    """ctypes array of levels x n_views pmb200_refine_view, level-major: P = K_l [R | t] (float64), K_l, [R | t], the
+    texturer's near plane (texture_view_table at level 0) and each view's level offset in the packed grey pyramids
+    (views in order, each view's levels in order).  -> (table, total grey floats)."""
+    import numpy as np
+
+    V = len(sizes)
+    base = texture_view_table(Ks, Es, sizes, box_centre)
+    table = (_native.RefineView * (levels * V))()
+    offset = 0
+    for v in range(V):
+        E = np.asarray(Es[v].detach().cpu().numpy() if isinstance(Es[v], Tensor) else Es[v], np.float64)
+        Rt = E[:3, :4]
+        for l, (Kl, (h, w)) in enumerate(zip(refine_level_intrinsics(Ks[v], levels), refine_level_sizes(sizes[v], levels))):
+            r = table[l * V + v]
+            r.P[:] = (Kl @ Rt).ravel().tolist()
+            r.K[:] = Kl.ravel().tolist()
+            r.Rt[:] = Rt.ravel().tolist()
+            r.near_z = base[v].near_z
+            r.offset = offset
+            r.height, r.width = h, w
+            offset += h * w
+    return table, offset
+
+
+def mesh_box_diagonal(xyz: Tensor) -> float:
+    """L, the refinement's length unit: the diagonal of the per-axis 1st-99th percentile box of the vertices,
+    sqrt((dx dx + dy dy) + dz dz) in float64 (1 when it is 0)."""
+    import numpy as np
+
+    n = xyz.shape[0]
+    if n == 0:
+        return 1.0
+    k = int(0.01 * (n - 1))
+    s = torch.sort(xyz, dim=0).values
+    d = s[n - 1 - k].double().cpu().numpy() - s[k].double().cpu().numpy()
+    L = float(np.sqrt((d[0] * d[0] + d[1] * d[1]) + d[2] * d[2]))
+    return L if L > 0 else 1.0
+
+
+def refine_mesh_bytes(n_vertices: int, n_faces: int, sizes, levels: int = REFINE_LEVELS) -> int:
+    """Estimate of the device memory ops.refine_mesh needs beyond its inputs: the workspace of pmb200_refine_mesh (8 bytes per
+    pixel of every view, 46 per pixel of the largest, about 112 per vertex and 52 per face), the grey pyramids (4 bytes per
+    pixel of every level), the refined positions and the per-vertex sums (52 bytes per vertex).  `sizes` the views' (H, W).
+    Needs a CUDA device."""
+    eye = [[[1, 0, 0], [0, 1, 0], [0, 0, 1]]] * len(sizes)
+    table, grey = refine_view_table(eye, [[[1, 0, 0, 0], [0, 1, 0, 0], [0, 0, 1, 0], [0, 0, 0, 1]]] * len(sizes), sizes, 1,
+                                    [0.0, 0.0, -1.0])
+    ws = _native.lib().pmb200_refine_mesh_workspace_bytes(n_vertices, n_faces, _addr(table), len(sizes))
+    if ws < 0:
+        _native.check(int(ws), "refine_mesh_workspace_bytes")
+    return int(ws) + refine_mesh_extra_bytes(n_vertices, sizes, levels)
+
+
+def refine_mesh_extra_bytes(n_vertices: int, sizes, levels: int) -> int:
+    """The part of refine_mesh_bytes outside the native workspace: the grey pyramids (4 bytes per pixel of every level of
+    every view) and 52 bytes per vertex (the refined positions and the int64 sums)."""
+    return 4 * sum(h * w for s in sizes for h, w in refine_level_sizes(s, levels)) + 52 * n_vertices
+
+
+def refine_mesh(xyz: Tensor, faces: Tensor, images: Sequence[Tensor], Ks, Es, pairs, iterations: int = REFINE_ITERATIONS,
+                levels: int = REFINE_LEVELS, smoothness: float = REFINE_SMOOTHNESS, alpha: float = REFINE_ALPHA,
+                with_sums: bool = False):
+    """Refine a triangle mesh's vertices by multi-view photo-consistency: windowed ZNCC between each reference view and its
+    sources reprojected through the mesh, gradient steps along the vertex normals and thin-plate smoothing, coarse to fine
+    over `levels` image levels, `iterations` each (definition in include/patchmatch_b200.h).  xyz CUDA float32 [nv,3];
+    faces int32 [nf,3]; per view the image float32 [3,H,W] in [0,1] (views may differ in size), K [3,3] scaled to that size
+    and E [4,4] world -> camera; pairs [(i, j)] ordered (reference, source) view indices.
+    -> (xyz_refined float32 [nv,3] on the device, stats dict: energy and windows per iteration coarse to fine, the seconds of
+    the call and of its z-buffer, pixel and update stages, pixel_pairs; with with_sums also `sums` int64 [nv,5], the last
+    iteration's fixed-point gradient, weight and footprint sums).  The inputs are not modified; reruns give the same bits.
+
+    ValueError before any launch on bad arguments (a face index outside 0..nv-1 included), and before allocating when
+    refine_mesh_bytes exceeds the device's free memory.  Host reads: one per iteration."""
+    import ctypes
+    import time
+
+    import numpy as np
+
+    what = "refine_mesh"
+    t0 = time.perf_counter()
+    pts = _render_xyz(xyz, what)
+    nv = pts.shape[0]
+    if not isinstance(faces, Tensor) or not _on_device(faces) or faces.dtype != torch.int32 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError(f"{what}: faces must be a CUDA int32 [nf,3] tensor")
+    if faces.device != pts.device:
+        raise ValueError(f"{what}: faces must be on the vertices' device")
+    fc = faces.contiguous()
+    nf = fc.shape[0]
+    if nv >= 2 ** 31 or nf >= 2 ** 29:
+        raise ValueError(f"{what}: at most 2^31 - 1 vertices and 2^29 - 1 faces, got {nv} and {nf}")
+    sizes = _texture_images(images, pts, what)
+    V = len(images)
+    if len(Ks) != V or len(Es) != V:
+        raise ValueError(f"{what}: one K and one E per image, got {len(Ks)} and {len(Es)} for {V} images")
+    if V > 65535:
+        raise ValueError(f"{what}: at most 65535 views")
+    if not isinstance(levels, int) or not 1 <= levels <= 16 or any(min(s) >> (levels - 1) < 1 for s in sizes):
+        raise ValueError(f"{what}: levels must be 1..16 and every view at least 2^(levels-1) pixels a side, got {levels}")
+    if not isinstance(iterations, int) or iterations < 0:
+        raise ValueError(f"{what}: iterations must be an int >= 0, got {iterations}")
+    for name, val in (("smoothness", smoothness), ("alpha", alpha)):
+        if not (0.0 <= float(val) < float("inf")):
+            raise ValueError(f"{what}: {name} must be finite and >= 0, got {val}")
+    pr = np.ascontiguousarray(np.asarray(pairs, np.int64).reshape(-1, 2))
+    if pr.size and (pr.min() < 0 or pr.max() >= V or (pr[:, 0] == pr[:, 1]).any()):
+        raise ValueError(f"{what}: every pair (i, j) needs two different views in 0..{V - 1}")
+    if iterations > 0 and len(pr) == 0:
+        raise ValueError(f"{what}: no (reference, source) pair: the iterations would smooth the mesh without a photometric term")
+    pr = pr.astype(np.int32)
+    if nf:
+        lo, hi = (int(v) for v in torch.aminmax(fc))
+        if lo < 0 or hi >= nv:
+            raise ValueError(f"{what}: a face refers to a vertex outside 0..{nv - 1}")
+    table, grey_floats = refine_view_table(Ks, Es, sizes, levels, mesh_box_centre(pts))
+    L = mesh_box_diagonal(pts)
+    dev = pts.device
+    lib = _native.lib()
+    ws_bytes = lib.pmb200_refine_mesh_workspace_bytes(nv, nf, _addr(table), V)
+    if ws_bytes < 0:
+        _native.check(int(ws_bytes), "refine_mesh_workspace_bytes")
+    need = refine_mesh_bytes(nv, nf, sizes, levels)
+    free = _free_bytes(dev)
+    if need > free:
+        raise ValueError(f"{what}: {nv} vertices, {nf} faces and {V} views need {need / 2 ** 30:.2f} GiB ({free / 2 ** 30:.2f} GiB free)")
+    grey = torch.empty(max(grey_floats, 1), dtype=torch.float32, device=dev)
+    with _device_guard(pts):
+        for v in range(V):
+            img = images[v].contiguous()
+            rc = lib.pmb200_refine_mesh_pyramid(img.data_ptr(), sizes[v][1], sizes[v][0], levels, grey.data_ptr() + 4 * table[v].offset,
+                                                _stream(pts))
+            _native.check(rc, what + "_pyramid")
+    out = pts.clone()
+    sums = torch.zeros((nv, 5), dtype=torch.int64, device=dev) if with_sums else None
+    ws = _workspace(ws_bytes, "refine_mesh_workspace_bytes", dev)
+    rows = levels * iterations
+    st = (ctypes.c_double * max(6 * rows, 1))()
+    with _device_guard(pts):
+        rc = lib.pmb200_refine_mesh(out.data_ptr(), nv, fc.data_ptr(), nf, grey.data_ptr(), grey_floats, _addr(table), V, levels,
+                                    pr.ctypes.data, len(pr), iterations, float(alpha), float(smoothness), L,
+                                    None if sums is None else sums.data_ptr(), st, ws.data_ptr(), int(ws_bytes), _stream(pts))
+    _native.check(rc, what)
+    torch.cuda.synchronize(dev)
+    s = np.array(st[:6 * rows]).reshape(rows, 6)
+    stats = {"energy": s[:, 0].tolist(), "windows": [int(n) for n in s[:, 1]], "pixel_pairs": int(s[:, 2].sum()),
+             "zbuffer_seconds": float(s[:, 3].sum()), "pixel_seconds": float(s[:, 4].sum()), "update_seconds": float(s[:, 5].sum()),
+             "iterations": rows, "seconds": time.perf_counter() - t0}
+    if sums is not None:
+        stats["sums"] = sums
+    return out, stats

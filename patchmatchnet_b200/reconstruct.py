@@ -54,6 +54,8 @@ independent collapses) to at most N faces and written to <scan>/mesh_simplified.
 drops connected pieces of fewer than F faces.  mesh.ply is the same with or without these options.
 With --mesh-texture the simplified mesh (the mesh without --mesh-target-faces) is also textured from the scan's reference
 views (ops.texture_mesh) and written as <scan>/mesh_textured.obj, .mtl and mesh_textured_NN.png.
+With --mesh-refine that mesh is first refined by photo-consistency (ops.refine_mesh) against the reference views and their
+pair.txt sources and written to <scan>/mesh_refined.ply; with --mesh-texture the refined mesh is the one textured.
 With --poisson (needs --normals and the fusion stage; off by default, it changes no other output) the oriented fused
 points are also meshed on the GPU by Poisson surface reconstruction (ops.poisson_mesh: a multigrid solve on a
 (2^depth + 1)^3 grid, marching cubes trimmed to 2 voxels around the points) and written to <scan>/mesh_poisson.ply, the same
@@ -138,6 +140,9 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--mesh-texture", action="store_true", default=argparse.SUPPRESS,
                     help="with --mesh, also write mesh_textured.obj (.mtl, _NN.png): the simplified mesh (or the mesh) textured "
                          "from the reference views, on the GPU")
+    ap.add_argument("--mesh-refine", action="store_true", default=argparse.SUPPRESS,
+                    help="with --mesh, also write mesh_refined.ply: the simplified mesh (or the mesh) refined by photo-consistency "
+                         "against the reference views and their pair.txt sources, on the GPU; --mesh-texture then textures it")
     ap.add_argument("--poisson", action="store_true", default=argparse.SUPPRESS,
                     help="with --normals, also write mesh_poisson.ply: Poisson surface reconstruction of the oriented fused "
                          "points, on the GPU")
@@ -155,12 +160,12 @@ def poisson_options(args: argparse.Namespace) -> argparse.Namespace:
 
 
 MESH_DEFAULTS = {"mesh": False, "mesh_voxel_size": None, "mesh_trunc": 3, "mesh_min_weight": 1, "mesh_target_faces": None,
-                 "mesh_min_component_faces": None, "mesh_texture": False}
+                 "mesh_min_component_faces": None, "mesh_texture": False, "mesh_refine": False}
 
 
 def mesh_options(args: argparse.Namespace) -> argparse.Namespace:
-    """--mesh, --mesh-voxel-size, --mesh-trunc, --mesh-min-weight, --mesh-target-faces, --mesh-min-component-faces and
-    --mesh-texture of `args`, with their defaults where not given."""
+    """--mesh, --mesh-voxel-size, --mesh-trunc, --mesh-min-weight, --mesh-target-faces, --mesh-min-component-faces,
+    --mesh-texture and --mesh-refine of `args`, with their defaults where not given."""
     return argparse.Namespace(**{k: getattr(args, k, v) for k, v in MESH_DEFAULTS.items()})
 
 
@@ -191,6 +196,8 @@ def check_args(args: argparse.Namespace) -> List[str]:
         raise ValueError(f"--mesh-min-component-faces needs --mesh-target-faces and a value >= 0, got {m.mesh_min_component_faces}")
     if m.mesh_texture and not m.mesh:
         raise ValueError("--mesh-texture needs --mesh")
+    if m.mesh_refine and not m.mesh:
+        raise ValueError("--mesh-refine needs --mesh")
     if m.mesh:
         if m.mesh_voxel_size is not None and not (0 < m.mesh_voxel_size < float("inf")):
             raise ValueError(f"--mesh-voxel-size must be positive and finite, got {m.mesh_voxel_size}")
@@ -211,6 +218,15 @@ def check_args(args: argparse.Namespace) -> List[str]:
         if not 5 <= p.poisson_depth <= 10:
             raise ValueError(f"--poisson-depth must be 5..10, got {p.poisson_depth}")
     scans = list_scans(args.scan_list)
+    if m.mesh_refine:
+        from .refine import pairs_among
+
+        for scan in scans:
+            pair_file = os.path.join(args.input_folder, scan, "pair.txt")
+            entries = data_io.read_pair_file(pair_file) if os.path.isfile(pair_file) else []
+            if not pairs_among(entries, [ref for ref, _ in entries], ops.REFINE_NEIGHBOURS):
+                raise ValueError(f"--mesh-refine: no reference view of {pair_file!r} has a source among the reference views, so "
+                                 "there is no pair to refine against")
     if not args.output_folder:
         args.output_folder = args.input_folder
     return scans
@@ -427,8 +443,9 @@ def default_mesh_voxel_size(depths: Sequence[Tensor], Ks: Sequence[np.ndarray]) 
 
 
 def mesh_scan(args: argparse.Namespace, bank: SceneBank, refs: Sequence[int], depths: Sequence[Tensor], bodies: Sequence[Tensor],
-              path: str) -> Dict[str, float]:
-    """mesh.ply of one scan from the kept final-masked depths, the fused points as seeds and the image bank."""
+              path: str, pairs: Optional[Sequence[Tuple[int, List[int]]]] = None) -> Dict[str, float]:
+    """mesh.ply of one scan from the kept final-masked depths, the fused points as seeds and the image bank; `pairs` (the
+    scan's pair.txt) gives --mesh-refine its source views."""
     t0 = time.perf_counter()
     m = mesh_options(args)
     Ks = [bank.intrinsics[r] for r in refs]
@@ -446,10 +463,23 @@ def mesh_scan(args: argparse.Namespace, bank: SceneBank, refs: Sequence[int], de
         data_io.save_ply(os.path.join(os.path.dirname(path), "mesh_simplified.ply"), body, sfaces)
         out.update({"simplified_vertices": int(body.shape[0]), "simplified_faces": int(sfaces.shape[0]), "simplify_rounds": rounds,
                     "simplify_seconds": time.perf_counter() - t0})
+    tb, tf = (body, sfaces) if m.mesh_target_faces is not None else (verts, faces)
+    if m.mesh_refine:
+        from .refine import refine_and_save
+
+        t0 = time.perf_counter()
+        from .refine import pairs_among
+
+        rpairs = pairs_among(pairs or [], refs, ops.REFINE_NEIGHBOURS)
+        rgb = tb[:, 12:15].contiguous() if tb.shape[1] >= 15 else None
+        rxyz, st = refine_and_save(tb[:, :12].contiguous().view(torch.float32), rgb, tf, [bank.images[r] for r in refs], Ks,
+                                   [bank.extrinsics[r] for r in refs], rpairs, os.path.join(os.path.dirname(path), "mesh_refined.ply"))
+        tb = torch.cat([rxyz.contiguous().view(torch.uint8), tb[:, 12:]], 1)
+        out.update({"refine_energy_first": st["energy"][0] if st["energy"] else 0.0,
+                    "refine_energy_last": st["energy"][-1] if st["energy"] else 0.0, "refine_seconds": time.perf_counter() - t0})
     if m.mesh_texture:
         from .texture import texture_and_save
 
-        tb, tf = (body, sfaces) if m.mesh_target_faces is not None else (verts, faces)
         xyz = tb[:, :12].contiguous().view(torch.float32)
         rgb = tb[:, 12:15].contiguous() if tb.shape[1] >= 15 else None
         st = texture_and_save(xyz, rgb, tf, [bank.images[r] for r in refs], Ks, [bank.extrinsics[r] for r in refs],
@@ -508,7 +538,7 @@ def fuse_scan(args: argparse.Namespace, scan: str, bank: SceneBank, pairs: Seque
         log("saving the Poisson mesh to", path, "({} vertices, {} faces)".format(st["vertices"], st["faces"]))
     if mesh_options(args).mesh:
         path = os.path.join(out_dir, "mesh.ply")
-        mesh.update(mesh_scan(args, bank, [ref for ref, _ in pairs], mesh_depths, bodies, path))
+        mesh.update(mesh_scan(args, bank, [ref for ref, _ in pairs], mesh_depths, bodies, path, pairs))
         log("saving the mesh to", path, "({} vertices, {} faces)".format(mesh["mesh_vertices"], mesh["mesh_faces"]))
     return sum(int(b.shape[0]) for b in bodies), mesh
 
@@ -534,6 +564,8 @@ def reconstruct(args: argparse.Namespace, *, device: str = "cuda:0", n_slots: in
         stats.update({"simplified_vertices": 0, "simplified_faces": 0, "simplify_rounds": 0, "simplify_seconds": 0.0})
     if mesh_options(args).mesh_texture:
         stats.update(dict.fromkeys(TEXTURE_STATS, 0))
+    if mesh_options(args).mesh_refine:
+        stats.update({"refine_energy_first": 0.0, "refine_energy_last": 0.0, "refine_seconds": 0.0})
     if poisson_options(args).poisson:
         stats.update({"poisson_vertices": 0, "poisson_faces": 0, "poisson_seconds": 0.0, "poisson_cycles": 0})
     t_start = time.perf_counter()
